@@ -28,6 +28,10 @@ def build(force: bool = False) -> str:
 
 _lib = None
 
+# the branch counters of or_coverage, in the order of OR_COV_* in swirld_oracle.c
+COVERAGE = ("coin_votes", "coin_ones", "coin_super", "decide_after_c", "decisions", "majority_empty",
+            "median_odd", "median_even", "single_seer", "tied")
+
 
 def lib():
     global _lib
@@ -53,6 +57,7 @@ def lib():
         L.or_get_witness.argtypes = [C.c_void_p, _u8p]
         L.or_get_witness_table.argtypes = [C.c_void_p, _i32p]
         L.or_get_consensus.argtypes = [C.c_void_p, _i32p, C.c_int]
+        L.or_coverage.argtypes = [C.c_void_p, _i64p]
         _lib = L
     return _lib
 
@@ -138,6 +143,12 @@ class Oracle:
         lib().or_get_can_see(self._h, first, n, out)
         return out
 
+    def coverage(self):
+        """How often this view took each rarely taken branch so far: {name in COVERAGE: count}."""
+        out = np.zeros(len(COVERAGE), np.int64)
+        assert lib().or_coverage(self._h, out) == len(COVERAGE)
+        return dict(zip(COVERAGE, out.tolist()))
+
 
 def run_oracle(tr, K, stake=None, coin_period=6, timing=None):
     """Feed a trace in chunks of K (the schedule) and return results()."""
@@ -162,5 +173,6 @@ def run_oracle(tr, K, stake=None, coin_period=6, timing=None):
     res["t_divide_rounds"] = t_dr
     res["t_decide_fame"] = t_df
     res["t_find_order"] = t_fo
+    res["coverage"] = o.coverage()
     res["oracle"] = o
     return res

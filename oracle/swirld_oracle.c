@@ -29,6 +29,23 @@
 #define OR_ERR_ARG     (-1)
 #define OR_ERR_KEY     (-3)  /* votes[w][x] KeyError, swirld.py:260 */
 
+/* Branch counters (or_coverage): how often a run took each rarely taken branch,
+ * so that a test can assert that its trace reaches the branch it is meant to
+ * test.  Counting never changes a result. */
+enum {
+    OR_COV_COIN_VOTES,       /* :272 votes cast by the coin */
+    OR_COV_COIN_ONES,        /* ... of which the coin said 1 */
+    OR_COV_COIN_SUPER,       /* :268-269 supermajority vote in a coin round */
+    OR_COV_DECIDE_AFTER_C,   /* :262-264 decisions at r_ - r > C */
+    OR_COV_DECISIONS,        /* :262-264 all decisions */
+    OR_COV_MAJORITY_EMPTY,   /* :260 majority() over an empty s */
+    OR_COV_MEDIAN_ODD,       /* :305 median over an odd number of times (the two middle-and-above entries) */
+    OR_COV_MEDIAN_EVEN,      /* :305 median over an even number of times (one entry, twice) */
+    OR_COV_SINGLE_SEER,      /* :305 IndexError: one time only */
+    OR_COV_TIED,             /* :306 adjacent events of a round's final with equal consensus time */
+    OR_NCOV
+};
+
 typedef struct {
     uint64_t *keys;   /* (y << 32 | x) + 1, 0 = empty */
     uint8_t  *vals;
@@ -64,6 +81,7 @@ typedef struct {
     int64_t *hits;
     int32_t *queue;
     uint8_t *mark;
+    int64_t cov[OR_NCOV];         /* branch counters, see OR_COV_* */
 } oracle;
 
 /* ---------------------------------------------------------------- votes */
@@ -304,6 +322,7 @@ int or_decide_fame(void *hd, int32_t *new_c_out, int cap) {
                         vm_put(&o->votes, (uint32_t)y, (uint32_t)x, in);
                     } else {
                         int64_t hv[2] = {0, 0};               /* majority :20-27 */
+                        if (ns == 0) o->cov[OR_COV_MAJORITY_EMPTY]++;
                         for (int i = 0; i < ns; i++) {
                             int v = vm_get(&o->votes, (uint32_t)s[i], (uint32_t)x);
                             if (v < 0) { free(done); free(s); return OR_ERR_KEY; }
@@ -315,14 +334,20 @@ int or_decide_fame(void *hd, int32_t *new_c_out, int cap) {
                             if ((double)tt > o->min_s) {      /* :261-263 */
                                 o->famous[x] = (int8_t)v;
                                 done[r] = 1;
+                                o->cov[OR_COV_DECISIONS]++;
+                                if (r_ - r > o->C) o->cov[OR_COV_DECIDE_AFTER_C]++;
                             } else
                                 vm_put(&o->votes, (uint32_t)y, (uint32_t)x, v);
                         } else {
-                            if ((double)tt > o->min_s)        /* :267-268 */
+                            if ((double)tt > o->min_s) {      /* :267-268 */
                                 vm_put(&o->votes, (uint32_t)y, (uint32_t)x, v);
-                            else                              /* :270-272 coin */
-                                vm_put(&o->votes, (uint32_t)y, (uint32_t)x,
-                                       o->sig[(size_t)64 * y] / 128 ? 1 : 0);
+                                o->cov[OR_COV_COIN_SUPER]++;
+                            } else {                          /* :270-272 coin */
+                                int coin = o->sig[(size_t)64 * y] / 128 ? 1 : 0;
+                                vm_put(&o->votes, (uint32_t)y, (uint32_t)x, coin);
+                                o->cov[OR_COV_COIN_VOTES]++;
+                                o->cov[OR_COV_COIN_ONES] += coin;
+                            }
                         }
                     }
                 }
@@ -416,8 +441,9 @@ int or_find_order(void *hd, const int32_t *new_c, int n) {
                     times[i] = o->t[a];
                 }
                 qsort(times, ns, sizeof(double), cmp_dbl);     /* :304 */
-                if ((ns + 1) / 2 >= ns) { rc = OR_ERR_INDEX; }  /* :305 IndexError */
+                if ((ns + 1) / 2 >= ns) { rc = OR_ERR_INDEX; o->cov[OR_COV_SINGLE_SEER]++; }  /* :305 IndexError */
                 else {
+                    o->cov[ns % 2 ? OR_COV_MEDIAN_ODD : OR_COV_MEDIAN_EVEN]++;
                     if (nk == kcap) { kcap = kcap ? kcap * 2 : 256; keys = (okey *)realloc(keys, sizeof(okey) * kcap); }
                     keys[nk].ts = .5 * (times[ns / 2] + times[(ns + 1) / 2]);
                     for (int b = 0; b < 64; b++) keys[nk].key[b] = white[b] ^ o->sig[(size_t)64 * x + b];
@@ -436,6 +462,8 @@ int or_find_order(void *hd, const int32_t *new_c, int n) {
         for (int i = 0; i < qt; i++) o->mark[o->queue[i]] = 0;
         if (rc == 0) {
             qsort(keys, nk, sizeof(okey), cmp_okey);           /* :306 */
+            for (int i = 1; i < nk; i++)
+                if (keys[i].ts == keys[i - 1].ts) o->cov[OR_COV_TIED]++;
             for (int i = 0; i < nk; i++) {                     /* :307-309 */
                 o->idx[keys[i].x] = i + o->n_tx;
             }
@@ -452,6 +480,8 @@ int or_find_order(void *hd, const int32_t *new_c, int n) {
 int or_n_events(void *h) { return ((oracle *)h)->n; }
 int or_max_round(void *h) { return ((oracle *)h)->max_r; }
 int or_n_transactions(void *h) { return ((oracle *)h)->n_tx; }
+/* copies the OR_NCOV branch counters to out; returns OR_NCOV */
+int or_coverage(void *h, int64_t *out) { oracle *o = (oracle *)h; memcpy(out, o->cov, sizeof o->cov); return OR_NCOV; }
 
 void or_get_round(void *h, int32_t *out) { oracle *o = (oracle *)h; memcpy(out, o->round, sizeof(int32_t) * o->n); }
 void or_get_famous(void *h, int8_t *out) { oracle *o = (oracle *)h; memcpy(out, o->famous, o->n); }

@@ -269,7 +269,16 @@ def test_find_order_with_already_ordered_famous_witness(seed, impl):
 @pytest.mark.parametrize("gen,M,N,K,seed,stake", [
     ("gossip", 65, 9000, 777, 61, None), ("gossip", 100, 16000, 4000, 62, None), ("adversarial", 130, 30000, 8192, 63, None),
     ("tick", 200, 24000, 5000, 64, None), ("gossip", 256, 40000, 16384, 65, None), ("gossip", 300, 36000, 36000, 66, None),
-    ("gossip", 72, 9000, 500, 67, "mixed"), ("adversarial", 96, 12000, 1, 68, None)])
+    ("gossip", 72, 9000, 500, 67, "mixed"), ("adversarial", 96, 12000, 1, 68, None),
+    # one member past a mask width (NJ = 4, 8, 16, 32): the last 32-bit word of every member mask holds one live bit
+    pytest.param("gossip", 97, 12000, 1000, 91, None, id="boundary-97"),
+    pytest.param("gossip", 97, 12000, 1000, 91, "mixed", id="boundary-97-mixed"),
+    pytest.param("gossip", 129, 16000, 3000, 92, None, id="boundary-129"),
+    pytest.param("gossip", 129, 16000, 3000, 92, "mixed", id="boundary-129-mixed"),
+    pytest.param("gossip", 257, 30000, 7000, 93, None, id="boundary-257"),
+    pytest.param("gossip", 257, 30000, 7000, 93, "mixed", id="boundary-257-mixed"),
+    pytest.param("gossip", 513, 40000, 10000, 94, None, id="boundary-513"),
+    pytest.param("gossip", 513, 40000, 10000, 94, "mixed", id="boundary-513-mixed")])
 def test_wide_engine_matches_oracle(gen, M, N, K, seed, stake):
     from swirld_b200 import traces
     tr = getattr(traces, gen)(M, N, seed)

@@ -49,11 +49,15 @@ def test_oracle_matches_live_reference(M, N, K, seed):
 
 def test_oracle_index_error_single_seer():
     """swirld.py:305 raises IndexError when only one famous witness sees an
-    event; the oracle reports it instead of inventing a timestamp."""
+    event; the oracle reports it instead of inventing a timestamp.  Member 0
+    holds all the stake, so its witness alone decides "received"."""
     from swirld_b200 import traces
-    tr = traces.gossip(3, 400, 3)
-    try:
-        orc.run_oracle(tr, 50, stake=[5, 1, 1])
-    except IndexError:
-        return
-    # not every trace reaches that state; it must at least run clean
+    tr = traces.gossip(4, 1000, 1)
+    o = orc.Oracle(4, [1, 0, 0, 0])
+    o.append(tr)
+    o.divide_rounds(0, 20)
+    nc = o.decide_fame()
+    assert nc
+    with pytest.raises(IndexError):
+        o.find_order(nc)
+    assert o.coverage()["single_seer"] == 1
