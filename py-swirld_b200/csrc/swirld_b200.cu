@@ -30,7 +30,7 @@ std::string g_create_error;
 using Id32 = std::array<uint64_t, 4>;
 struct Id32Hash { size_t operator()(const Id32 &k) const { return (size_t)(k[0] ^ (k[1] * 0x9E3779B97F4A7C15ull)); } };
 
-struct TimedSpan { cudaEvent_t a, b; int cat; };
+struct TimedSpan { cudaEvent_t a, b; int cat; bool shared_a = false; };   // shared_a: `a` is another span's start too
 
 }  // namespace
 
@@ -47,6 +47,11 @@ struct sw_engine {
     std::vector<int32_t> h_creator, h_head, h_count;
     int32_t *h_height = nullptr, *h_seq = nullptr;   // pinned, cap entries: sources of asynchronous copies
     uint8_t *h_stale = nullptr;                      // pinned: the other-parent is not its member's latest event
+    // M <= 64: h_count as it stood after every SNAP-th event and at the end of every append, so that the per-member
+    // counts of any chunk cost O(M) plus fewer than SNAP events (round_batch_prep)
+    static constexpr int SNAP = 4096;
+    std::vector<int> snap_at;                        // event counts of the snapshots, ascending
+    std::vector<int32_t> snap_cnt;                   // [snapshot][M]
     cudaStream_t copy_stream = nullptr;              // sw_append's copies run beside the kernels of earlier chunks
     struct PendingAppend { int base; cudaEvent_t done; };
     std::vector<PendingAppend> appends;              // copies (+ eager can_see scans) the compute stream has not waited for yet
@@ -120,7 +125,7 @@ struct sw_engine {
     int stage_next = 0;
     int stream_n = 16;            // divide_rounds calls of at most this many events take the one-launch path (SW_STREAM_N)
     int32_t *h_scal = nullptr;    // pinned
-    int32_t *h_newc = nullptr;    // pinned, Rcap
+    int32_t *h_newc = nullptr;    // pinned, Rcap: right behind h_scal (one copy brings both back)
     cudaStream_t stream = nullptr;
     cudaEvent_t user_ev[16] = {nullptr};
     std::vector<TimedSpan> spans;
@@ -183,7 +188,8 @@ void fold_spans(sw_engine *e) {
             else if (s.cat == 3) { e->stats.ms_can_see += ms; e->stats.ms_divide_rounds += ms; }
             else if (s.cat == 4) e->stats.ms_rounds_kernel += ms;
         }
-        e->pool.push_back(s.a); e->pool.push_back(s.b);
+        if (!s.shared_a) e->pool.push_back(s.a);
+        e->pool.push_back(s.b);
     }
     e->spans.swap(pending);
 }
@@ -243,6 +249,7 @@ int reset_state(sw_engine *e, bool keep_events = false) {
         e->n_events = 0;
         std::fill(e->h_head.begin(), e->h_head.end(), -1);
         std::fill(e->h_count.begin(), e->h_count.end(), 0);
+        e->snap_at.clear(); e->snap_cnt.clear();
     }
     memset(e->h_scal, 0, sizeof(int32_t) * SC_COUNT);
     return 0;
@@ -360,9 +367,29 @@ int cansee_scan(sw_engine *e, cudaStream_t st, int upto) {
     return 0;
 }
 
-// rounds of the chunk by the cooperative round-batch kernel (swirld_rounds.cuh), M <= 64: parameters + the kernels
-// that group the chunk's events by creator (`grid` = CTAs this view's round kernel will run on)
-int round_batch_prep(sw_engine *e, int first, int n, int grid, RbParams &R, int min_L = 1) {
+void push_snapshot(sw_engine *e, int at, const std::vector<int32_t> &cnt) {
+    e->snap_at.push_back(at);
+    e->snap_cnt.insert(e->snap_cnt.end(), cnt.begin(), cnt.end());
+}
+
+// events of each member among the first x appended events: the nearest snapshot at or below x, then the rest one by one
+void counts_at(const sw_engine *e, int x, int32_t *out) {
+    const int M = e->M;
+    const auto it = std::upper_bound(e->snap_at.begin(), e->snap_at.end(), x);
+    int from = 0;
+    if (it == e->snap_at.begin()) std::fill(out, out + M, 0);
+    else {
+        const size_t k = (size_t)(it - e->snap_at.begin()) - 1;
+        from = e->snap_at[k];
+        std::copy_n(e->snap_cnt.begin() + k * M, M, out);
+    }
+    for (int i = from; i < x; i++) out[e->h_creator[i]]++;
+}
+
+// rounds of the chunk by the cooperative round-batch kernel (swirld_rounds.cuh), M <= 64: parameters + the kernel that
+// groups the chunk's events by creator and, for the cluster round kernel (`rows`), writes their seq-space rows
+// (`grid` = CTAs this view's round kernel will run on)
+int round_batch_prep(sw_engine *e, int first, int n, int grid, bool rows, RbParams &R, int min_L = 1) {
     R = RbParams{};
     R.M = e->M; R.first = first; R.n = n; R.Rcap = e->Rcap;
     R.L = std::max(std::min(min_L, RB_LMAX), std::min(RB_LMAX, grid * (RB_THREADS / 32) / e->M));
@@ -377,13 +404,27 @@ int round_batch_prep(sw_engine *e, int first, int n, int grid, RbParams &R, int 
     R.res = e->d_res; R.stake = e->d_stake; R.tot2 = 2 * e->tot; R.scal = e->d_scal;
     R.wit = e->d_wit; R.W = e->d_W; R.SM = e->d_SM; R.dbg = e->d_dbg;
     R.wlist = e->d_cev + e->cap; R.wcnt = e->d_rbmeta + 225;
-    CK(cudaMemsetAsync(R.ccnt, 0, sizeof(int32_t) * 64, e->stream));
-    CK(cudaMemsetAsync(R.cmin, 0x7f, sizeof(int32_t) * 64, e->stream));
-    const int blocks = std::max(1, std::min(296, (n + 255) / 256));
-    k_rb_count<<<blocks, 256, 0, e->stream>>>(R);
-    k_rb_offsets<<<1, 32, 0, e->stream>>>(R);
-    k_rb_scatter<<<blocks, 256, 0, e->stream>>>(R);
+    // the chunk's per-member counts from the host mirror: [first, first+n) holds seqs [lo[c], hi[c]) of member c
+    RbChunk K;
+    int32_t lo[64], hi[64];
+    counts_at(e, first, lo);
+    counts_at(e, first + n, hi);
+    int o = 0;
+    for (int c = 0; c < 64; c++) {
+        const int cnt = c < e->M ? hi[c] - lo[c] : 0;
+        K.ccnt[c] = cnt; K.cmin[c] = cnt > 0 ? lo[c] : 0x7f7f7f7f; K.ctot[c] = c < e->M ? hi[c] : 0;
+        K.coff[c] = o; o += cnt;
+    }
+    K.coff[64] = o;
+    if (rows && (size_t)n > e->rsg_cap) {
+        if (e->d_rsg) { CK(cudaStreamSynchronize(e->stream)); CK(cudaFree(e->d_rsg)); e->d_rsg = nullptr; e->rsg_cap = 0; }
+        const size_t want = std::min<size_t>((size_t)e->cap, std::max<size_t>((size_t)n, 1 << 16));
+        CK(dalloc(&e->d_rsg, want * 64));
+        e->rsg_cap = want;
+    }
+    k_rb_prep<<<std::max(1, std::min(8 * e->n_sm, (n + 7) / 8)), 256, 0, e->stream>>>(R, K, rows ? e->d_rsg : nullptr);
     CK(cudaGetLastError());
+    e->stats.kernel_launches += 1;
     return 0;
 }
 
@@ -391,8 +432,7 @@ int round_batch_prep(sw_engine *e, int first, int n, int grid, RbParams &R, int 
 template <int NC>
 int round_batch_finish(sw_engine *e, const RbParams &R) {
     const int n = R.n, blocks = std::max(1, std::min(296, (n + 255) / 256));
-    k_rb_tail<<<blocks, 256, 0, e->stream>>>(R);
-    k_rb_witness<<<blocks, 256, 0, e->stream>>>(R);
+    k_rb_finish<<<blocks, 256, 0, e->stream>>>(R);
     k_rb_seenmask<NC><<<(n + 7) / 8, 256, 0, e->stream>>>(R);
     CK(cudaGetLastError());
     StrongParams Q{};
@@ -403,23 +443,10 @@ int round_batch_finish(sw_engine *e, const RbParams &R) {
     const int sblocks = std::max(1, std::min((n + 7) / 8, 4 * e->n_sm));
     k_strong<NC><<<sblocks, 256, 0, e->stream>>>(Q);
     CK(cudaGetLastError());
-    e->stats.kernel_launches += 8;
+    e->stats.kernel_launches += 3;
     return 0;
 }
 
-// seq-space rows of the chunk for the cluster round kernel (after round_batch_prep grouped the chunk by creator)
-int rc_seqrows(sw_engine *e, const RbParams &R) {
-    const int n = R.n;
-    if ((size_t)n > e->rsg_cap) {
-        if (e->d_rsg) { CK(cudaStreamSynchronize(e->stream)); CK(cudaFree(e->d_rsg)); e->d_rsg = nullptr; e->rsg_cap = 0; }
-        const size_t want = std::min<size_t>((size_t)e->cap, std::max<size_t>((size_t)n, 1 << 16));
-        CK(dalloc(&e->d_rsg, want * 64));
-        e->rsg_cap = want;
-    }
-    k_rc_seqrows<<<std::max(1, std::min(4 * e->n_sm, (n + 7) / 8)), 256, 0, e->stream>>>(R, e->d_rsg);
-    CK(cudaGetLastError());
-    return 0;
-}
 void rc_launch_config(cudaLaunchConfig_t &cfg, cudaLaunchAttribute *at, int clusters, cudaStream_t stream) {
     cfg = cudaLaunchConfig_t{};
     cfg.gridDim = dim3(RC_CS * clusters); cfg.blockDim = dim3(RC_THREADS); cfg.dynamicSmemBytes = RC_SMEM_BYTES; cfg.stream = stream;
@@ -428,21 +455,22 @@ void rc_launch_config(cudaLaunchConfig_t &cfg, cudaLaunchAttribute *at, int clus
     cfg.attrs = at; cfg.numAttrs = 1;
 }
 
+// `start`: the event that opens the caller's span, recorded just before (the round-kernel span starts there too: an
+// event record costs the stream a few microseconds)
 template <int NC, bool UNIT>
-int divide_round_batch(sw_engine *e, int first, int n) {
+int divide_round_batch(sw_engine *e, int first, int n, cudaEvent_t start) {
     // a few SMs stay free for the can_see scan of the next chunk, which runs beside this kernel (SW_RB_FREE_SMS)
     int free_sms = 16;
     if (const char *v = getenv("SW_RB_FREE_SMS")) free_sms = std::max(0, atoi(v));
     const int grid = std::max(e->n_sm / 2, e->n_sm - free_sms);
+    const bool rc = e->rc_ok && n >= e->rc_min_n;
     RbParams R;
-    if (round_batch_prep(e, first, n, grid, R) < 0) return SW_E_CUDA;
     void *args[] = {(void *)&R};
     {
-        cudaEvent_t a = get_event(e), b = get_event(e);
-        cudaEventRecord(a, e->stream);
-        if (e->rc_ok && n >= e->rc_min_n) {
+        cudaEvent_t b = get_event(e);
+        if (round_batch_prep(e, first, n, grid, rc, R) < 0) return SW_E_CUDA;
+        if (rc) {
             // the chunk inside one thread-block cluster; k_rounds_batch takes over whatever it hands back (normally nothing)
-            if (rc_seqrows(e, R) < 0) return SW_E_CUDA;
             RcParams Q{R, e->d_rsg, e->d_rccont};
             cudaLaunchConfig_t cfg;
             cudaLaunchAttribute at[1];
@@ -450,12 +478,13 @@ int divide_round_batch(sw_engine *e, int first, int n) {
             if (e->rc_mb) CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster<UNIT, true>, Q));
             else CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster<UNIT, false>, Q));
             R.cont = e->d_rccont;
-            e->stats.kernel_launches += 2;
+            e->stats.kernel_launches += 1;
             e->stats.rounds_cluster_launches += 1;
         }
         CK(cudaLaunchCooperativeKernel((void *)k_rounds_batch<NC, UNIT>, dim3(grid), dim3(RB_THREADS), args, 0, e->stream));
+        e->stats.kernel_launches += 1;
         cudaEventRecord(b, e->stream);
-        e->spans.push_back(TimedSpan{a, b, 4});
+        e->spans.push_back(TimedSpan{start, b, 4, true});
     }
     return round_batch_finish<NC>(e, R);
 }
@@ -508,8 +537,7 @@ int divide_rounds_wide(sw_engine *e, int first, int n) {
     T.M = M; T.first = first; T.n = n; T.Rcap = e->Rcap; T.p0 = e->d_p0; T.creator = e->d_creator; T.seq = e->d_seq;
     T.round = e->d_round; T.ctot = e->d_rbtot; T.gchain = e->d_gchain; T.wit = e->d_wit; T.W = e->d_W;
     T.wlist = wlist; T.wcnt = wcnt;
-    k_rb_tail<<<blocks, 256, 0, e->stream>>>(T);
-    k_rb_witness<<<blocks, 256, 0, e->stream>>>(T);
+    k_rb_finish<<<blocks, 256, 0, e->stream>>>(T);
     k_w_seenmask<NJ><<<std::max(1, std::min(8 * e->n_sm, (n + 7) / 8)), 256, 0, e->stream>>>(M, first, n, e->Rcap, e->d_row, e->d_round, e->d_W, e->d_SMw);
     CK(cudaGetLastError());
     StrongParams Q{};
@@ -521,7 +549,7 @@ int divide_rounds_wide(sw_engine *e, int first, int n) {
     CK(cudaFuncSetAttribute(k_w_strong<NJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssm));
     k_w_strong<NJ><<<std::max(1, std::min(4 * e->n_sm, (n + 7) / 8)), 256, ssm, e->stream>>>(Q);
     CK(cudaGetLastError());
-    e->stats.kernel_launches += 8;
+    e->stats.kernel_launches += 7;
     return 0;
 }
 
@@ -639,8 +667,9 @@ int sw_create(int M, int capacity_events, const int64_t *stake, int coin_period,
         CK(dalloc(&e->d_round, cap)); CK(dalloc(&e->d_wit, cap)); CK(dalloc(&e->d_famous_ev, cap));
         CK(dalloc(&e->d_W, RM)); CK(dalloc(&e->d_famous, RM));
         CK(dalloc(&e->d_consensus, (size_t)e->Rcap)); CK(dalloc(&e->d_done, (size_t)e->Rcap)); CK(dalloc(&e->d_coin, RM));
-        CK(dalloc(&e->d_rem, (size_t)e->Rcap)); CK(dalloc(&e->d_newc, (size_t)e->Rcap));
-        CK(dalloc(&e->d_stake, (size_t)M)); CK(dalloc(&e->d_scal, (size_t)SC_COUNT));
+        CK(dalloc(&e->d_rem, (size_t)e->Rcap));
+        CK(dalloc(&e->d_stake, (size_t)M)); CK(dalloc(&e->d_scal, (size_t)SC_COUNT + e->Rcap));
+        e->d_newc = e->d_scal + SC_COUNT;                  // (sw_decide_fame copies the scalars and the new rounds at once)
         CK(dalloc(&e->d_lastord, MP)); CK(dalloc(&e->d_tx, cap)); CK(dalloc(&e->d_idx, cap));
         CK(dalloc(&e->d_batch_ev, cap)); CK(dalloc(&e->d_batch_seg, cap)); CK(dalloc(&e->d_perm, 2 * cap));
         CK(dalloc(&e->d_ts, cap)); CK(dalloc(&e->d_key, cap * 8));
@@ -650,8 +679,8 @@ int sw_create(int M, int capacity_events, const int64_t *stake, int coin_period,
         for (auto &ev : e->stage_ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
         if (const char *v = getenv("SW_STREAM_N")) e->stream_n = std::max(0, std::min(1024, atoi(v)));
         CK(cudaFuncSetAttribute(k_stream_divide<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
-        CK(cudaMallocHost((void **)&e->h_scal, sizeof(int32_t) * SC_COUNT));
-        CK(cudaMallocHost((void **)&e->h_newc, sizeof(int32_t) * e->Rcap));
+        CK(cudaMallocHost((void **)&e->h_scal, sizeof(int32_t) * ((size_t)SC_COUNT + e->Rcap)));
+        e->h_newc = e->h_scal + SC_COUNT;
         CK(cudaMemcpyAsync(e->d_stake, e->h_stake.data(), sizeof(i64) * M, cudaMemcpyHostToDevice, e->stream));
         // kernels that need more than the default 48 KB of dynamic shared memory
         const size_t cs_smem = (size_t)(M + CS_SV) * CS_CT * sizeof(int) + CS_TILE * sizeof(int4) + 3 * CS_TILE;
@@ -696,12 +725,11 @@ void sw_destroy(sw_engine *e) {
                     e->d_p0, e->d_p1, e->d_creator, e->d_seq, e->d_t, e->d_sig, e->d_row, e->d_SM,
                     e->d_scw, e->d_sctag, e->d_SMw, e->d_Sw, e->d_hitmin, e->d_xbuf, e->d_xstep,
                     e->d_round, e->d_wit, e->d_famous_ev, e->d_W, e->d_S, e->d_famous, e->d_consensus,
-                    e->d_done, e->d_rem, e->d_newc, e->d_stake, e->d_scal, e->d_lastord, e->d_tx, e->d_idx,
+                    e->d_done, e->d_rem, e->d_stake, e->d_scal, e->d_lastord, e->d_tx, e->d_idx,
                     e->d_batch_ev, e->d_batch_seg, e->d_perm, e->d_ts, e->d_key, e->d_seg_start, e->d_seg_fw,
                     e->d_seg_nf, e->d_seg_white, e->d_rounds_in, e->d_plan, e->d_flush, e->d_rsg, e->d_rccont};
     for (void *p : ptrs) if (p) cudaFree(p);
     if (e->h_scal) cudaFreeHost(e->h_scal);
-    if (e->h_newc) cudaFreeHost(e->h_newc);
     if (e->h_height) cudaFreeHost(e->h_height);
     if (e->h_seq) cudaFreeHost(e->h_seq);
     if (e->h_stale) cudaFreeHost(e->h_stale);
@@ -763,6 +791,7 @@ int sw_append(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const i
     std::vector<int32_t> head_save(e->h_head), count_save(e->h_count);
     e->h_creator.resize((size_t)base + n);
     int rc = SW_OK;
+    int next_snap = e->wide ? INT32_MAX : (base / sw_engine::SNAP + 1) * sw_engine::SNAP;
     for (int j = 0; j < n && rc == SW_OK; j++) {
         const int i = base + j, c = creator[j], a = p0[j], b = p1[j];
         if (c < 0 || c >= e->M) { rc = fail(e, SW_E_ARG, "event %d: creator %d out of range", i, c); break; }
@@ -781,14 +810,17 @@ int sw_append(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const i
         e->h_creator[i] = c;
         e->h_head[c] = i;
         e->h_seq[i] = e->h_count[c]++;
+        if (i + 1 == next_snap) { push_snapshot(e, i + 1, e->h_count); next_snap += sw_engine::SNAP; }
     }
     if (rc == SW_OK) {
         e->h_stale_cum.resize((size_t)base + n + 1);
         for (int j = 0; j < n; j++) e->h_stale_cum[base + j + 1] = e->h_stale_cum[base + j] + e->h_stale[base + j];
+        if (!e->wide && (e->snap_at.empty() || e->snap_at.back() != base + n)) push_snapshot(e, base + n, e->h_count);
     }
     if (rc != SW_OK) {
         e->h_head = head_save; e->h_count = count_save;
         e->h_creator.resize(base);
+        while (!e->snap_at.empty() && e->snap_at.back() > base) { e->snap_at.pop_back(); e->snap_cnt.resize(e->snap_at.size() * e->M); }
         return rc;
     }
     // The copies go to their own stream: they touch only the new rows, so they overlap the kernels of
@@ -888,8 +920,8 @@ int sw_divide_rounds(sw_engine *e, int first, int n) {
         Span sp(e, 0);
         int rc;
         if (e->wide) rc = SW_NJ(divide_rounds_wide, e, first, n);
-        else rc = e->NC == 1 ? (e->unit ? divide_round_batch<1, true>(e, first, n) : divide_round_batch<1, false>(e, first, n))
-                             : (e->unit ? divide_round_batch<2, true>(e, first, n) : divide_round_batch<2, false>(e, first, n));
+        else rc = e->NC == 1 ? (e->unit ? divide_round_batch<1, true>(e, first, n, sp.s.a) : divide_round_batch<1, false>(e, first, n, sp.s.a))
+                             : (e->unit ? divide_round_batch<2, true>(e, first, n, sp.s.a) : divide_round_batch<2, false>(e, first, n, sp.s.a));
         if (rc < 0) return rc;
     }
     e->stats.events_divided += n;
@@ -937,12 +969,10 @@ int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, c
                 x->scan_ev_set = true;
             } else if (wait_appends(x, first[v] + n[v]) < 0) return SW_E_CUDA;
             // a view's window stays a round deep (16 pending events per chain) however few warps it has: they loop
-            if (round_batch_prep(x, first[v], n[v], G, Rv[v], 16) < 0) { e->err = x->err; return SW_E_CUDA; }
+            if (round_batch_prep(x, first[v], n[v], G, use_rc, Rv[v], 16) < 0) { e->err = x->err; return SW_E_CUDA; }
             if (use_rc) {
-                if (rc_seqrows(x, Rv[v]) < 0) { e->err = x->err; return SW_E_CUDA; }
                 Qv[v] = RcParams{Rv[v], x->d_rsg, x->d_rccont};
                 Rv[v].cont = x->d_rccont;
-                x->stats.kernel_launches += 1;
             }
             cudaEvent_t ev = get_event(x);
             CK(cudaEventRecord(ev, x->stream));
@@ -970,6 +1000,7 @@ int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, c
             void *fn = e->NC == 1 ? (e->unit ? (void *)k_rounds_batch_views<1, true> : (void *)k_rounds_batch_views<1, false>)
                                   : (e->unit ? (void *)k_rounds_batch_views<2, true> : (void *)k_rounds_batch_views<2, false>);
             CK(cudaLaunchCooperativeKernel(fn, dim3(nv * G), dim3(RB_THREADS), args, 0, e->stream));
+            e->stats.kernel_launches += 1;
             cudaEventRecord(b, e->stream);
             e->spans.push_back(TimedSpan{a, b, 4});
         }
@@ -997,19 +1028,24 @@ int sw_decide_fame(sw_engine *e, int32_t *new_c_out, int cap) {
     P.Sw = e->d_Sw;
     {
         Span sp(e, 1);
-        k_fame_begin<<<1, 32, 0, e->stream>>>(P);
-        if (e->wide) SW_NJ(fame_rounds_wide, e, P);
-        else k_fame_rounds<<<2 * e->n_sm, 256, 0, e->stream>>>(P);
-        k_fame_finish<<<1, 1024, 0, e->stream>>>(P);
+        if (e->wide) {
+            k_fame_begin<<<1, 32, 0, e->stream>>>(P);
+            SW_NJ(fame_rounds_wide, e, P);
+            k_fame_finish<<<1, 1024, 0, e->stream>>>(P);
+            e->stats.kernel_launches += 3;
+        } else {
+            k_fame_rounds<<<2 * e->n_sm, 256, 0, e->stream>>>(P);
+            e->stats.kernel_launches += 1;
+        }
         CK(cudaGetLastError());
     }
-    e->stats.kernel_launches += 3;
-    // one copy pair, one synchronisation: the scalars and (speculatively) the first new consensus rounds together
-    const int spec = std::min(e->Rcap, 64);
-    CK(cudaMemcpyAsync(e->h_scal, e->d_scal, sizeof(int32_t) * SC_COUNT, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaMemcpyAsync(e->h_newc, e->d_newc, sizeof(int32_t) * spec, cudaMemcpyDeviceToHost, e->stream));
+    // one copy, one synchronisation: the scalars and (speculatively) the first new consensus rounds together
+    // (a 64-member chunk of 64 K events brings about 90 new rounds: room for 64 only would add a copy and a
+    // synchronisation to every such call)
+    const int spec = std::min(e->Rcap, 1024);
+    CK(cudaMemcpyAsync(e->h_scal, e->d_scal, sizeof(int32_t) * (SC_COUNT + spec), cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
-    fold_spans(e);
+    if (e->spans.size() >= 256) fold_spans(e);         // (the timings are read in sw_sync / sw_stats; not on every call)
     e->stats.d2h_bytes += sizeof(int32_t) * (SC_COUNT + spec);
     int rc = device_error(e);
     if (rc < 0) return rc;
@@ -1418,6 +1454,13 @@ int sw_load(const char *path, int device, int capacity_events, sw_engine **out) 
     e->n_events = n; e->n_divided = nd; e->n_tx = H.n_tx; e->n_rowed = nr; e->rb_epoch = H.rb_epoch;
     e->h_stale_cum.assign((size_t)n + 1, 0);
     for (int i = 0; i < n; i++) e->h_stale_cum[i + 1] = e->h_stale_cum[i] + e->h_stale[i];
+    if (!e->wide) {
+        std::vector<int32_t> cnt(M, 0);
+        for (int i = 0; i < n; i++) {
+            cnt[e->h_creator[i]]++;
+            if ((i + 1) % sw_engine::SNAP == 0 || i + 1 == n) push_snapshot(e, i + 1, cnt);
+        }
+    }
     e->stats.events = n; e->stats.events_divided = nd;
     *out = e;
     return SW_OK;

@@ -24,7 +24,7 @@ typedef long long i64;
 
 #define SW_WC 16             // rounds of the witness table cached in shared memory
 
-enum { SC_MAX_ROUND = 0, SC_ERR = 1, SC_NEWC = 2, SC_BATCH = 3, SC_NSEG = 4, SC_MAXC = 5, SC_COUNT = 8 };
+enum { SC_MAX_ROUND = 0, SC_ERR = 1, SC_NEWC = 2, SC_BATCH = 3, SC_NSEG = 4, SC_MAXC = 5, SC_TICKET = 6, SC_COUNT = 8 };
 
 struct DivParams {
     int M, first, n, Rcap;
@@ -141,8 +141,10 @@ __global__ void __launch_bounds__(256) k_strong(StrongParams P) {
 // threads per witness (each covers a quarter of the <= 64 voters of a round), and a CTA stops as
 // soon as all of its witnesses are decided (2-4 voter rounds, unless coin rounds are needed).
 // The vote mask of x lives in registers; the voter rows (W, S, coin of round r_) are staged in
-// shared memory one round ahead.  k_fame_begin finds max_c (swirld.py:226-228), k_fame_finish
-// collects the rounds that reached consensus in ascending order (swirld.py:274-276).
+// shared memory one round ahead.  Every CTA first finds max_c (swirld.py:226-228); the last CTA to
+// finish collects the rounds that reached consensus in ascending order (swirld.py:274-276).  The wide
+// kernel (swirld_wide.cuh) adds its tallies up from several CTAs per round, so there k_fame_begin and
+// k_fame_finish do these two parts as kernels of their own.
 struct FameParams {
     int M, Rcap, C;
     const int32_t *W;        // [Rcap][M]
@@ -161,9 +163,10 @@ struct FameParams {
     const unsigned *Sw;      // wide path: S as [Rcap][M][NJ] words
 };
 
-__global__ void k_fame_begin(FameParams P) {                    // one warp
-    const int lane = threadIdx.x;
-    int mc = max(P.scal[SC_MAXC], 0);                           // consensus only grows: resume from the last answer
+// max_c: the first round without consensus (swirld.py:226-228), by one whole warp.  Consensus only grows: the scan
+// resumes from the last answer.
+__device__ __forceinline__ int fame_max_c(const FameParams &P, int lane) {
+    int mc = max(P.scal[SC_MAXC], 0);
     for (;;) {
         const int r = mc + lane;
         const bool open = r >= P.Rcap || !P.consensus[r];
@@ -171,22 +174,55 @@ __global__ void k_fame_begin(FameParams P) {                    // one warp
         if (b) { mc += __ffs(b) - 1; break; }
         mc += 32;
     }
-    if (lane == 0) { P.scal[SC_MAXC] = min(mc, P.Rcap); P.scal[SC_NEWC] = 0; }
-    // the open rounds' tallies (the wide kernel adds them up from several CTAs per round)
-    const int max_r = P.scal[SC_MAX_ROUND];
-    for (int r = min(mc, P.Rcap) + lane; r <= max_r && r < P.Rcap; r += 32) { P.rem[r] = 0; P.done[r] = 0; }
+    return min(mc, P.Rcap);
 }
 
+// the rounds of [max_c, max_r] that reached consensus, ascending, into newc (swirld.py:274-276), by one whole CTA
+__device__ __forceinline__ void fame_collect(const FameParams &P, int max_c, int max_r) {
+    __shared__ int wsum_s[32], s_base;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarp = blockDim.x >> 5;
+    if (tid == 0) s_base = 0;
+    __syncthreads();
+    for (int r0 = max_c; r0 <= max_r; r0 += blockDim.x) {
+        const int r = r0 + tid;
+        const bool hit = r <= max_r && __ldcg(P.done + r) && __ldcg(P.rem + r) == 0;
+        const unsigned b = __ballot_sync(0xffffffffu, hit);
+        if (lane == 0) wsum_s[warp] = __popc(b);
+        __syncthreads();
+        int before = s_base;
+        for (int w = 0; w < warp; w++) before += wsum_s[w];
+        if (hit) { P.newc[before + __popc(b & ((1u << lane) - 1))] = r; P.consensus[r] = 1; }
+        __syncthreads();
+        if (tid == 0) { int t = 0; for (int w = 0; w < nwarp; w++) t += wsum_s[w]; s_base += t; }
+        __syncthreads();
+    }
+    if (tid == 0) { P.scal[SC_NEWC] = s_base; P.scal[SC_MAXC] = max_c; }
+}
+
+__global__ void k_fame_begin(FameParams P) {                    // one warp
+    const int lane = threadIdx.x;
+    const int mc = fame_max_c(P, lane);
+    if (lane == 0) { P.scal[SC_MAXC] = mc; P.scal[SC_NEWC] = 0; }
+    // the open rounds' tallies (the wide kernel adds them up from several CTAs per round)
+    const int max_r = P.scal[SC_MAX_ROUND];
+    for (int r = mc + lane; r <= max_r && r < P.Rcap; r += 32) { P.rem[r] = 0; P.done[r] = 0; }
+}
+
+// M <= 64: each candidate round is one CTA's, which writes its rem / done whole
 __global__ void __launch_bounds__(256) k_fame_rounds(FameParams P) {
     __shared__ u64 sv[2][64];
     __shared__ i64 vsum[2][64];
     __shared__ i64 stake_s[64];
     __shared__ int vw[2][64];
     __shared__ int vcoin[2][64];
+    __shared__ int s_maxc;
+    __shared__ bool s_last;
     const int tid = threadIdx.x, M = P.M;
     const int max_r = P.scal[SC_MAX_ROUND];                     // swirld.py:225
-    const int max_c = P.scal[SC_MAXC];
+    if (tid < 32) { const int mc = fame_max_c(P, tid); if (tid == 0) s_maxc = mc; }
     if (tid < 64) stake_s[tid] = tid < M ? P.stake[tid] : 0;
+    __syncthreads();
+    const int max_c = s_maxc;
     const int mx = tid >> 2, q = tid & 3, mq0 = q * 16;
     const unsigned qmask = 0xFu << (tid & 28);
     auto load_voters = [&](int r_, int buf) {                   // threads 0..63
@@ -254,28 +290,22 @@ __global__ void __launch_bounds__(256) k_fame_rounds(FameParams P) {
         const int dn = __syncthreads_or(any_decided);
         if (tid == 0) { P.rem[r] = left; P.done[r] = dn ? 1 : 0; }
     }
+    // the last CTA to get here collects (every CTA read SC_MAXC and the consensus flags before it arrived); the ticket
+    // is back at zero for the next call
+    __syncthreads();
+    if (tid == 0) {
+        __threadfence();
+        s_last = atomicAdd(reinterpret_cast<unsigned *>(P.scal + SC_TICKET), 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    if (tid == 0) P.scal[SC_TICKET] = 0;
+    fame_collect(P, max_c, max_r);
 }
 
-__global__ void __launch_bounds__(1024, 1) k_fame_finish(FameParams P) {   // swirld.py:274-276
-    __shared__ int wsum_s[32], s_base;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int max_r = P.scal[SC_MAX_ROUND], max_c = P.scal[SC_MAXC];
-    if (tid == 0) s_base = 0;
-    __syncthreads();
-    for (int r0 = max_c; r0 <= max_r; r0 += 1024) {
-        const int r = r0 + tid;
-        const bool hit = r <= max_r && P.done[r] && P.rem[r] == 0;
-        const unsigned b = __ballot_sync(0xffffffffu, hit);
-        if (lane == 0) wsum_s[warp] = __popc(b);
-        __syncthreads();
-        int before = s_base;
-        for (int w = 0; w < warp; w++) before += wsum_s[w];
-        if (hit) { P.newc[before + __popc(b & ((1u << lane) - 1))] = r; P.consensus[r] = 1; }
-        __syncthreads();
-        if (tid == 0) { int t = 0; for (int w = 0; w < 32; w++) t += wsum_s[w]; s_base += t; }
-        __syncthreads();
-    }
-    if (tid == 0) P.scal[SC_NEWC] = s_base;
+__global__ void __launch_bounds__(1024, 1) k_fame_finish(FameParams P) {
+    fame_collect(P, P.scal[SC_MAXC], P.scal[SC_MAX_ROUND]);
 }
 
 // ---------------------------------------------------------------- K4: find_order

@@ -7,7 +7,7 @@
 // shared memory of 16 CTAs and moves it over distributed shared memory (~200 cycles a hop):
 //
 //   * rows in SEQ space: rs(h)[c] = the chain position (swirld.py's implicit per-creator sequence number) of the
-//     event of member c that h sees (k_rc_seqrows, from the can_see table).  Every comparison of the scheme
+//     event of member c that h sees (k_rb_prep, from the can_see table).  Every comparison of the scheme
 //     ("row(k)[c_] >= Wf_r[c_]") holds in seq space as it does in index space -- a member's events are ordered the
 //     same way in both -- and a mask S_r(k) is addressed by (member, position) without any lookup.
 //   * CTA q owns chains 4q..4q+3: a window of RC_WN consecutive rows per chain (and their event indices) in its
@@ -52,7 +52,7 @@
 
 struct RcParams {
     RbParams R;
-    const int32_t *rsg;      // [n][64] seq-space rows of the chunk's events in cev order (k_rc_seqrows)
+    const int32_t *rsg;      // [n][64] seq-space rows of the chunk's events in cev order (k_rb_prep)
     int32_t *cont;           // [0,64) positions, [64,128) rounds, [128] 1 = k_rounds_batch has work left
 };
 
@@ -60,20 +60,6 @@ struct RcParams {
 #define RC_SMEM_MASK ((size_t)2 * 64 * RC_MRS * 8)   // two mask tables: a CTA may receive the next step's masks while it still tests
 #define RC_SMEM_WLS ((size_t)RB_WR * 64 * 4)
 #define RC_SMEM_BYTES (RC_SMEM_ROWS + RC_SMEM_MASK + RC_SMEM_WLS + 512 + 10240)
-
-// seq-space rows of the chunk, grouped by creator like cev: one warp per event
-__global__ void __launch_bounds__(256) k_rc_seqrows(RbParams P, int32_t *rsg) {
-    const int lane = threadIdx.x & 31;
-    for (int j = blockIdx.x * 8 + (threadIdx.x >> 5); j < P.n; j += gridDim.x * 8) {
-        const int h = P.cev[P.first + j];
-#pragma unroll
-        for (int u = 0; u < 2; u++) {
-            const int c = lane + 32 * u;
-            const int v = c < P.M ? P.row[(size_t)h * P.M + c] : -1;
-            rsg[(size_t)j * 64 + c] = v < 0 ? -1 : P.seq[v];
-        }
-    }
-}
 
 __device__ __forceinline__ unsigned rc_cta_rank() { unsigned r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ void rc_cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }

@@ -53,7 +53,7 @@ struct RbParams {
     int32_t *ctot;              // [64] events of the member so far (1 + its largest seq)
     int32_t *gchain;            // [64][RB_RING] the member's most recent events by seq % RB_RING
     int32_t *coff;              // [65]
-    unsigned *bar;              // grid barrier counter of k_rounds_batch (zeroed by k_rb_offsets)
+    unsigned *bar;              // grid barrier counter of k_rounds_batch (zeroed by k_rb_prep)
     uint8_t *res;               // per-step results of k_rounds_batch, 2 x (64 x u64 + 64 x int)
     const i64 *stake;
     i64 tot2;
@@ -62,58 +62,55 @@ struct RbParams {
     uint8_t *wit;               // [cap]   (finish kernels)
     int32_t *W;                 // [Rcap][M] the reference's witnesses table
     u64 *SM;                    // [cap]
-    int32_t *wlist, *wcnt;      // witnesses of the chunk (k_rb_witness -> k_strong)
+    int32_t *wlist, *wcnt;      // witnesses of the chunk (k_rb_finish -> k_strong)
     const int32_t *cont;        // NULL, or where k_rounds_cluster (swirld_rcluster.cuh) stopped: [0,64) positions, [64,128) rounds,
                                 // [128] != 0: there is work left
 };
 
-// ---- per-member event lists of the chunk
-__global__ void __launch_bounds__(256) k_rb_count(RbParams P) {
-    __shared__ int cnt[64], mn[64], mx[64];                   // per CTA first, then one global atomic per member
-    if (threadIdx.x < 64) { cnt[threadIdx.x] = 0; mn[threadIdx.x] = 0x7fffffff; mx[threadIdx.x] = 0; }
-    __syncthreads();
-    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < P.n; j += gridDim.x * blockDim.x) {
+// ---- per-member event lists of the chunk.  Events are divided in arrival order and seq[h] counts the earlier events
+// of h's creator, so the per-member counts of a chunk are known on the host (round_batch_prep) and arrive by value.
+struct RbChunk {
+    int ccnt[64];               // events of the member in the chunk
+    int cmin[64];               // the smallest seq among them (0x7f7f7f7f: none)
+    int ctot[64];               // events of the member up to the end of the chunk
+    int coff[65];               // exclusive prefix sum of ccnt
+};
+
+// the chunk's meta arrays, cev, and (rsg != NULL) the seq-space rows of swirld_rcluster.cuh in cev order: one warp per event
+__global__ void __launch_bounds__(256) k_rb_prep(RbParams P, const __grid_constant__ RbChunk K, int32_t *rsg) {
+    const int tid = threadIdx.x, lane = tid & 31;
+    if (blockIdx.x == 0) {
+        if (tid < 64) { P.ccnt[tid] = K.ccnt[tid]; P.cmin[tid] = K.cmin[tid]; if (tid < P.M) P.ctot[tid] = K.ctot[tid]; }
+        if (tid <= 64) P.coff[tid] = K.coff[tid];
+        if (tid == 0) { *P.bar = 0; *P.wcnt = 0; }
+    }
+    for (int j = blockIdx.x * 8 + (tid >> 5); j < P.n; j += gridDim.x * 8) {
         const int h = P.first + j, c = P.creator[h];
-        const int sq = P.seq[h];
-        atomicAdd(&cnt[c], 1);
-        atomicMin(&mn[c], sq);
-        atomicMax(&mx[c], sq + 1);
-    }
-    __syncthreads();
-    if (threadIdx.x < P.M && cnt[threadIdx.x] > 0) {
-        const int c = threadIdx.x;
-        atomicAdd(&P.ccnt[c], cnt[c]);
-        atomicMin(&P.cmin[c], mn[c]);
-        atomicMax(&P.ctot[c], mx[c]);
-    }
-}
-__global__ void k_rb_offsets(RbParams P) {       // one warp
-    const int lane = threadIdx.x;
-    int a = lane < P.M ? P.ccnt[lane] : 0, b = lane + 32 < P.M ? P.ccnt[lane + 32] : 0;
-    int sa = a, sb = b;
+        const int d = K.coff[c] + P.seq[h] - K.cmin[c];
+        if (lane == 0) P.cev[P.first + d] = h;
+        if (rsg) {
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int x = __shfl_up_sync(0xffffffffu, sa, o), y = __shfl_up_sync(0xffffffffu, sb, o);
-        if (lane >= o) { sa += x; sb += y; }
-    }
-    const int tot_a = __shfl_sync(0xffffffffu, sa, 31);
-    P.coff[lane] = sa - a;
-    P.coff[lane + 32] = tot_a + sb - b;
-    if (lane == 31) P.coff[64] = tot_a + sb;
-    if (lane == 0) { *P.bar = 0; *P.wcnt = 0; }
-}
-__global__ void k_rb_scatter(RbParams P) {
-    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < P.n; j += gridDim.x * blockDim.x) {
-        const int h = P.first + j, c = P.creator[h];
-        P.cev[P.first + P.coff[c] + P.seq[h] - P.cmin[c]] = h;
+            for (int u = 0; u < 2; u++) {
+                const int m = lane + 32 * u;
+                const int v = m < P.M ? P.row[(size_t)h * P.M + m] : -1;
+                rsg[(size_t)d * 64 + m] = v < 0 ? -1 : P.seq[v];
+            }
+        }
     }
 }
 
-// after the chunk: remember each member's most recent RB_RING events for the next chunk
-__global__ void k_rb_tail(RbParams P) {
+// ---- after the round kernel, one pass over the chunk: each member's most recent RB_RING events for the next chunk, and
+// the reference's witness flags / witnesses table from the finished rounds (swirld.py:221-222, 196-197)
+__global__ void k_rb_finish(RbParams P) {
     for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < P.n; j += gridDim.x * blockDim.x) {
-        const int h = P.first + j, c = P.creator[h], sq = P.seq[h];
+        const int h = P.first + j, c = P.creator[h], sq = P.seq[h], pa = P.p0[h], r = P.round[h];
         if (P.ctot[c] - sq <= RB_RING) P.gchain[c * RB_RING + (sq & (RB_RING - 1))] = h;
+        const bool wit = pa < 0 || r > P.round[pa];
+        P.wit[h] = wit ? 1 : 0;
+        if (wit && r >= 0 && r < P.Rcap) {
+            P.W[(size_t)r * P.M + c] = h;
+            P.wlist[atomicAdd(P.wcnt, 1)] = h;                // k_strong runs over the witnesses only
+        }
     }
 }
 
@@ -555,18 +552,6 @@ __global__ void __launch_bounds__(RB_THREADS, 1) k_rounds_batch_views(const RbPa
     rounds_batch_body<NC, UNIT>(Ps, blockIdx.x % G, G);
 }
 
-// ---- the reference's witness flags / witnesses table from the finished rounds (swirld.py:221-222, 196-197)
-__global__ void k_rb_witness(RbParams P) {
-    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < P.n; j += gridDim.x * blockDim.x) {
-        const int h = P.first + j, pa = P.p0[h], r = P.round[h];
-        const bool wit = pa < 0 || r > P.round[pa];
-        P.wit[h] = wit ? 1 : 0;
-        if (wit && r >= 0 && r < P.Rcap) {
-            P.W[(size_t)r * P.M + P.creator[h]] = h;
-            P.wlist[atomicAdd(P.wcnt, 1)] = h;                // k_strong runs over the witnesses only
-        }
-    }
-}
 // ---- SM(h) = {c_ : W[round h][c_] >= 0 and row(h)[c_] >= W[round h][c_]}, one warp per event
 template <int NC>
 __global__ void __launch_bounds__(256) k_rb_seenmask(RbParams P) {
