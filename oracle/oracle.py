@@ -123,6 +123,10 @@ class Oracle:
     def max_round(self):
         return lib().or_max_round(self._h)
 
+    @property
+    def n_transactions(self):
+        return lib().or_n_transactions(self._h)
+
     def results(self):
         n, M = self.n, self.M
         rnd = np.empty(n, np.int32); lib().or_get_round(self._h, rnd)

@@ -18,6 +18,8 @@ crypto:
   valid event per swirld.py:103-108, never a true fork).
 * G3 ``tick``         -- tick-synchronous: every tick each member creates one
   event on a random peer's previous-tick head (frontier width == M).
+* G5 ``partition``    -- G1 with the network split in two sides for a window of
+  events, then healed (stalled rounds, chains far behind, huge heal rounds).
 
 Everything is pure ``random.Random(seed)`` + ``hashlib.blake2b`` so that the
 same trace is rebuilt bit-for-bit here, in the golden-fixture script and on
@@ -129,6 +131,42 @@ def adversarial(M: int, N: int, seed: int = 1, p_cross: float = 0.02,
         head[a] = i
     return _finish(M, p0, p1, cr, seed,
                    "G2(M=%d,N=%d,seed=%d,pc=%g,ps=%g)" % (M, N, seed, p_cross, p_stale), tied)
+
+
+def partition(M: int, N: int, seed: int = 1, split: int | None = None, start: int = 0, end: int | None = None,
+              tied: int = 0) -> Trace:
+    """G5: a network partition that heals.  G1, except that for events ``start <= i < end`` the peer ``b`` is drawn
+    from the creator's own side, ``[0, split)`` or ``[split, M)`` (``split`` defaults to M // 2, ``end`` to N).
+
+    With an even split neither side holds more than 2/3 of the members, so no witness of either side can strongly see
+    a supermajority: every member stalls in one round for the whole partition, hundreds of events per chain.  With
+    a split above 2/3 the majority side keeps advancing rounds while the minority stalls, and on heal the minority's
+    chains are dozens to hundreds of rounds behind.  The heal round orders a whole partition's events at once.  These
+    are the sizes the kernels are built around (DESIGN.md section 2): runs of one member's events in one round longer
+    than the 256-event rings of the round kernels (RB_RING, RW_RING) and the 128-row window of the cluster round
+    kernel (RC_WN), chains more than the 32 rounds of its Wf mirror (RB_WR) apart, and consensus rounds of more than
+    the 1024 events k_order_sort's block sorts in one pass."""
+    split = M // 2 if split is None else split
+    end = N if end is None else end
+    assert 2 <= split <= M - 2 and N >= M and 0 <= start <= end
+    rng = random.Random(seed)
+    p0 = [-1] * M
+    p1 = [-1] * M
+    cr = list(range(M))
+    head = list(range(M))
+    for i in range(M, N):
+        a = rng.randrange(M)
+        if start <= i < end:
+            lo, hi = (0, split) if a < split else (split, M)
+            b = lo + rng.randrange(hi - lo - 1)
+        else:
+            b = rng.randrange(M - 1)
+        b += (b >= a)
+        p0.append(head[a])
+        p1.append(head[b])
+        cr.append(a)
+        head[a] = i
+    return _finish(M, p0, p1, cr, seed, "G5(M=%d,N=%d,seed=%d,split=%d,[%d,%d))" % (M, N, seed, split, start, end), tied)
 
 
 def tick(M: int, N: int, seed: int = 1) -> Trace:

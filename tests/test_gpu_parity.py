@@ -466,7 +466,8 @@ def test_native_ingest_orders_and_validates():
 @pytest.mark.parametrize("M,N,K,B", [(4, 2000, 50, 5), (16, 30000, 4096, 8), (64, 40000, 8192, 3), (33, 9000, 1500, 40)])
 def test_batched_views_match_the_oracle(M, N, K, B):
     """B independent node-views (own traces) advanced together by sw_batch_divide_rounds: every view equals the
-    oracle on its own trace and schedule (40 views need more than one cooperative launch at 33 members)."""
+    oracle on its own trace and schedule.  Up to n_sm views share one launch, so 40 views at 33 members are one group
+    of n_sm / 40 CTAs per view; test_gpu_partition.py runs more views than SMs."""
     from swirld_b200 import engine, traces
     from swirld_b200.traces import chunks
     trs = [traces.gossip(M, N - 7 * v, 100 + v) for v in range(B)]       # ragged: the views differ in length
