@@ -106,6 +106,27 @@ int sw_decide_fame(sw_engine *e, int32_t *new_c_out, int cap);
  * swirld.py:310-311). */
 int sw_find_order(sw_engine *e, const int32_t *new_c, int n);
 
+/* Node.decide_fame() and Node.find_order(new_c) for B independent node-views in one call each (the simulation's nodes
+ * each run the reference's whole main loop, swirld.py:325-328).  The views share one member count (any M up to
+ * SW_MAX_MEMBERS), one kernel family (the M <= 64 kernels, or the any-M kernels that SW_FORCE_WIDE=1 selects) and one
+ * device; stakes and coin periods may differ.  Every view's kernels run side by side in a fixed number of launches on
+ * the first engine's stream, after what each view has queued on its own; one copy brings back the scalars of all views
+ * and the call synchronises once.  Timings and launches are charged to the first engine.
+ * Each view ends with exactly the state and results B single calls would have left it.
+ * Argument errors refuse the whole call before anything runs, leave count_out unwritten and put the message in the
+ * first engine's sw_last_error: B < 1, a NULL or repeated engine, a view peer-connected to other GPUs, views that
+ * differ in device, M or kernel family (SW_E_UNSUPPORTED); for decide_fame a view with nothing divided (SW_E_ARG); for
+ * find_order offsets that are not monotone (SW_E_ARG) or a round outside the view's round table (SW_E_KEY).
+ * Errors the device finds belong to their view: count_out[v] gets the code sw_decide_fame / sw_find_order would
+ * have returned (e.g. SW_E_INDEX, a single seer) and the message is in that view's sw_last_error; the other views
+ * complete normally.  Returns SW_OK when every view succeeded, else the first failing view's code. */
+/* new_c_out is B x cap: row v holds view v's new consensus rounds, ascending; count_out[v] = their count.  A view that
+ * brings more than 1024 new rounds costs one more copy. */
+int sw_batch_decide_fame(sw_engine *const *engines, int B, int32_t *new_c_out, int cap, int32_t *count_out);
+/* View v's rounds are new_c[offsets[v] .. offsets[v+1]) (an empty range does nothing); count_out[v] = events appended
+ * to view v's order. */
+int sw_batch_find_order(sw_engine *const *engines, int B, const int32_t *new_c, const int *offsets, int32_t *count_out);
+
 /* ---- views of the Node attributes (swirld.py:48-72) ---- */
 int sw_members(const sw_engine *e);           /* n (swirld.py:40) */
 int sw_n_events(const sw_engine *e);          /* len(hg) */

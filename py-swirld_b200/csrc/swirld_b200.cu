@@ -77,6 +77,10 @@ struct sw_engine {
     RbParams *d_views = nullptr;  // sw_batch_divide_rounds: the views' parameters (owned by the first engine of a batch)
     int views_cap = 0;
     cudaEvent_t view_ev = nullptr;
+    // sw_batch_decide_fame / sw_batch_find_order (owned by the first engine of a batch): the views' parameters, rounds
+    // and gathered scalars, laid out per call in one device block and its pinned host mirror
+    char *d_vbuf = nullptr, *h_vbuf = nullptr;
+    size_t vbuf_bytes = 0;
     int n_rowed = 0;              // events whose can_see row is complete
     // can_see scan scratch (swirld_cansee.cuh)
     int4 *d_cs_meta = nullptr;
@@ -553,11 +557,113 @@ int divide_rounds_wide(sw_engine *e, int first, int n) {
     return 0;
 }
 
+size_t w_fame_smem(int NJ, int M) { return (size_t)(32 * NJ + 64) * sizeof(int) + (size_t)(32 + M) * sizeof(i64); }
+
 template <int NJ>
 int fame_rounds_wide(sw_engine *e, const FameParams &P) {
-    const size_t smem = (size_t)(32 * NJ + 64) * sizeof(int) + (size_t)(32 + e->M) * sizeof(i64);
     const int parts = (e->M + FW_THREADS - 1) / FW_THREADS;
-    k_w_fame_rounds<NJ><<<(2 * e->n_sm / parts + 1) * parts, FW_THREADS, smem, e->stream>>>(P);
+    k_w_fame_rounds<NJ><<<(2 * e->n_sm / parts + 1) * parts, FW_THREADS, w_fame_smem(NJ, e->M), e->stream>>>(P);
+    return 0;
+}
+
+// B views: `x` CTA groups of `parts` CTAs per view
+template <int NJ>
+int fame_rounds_wide_views(sw_engine *e, const FameParams *Pv, int B, int x) {
+    const int parts = (e->M + FW_THREADS - 1) / FW_THREADS;
+    k_w_fame_rounds_views<NJ><<<dim3(x * parts, B), FW_THREADS, w_fame_smem(NJ, e->M), e->stream>>>(Pv);
+    return 0;
+}
+
+FameParams fame_params(const sw_engine *e) {
+    FameParams P{};
+    P.M = e->M; P.Rcap = e->Rcap; P.C = e->C; P.W = e->d_W; P.S = e->d_S; P.famous = e->d_famous;
+    P.famous_ev = e->d_famous_ev; P.consensus = e->d_consensus; P.done = e->d_done; P.rem = e->d_rem;
+    P.coin = e->d_coin; P.stake = e->d_stake; P.tot2 = 2 * e->tot; P.unit = e->unit ? 1 : 0; P.newc = e->d_newc; P.scal = e->d_scal;
+    P.Sw = e->d_Sw;
+    return P;
+}
+
+// find_order's per-round scratch, grown on demand to n rounds
+int order_scratch(sw_engine *e, int n) {
+    if (n <= e->seg_cap) return 0;
+    const size_t MS = e->MS;
+    int nc = std::max(n, std::max(64, 2 * e->seg_cap));
+    for (void *p : {(void *)e->d_seg_start, (void *)e->d_seg_fw, (void *)e->d_seg_nf, (void *)e->d_seg_white, (void *)e->d_rounds_in, (void *)e->d_plan})
+        if (p) cudaFree(p);
+    CK(dalloc(&e->d_seg_start, (size_t)nc + 1)); CK(dalloc(&e->d_seg_fw, (size_t)nc * MS));
+    CK(dalloc(&e->d_seg_nf, (size_t)nc)); CK(dalloc(&e->d_seg_white, (size_t)nc * 64));
+    CK(dalloc(&e->d_rounds_in, (size_t)nc)); CK(dalloc(&e->d_plan, (size_t)nc * MS * 8));
+    e->seg_cap = nc;
+    return 0;
+}
+
+// find_order over the n sorted rounds at `rounds` (device memory)
+OrderParams order_params(const sw_engine *e, int n, const int32_t *rounds) {
+    OrderParams P{};
+    P.M = e->M; P.Rcap = e->Rcap; P.nrounds = n; P.rounds = rounds; P.W = e->d_W; P.famous = e->d_famous;
+    P.row = e->d_row; P.p0 = e->d_p0; P.creator = e->d_creator; P.seq = e->d_seq; P.t = e->d_t; P.sig = e->d_sig;
+    P.stake = e->d_stake; P.tot = e->tot; P.lastord = e->d_lastord; P.batch_ev = e->d_batch_ev; P.batch_seg = e->d_batch_seg;
+    P.seg_start = e->d_seg_start; P.seg_fw = e->d_seg_fw; P.seg_nf = e->d_seg_nf; P.seg_white = e->d_seg_white;
+    P.ts = e->d_ts; P.key = e->d_key; P.perm = e->d_perm; P.tx = e->d_tx; P.idx = e->d_idx; P.tx_base = e->n_tx; P.scal = e->d_scal;
+    P.plan = e->d_plan; P.plan_stride = (int)(e->seg_cap * e->MS);
+    return P;
+}
+
+// ---- several node-views per call (sw_batch_decide_fame / sw_batch_find_order)
+// The shape checks shared by both calls: they refuse the whole batch before anything runs (the message goes to the first
+// engine).
+int check_views(sw_engine *const *engines, int B, const char *what) {
+    sw_engine *e = engines[0];
+    std::vector<const sw_engine *> seen(engines, engines + B);
+    for (int v = 0; v < B; v++)
+        if (!engines[v]) return fail(e, SW_E_ARG, "%s: view %d is NULL", what, v);
+    std::sort(seen.begin(), seen.end());
+    if (std::adjacent_find(seen.begin(), seen.end()) != seen.end()) return fail(e, SW_E_ARG, "%s: an engine appears twice", what);
+    for (int v = 0; v < B; v++) {
+        const sw_engine *x = engines[v];
+        if (x->device != e->device || x->M != e->M || x->wide != e->wide)
+            return fail(e, SW_E_UNSUPPORTED, "%s: view %d: the views must have one member count and one kernel family on one device", what, v);
+        if (x->nranks > 1) return fail(e, SW_E_UNSUPPORTED, "%s: view %d is one rank of a multi-GPU engine", what, v);
+    }
+    return 0;
+}
+
+// the per-call block of the first engine: at least `bytes` on the device and in pinned host memory
+int views_buffer(sw_engine *e, size_t bytes) {
+    if (bytes <= e->vbuf_bytes) return 0;
+    if (e->d_vbuf) { CK(cudaFree(e->d_vbuf)); e->d_vbuf = nullptr; }
+    if (e->h_vbuf) { CK(cudaFreeHost(e->h_vbuf)); e->h_vbuf = nullptr; }
+    const size_t want = std::max(bytes, 2 * e->vbuf_bytes);
+    e->vbuf_bytes = 0;
+    CK(cudaMalloc((void **)&e->d_vbuf, want));
+    CK(cudaMallocHost((void **)&e->h_vbuf, want));
+    e->vbuf_bytes = want;
+    return 0;
+}
+
+size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// the batch runs on the stream of `e`, the first engine: after everything each view has queued on its own
+int views_enter(sw_engine *e, sw_engine *const *views, int B) {
+    for (int v = 0; v < B; v++) {
+        sw_engine *x = views[v];
+        if (x == e) continue;
+        cudaEvent_t ev = get_event(x);
+        CK(cudaEventRecord(ev, x->stream));
+        CK(cudaStreamWaitEvent(e->stream, ev, 0));
+        x->pool.push_back(ev);
+    }
+    return 0;
+}
+
+// ... and each view's next call runs after the batch; then the one copy of the gathered scalars and the one synchronisation
+int views_leave(sw_engine *e, sw_engine *const *views, int B, void *h_dst, const void *d_src, size_t bytes) {
+    if (!e->view_ev) CK(cudaEventCreateWithFlags(&e->view_ev, cudaEventDisableTiming));
+    CK(cudaEventRecord(e->view_ev, e->stream));
+    for (int v = 0; v < B; v++) if (views[v] != e) CK(cudaStreamWaitEvent(views[v]->stream, e->view_ev, 0));
+    CK(cudaMemcpyAsync(h_dst, d_src, bytes, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    e->stats.d2h_bytes += bytes;
     return 0;
 }
 
@@ -565,7 +671,7 @@ int fame_rounds_wide(sw_engine *e, const FameParams &P) {
 
 extern "C" {
 
-int sw_version(void) { return 201; }
+int sw_version(void) { return 202; }
 
 const char *sw_last_error(const sw_engine *e) { return e ? e->err.c_str() : g_create_error.c_str(); }
 
@@ -714,6 +820,8 @@ void sw_destroy(sw_engine *e) {
     if (e->view_ev) cudaEventDestroy(e->view_ev);
     if (e->d_views) cudaFree(e->d_views);
     if (e->d_rcviews) cudaFree(e->d_rcviews);
+    if (e->d_vbuf) cudaFree(e->d_vbuf);
+    if (e->h_vbuf) cudaFreeHost(e->h_vbuf);
     for (auto ev : e->stage_ev) if (ev) cudaEventDestroy(ev);
     if (e->h_stage) cudaFreeHost(e->h_stage);
     if (e->d_stage) cudaFree(e->d_stage);
@@ -1021,11 +1129,7 @@ int sw_decide_fame(sw_engine *e, int32_t *new_c_out, int cap) {
     if (!e || cap < 0 || (cap > 0 && !new_c_out)) return fail(e, SW_E_ARG, "bad argument");
     CK(cudaSetDevice(e->device));
     if (e->n_divided == 0) return fail(e, SW_E_ARG, "decide_fame: no witnesses yet (max() of an empty dict, swirld.py:225)");
-    FameParams P{};
-    P.M = e->M; P.Rcap = e->Rcap; P.C = e->C; P.W = e->d_W; P.S = e->d_S; P.famous = e->d_famous;
-    P.famous_ev = e->d_famous_ev; P.consensus = e->d_consensus; P.done = e->d_done; P.rem = e->d_rem;
-    P.coin = e->d_coin; P.stake = e->d_stake; P.tot2 = 2 * e->tot; P.unit = e->unit ? 1 : 0; P.newc = e->d_newc; P.scal = e->d_scal;
-    P.Sw = e->d_Sw;
+    const FameParams P = fame_params(e);
     {
         Span sp(e, 1);
         if (e->wide) {
@@ -1067,24 +1171,9 @@ int sw_find_order(sw_engine *e, const int32_t *new_c, int n) {
     std::vector<int32_t> rs(new_c, new_c + n);
     std::sort(rs.begin(), rs.end());                                  // sorted(new_c), swirld.py:283
     for (int r : rs) if (r < 0 || r >= e->Rcap) return fail(e, SW_E_KEY, "find_order: unknown round %d", r);
-    const size_t MS = e->MS;
-    if (n > e->seg_cap) {
-        int nc = std::max(n, std::max(64, 2 * e->seg_cap));
-        for (void *p : {(void *)e->d_seg_start, (void *)e->d_seg_fw, (void *)e->d_seg_nf, (void *)e->d_seg_white, (void *)e->d_rounds_in, (void *)e->d_plan})
-            if (p) cudaFree(p);
-        CK(dalloc(&e->d_seg_start, (size_t)nc + 1)); CK(dalloc(&e->d_seg_fw, (size_t)nc * MS));
-        CK(dalloc(&e->d_seg_nf, (size_t)nc)); CK(dalloc(&e->d_seg_white, (size_t)nc * 64));
-        CK(dalloc(&e->d_rounds_in, (size_t)nc)); CK(dalloc(&e->d_plan, (size_t)nc * MS * 8));
-        e->seg_cap = nc;
-    }
+    if (order_scratch(e, n) < 0) return SW_E_CUDA;
     CK(cudaMemcpyAsync(e->d_rounds_in, rs.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, e->stream));
-    OrderParams P{};
-    P.M = e->M; P.Rcap = e->Rcap; P.nrounds = n; P.rounds = e->d_rounds_in; P.W = e->d_W; P.famous = e->d_famous;
-    P.row = e->d_row; P.p0 = e->d_p0; P.creator = e->d_creator; P.seq = e->d_seq; P.t = e->d_t; P.sig = e->d_sig;
-    P.stake = e->d_stake; P.tot = e->tot; P.lastord = e->d_lastord; P.batch_ev = e->d_batch_ev; P.batch_seg = e->d_batch_seg;
-    P.seg_start = e->d_seg_start; P.seg_fw = e->d_seg_fw; P.seg_nf = e->d_seg_nf; P.seg_white = e->d_seg_white;
-    P.ts = e->d_ts; P.key = e->d_key; P.perm = e->d_perm; P.tx = e->d_tx; P.idx = e->d_idx; P.tx_base = e->n_tx; P.scal = e->d_scal;
-    P.plan = e->d_plan; P.plan_stride = (int)(e->seg_cap * MS);
+    const OrderParams P = order_params(e, n, e->d_rounds_in);
     const int M = e->M;
     cudaEvent_t a = get_event(e), b = get_event(e);
     cudaEventRecord(a, e->stream);
@@ -1119,6 +1208,155 @@ int sw_find_order(sw_engine *e, const int32_t *new_c, int n) {
     const int nbatch = e->h_scal[SC_BATCH];
     e->n_tx += nbatch;
     return nbatch;
+}
+
+// Node.decide_fame for B node-views in one call: the fame kernels of every view side by side in one grid (blockIdx.y =
+// view), then the scalars and the first new rounds of all views back in one copy.
+int sw_batch_decide_fame(sw_engine *const *engines, int B, int32_t *new_c_out, int cap, int32_t *count_out) {
+    sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
+    if (!e || cap < 0 || (cap > 0 && !new_c_out) || !count_out) return fail(e, SW_E_ARG, "bad argument");
+    int rc = check_views(engines, B, "sw_batch_decide_fame");
+    if (rc < 0) return rc;
+    for (int v = 0; v < B; v++)
+        if (engines[v]->n_divided == 0)
+            return fail(e, SW_E_ARG, "sw_batch_decide_fame: view %d: no witnesses yet (max() of an empty dict, swirld.py:225)", v);
+    CK(cudaSetDevice(e->device));
+    const int S = SC_COUNT + 1024;                     // per view: the scalars and the new rounds sw_decide_fame copies
+    const size_t pbytes = align256(sizeof(FameParams) * B), sbytes = sizeof(int32_t) * (size_t)S * B;
+    if (views_buffer(e, pbytes + sbytes) < 0) return SW_E_CUDA;
+    FameParams *hP = reinterpret_cast<FameParams *>(e->h_vbuf);
+    for (int v = 0; v < B; v++) hP[v] = fame_params(engines[v]);
+    const FameParams *Pv = reinterpret_cast<const FameParams *>(e->d_vbuf);
+    int32_t *d_st = reinterpret_cast<int32_t *>(e->d_vbuf + pbytes), *h_st = reinterpret_cast<int32_t *>(e->h_vbuf + pbytes);
+    if (views_enter(e, engines, B) < 0) return SW_E_CUDA;
+    CK(cudaMemcpyAsync(e->d_vbuf, e->h_vbuf, sizeof(FameParams) * B, cudaMemcpyHostToDevice, e->stream));
+    e->stats.h2d_bytes += sizeof(FameParams) * B;
+    {
+        // every view gets the CTAs its single call launches (the kernels are latency-bound; spare CTAs exit at once)
+        Span sp(e, 1);
+        if (e->wide) {
+            const int parts = (e->M + FW_THREADS - 1) / FW_THREADS;
+            k_fame_begin_views<<<dim3(1, B), 32, 0, e->stream>>>(Pv);
+            SW_NJ(fame_rounds_wide_views, e, Pv, B, 2 * e->n_sm / parts + 1);
+            k_fame_finish_views<<<dim3(1, B), 1024, 0, e->stream>>>(Pv);
+        } else {
+            k_fame_rounds_views<<<dim3(2 * e->n_sm, B), 256, 0, e->stream>>>(Pv);
+        }
+        k_views_gather<<<B, 256, 0, e->stream>>>(Pv, d_st, S);
+        CK(cudaGetLastError());
+        e->stats.kernel_launches += e->wide ? 4 : 2;
+    }
+    if (views_leave(e, engines, B, h_st, d_st, sbytes) < 0) return SW_E_CUDA;
+    if (e->spans.size() >= 256) fold_spans(e);
+    // per view what sw_decide_fame does after its copy: the host mirror of the scalars, the error the device found, and a
+    // second copy when more new rounds came than the first one held
+    int first_err = SW_OK;
+    for (int v = 0; v < B; v++) {
+        sw_engine *x = engines[v];
+        const int spec = std::min(x->Rcap, 1024);
+        memcpy(x->h_scal, h_st + (size_t)S * v, sizeof(int32_t) * (SC_COUNT + spec));
+        int r = device_error(x);
+        if (r == 0) {
+            const int cnt = x->h_scal[SC_NEWC];
+            if (cnt > cap) r = fail(x, SW_E_ARG, "decide_fame: %d new consensus rounds do not fit cap=%d", cnt, cap);
+            else {
+                if (cnt > spec) {
+                    CK(cudaMemcpyAsync(x->h_newc, x->d_newc, sizeof(int32_t) * cnt, cudaMemcpyDeviceToHost, x->stream));
+                    CK(cudaStreamSynchronize(x->stream));
+                    x->stats.d2h_bytes += sizeof(int32_t) * cnt;
+                }
+                if (cnt > 0) memcpy(new_c_out + (size_t)cap * v, x->h_newc, sizeof(int32_t) * cnt);
+                r = cnt;
+            }
+        }
+        count_out[v] = r;
+        if (r < 0 && first_err == SW_OK) first_err = r;
+    }
+    return first_err;
+}
+
+// Node.find_order for B node-views in one call: the five order kernels of every view with rounds to order side by side
+// (blockIdx.y = view), the views' parameters and rounds in one copy there, their scalars in one copy back.
+int sw_batch_find_order(sw_engine *const *engines, int B, const int32_t *new_c, const int *offsets, int32_t *count_out) {
+    sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
+    if (!e || !offsets || !count_out) return fail(e, SW_E_ARG, "bad argument");
+    int rc = check_views(engines, B, "sw_batch_find_order");
+    if (rc < 0) return rc;
+    if (offsets[0] < 0) return fail(e, SW_E_ARG, "sw_batch_find_order: offsets[0] = %d", offsets[0]);
+    for (int v = 0; v < B; v++)
+        if (offsets[v + 1] < offsets[v])
+            return fail(e, SW_E_ARG, "sw_batch_find_order: offsets[%d] = %d > offsets[%d] = %d", v, offsets[v], v + 1, offsets[v + 1]);
+    const int total = offsets[B] - offsets[0];
+    if (total > 0 && !new_c) return fail(e, SW_E_ARG, "bad argument");
+    std::vector<int32_t> rs(total);
+    if (total > 0) std::copy(new_c + offsets[0], new_c + offsets[B], rs.begin());
+    std::vector<sw_engine *> act;                      // the views with rounds to order
+    std::vector<int> act_v;
+    int maxn = 0;
+    for (int v = 0; v < B; v++) {
+        const int n = offsets[v + 1] - offsets[v];
+        auto b = rs.begin() + (offsets[v] - offsets[0]);
+        std::sort(b, b + n);                                           // sorted(new_c), swirld.py:283
+        for (auto it = b; it != b + n; ++it)
+            if (*it < 0 || *it >= engines[v]->Rcap) return fail(e, SW_E_KEY, "sw_batch_find_order: view %d: unknown round %d", v, *it);
+        if (n > 0) { act.push_back(engines[v]); act_v.push_back(v); maxn = std::max(maxn, n); }
+    }
+    for (int v = 0; v < B; v++) count_out[v] = 0;
+    const int A = (int)act.size();
+    if (A == 0) return SW_OK;
+    CK(cudaSetDevice(e->device));
+    for (int i = 0; i < A; i++) if (order_scratch(act[i], offsets[act_v[i] + 1] - offsets[act_v[i]]) < 0) { e->err = act[i]->err; return SW_E_CUDA; }
+    // [A parameter blocks][the rounds] go over in one copy; [A x SC_COUNT] scalars come back in one
+    const size_t pbytes = sizeof(OrderParams) * A, inbytes = pbytes + sizeof(int32_t) * total, soff = align256(inbytes);
+    const size_t sbytes = sizeof(int32_t) * (size_t)SC_COUNT * A;
+    if (views_buffer(e, soff + sbytes) < 0) return SW_E_CUDA;
+    OrderParams *hP = reinterpret_cast<OrderParams *>(e->h_vbuf);
+    int32_t *h_rounds = reinterpret_cast<int32_t *>(e->h_vbuf + pbytes);
+    const int32_t *d_rounds = reinterpret_cast<const int32_t *>(e->d_vbuf + pbytes);
+    if (total > 0) memcpy(h_rounds, rs.data(), sizeof(int32_t) * total);
+    for (int i = 0; i < A; i++) {
+        const int v = act_v[i];
+        hP[i] = order_params(act[i], offsets[v + 1] - offsets[v], d_rounds + (offsets[v] - offsets[0]));
+    }
+    const OrderParams *Pv = reinterpret_cast<const OrderParams *>(e->d_vbuf);
+    int32_t *d_st = reinterpret_cast<int32_t *>(e->d_vbuf + soff), *h_st = reinterpret_cast<int32_t *>(e->h_vbuf + soff);
+    if (views_enter(e, act.data(), A) < 0) return SW_E_CUDA;
+    CK(cudaMemcpyAsync(e->d_vbuf, e->h_vbuf, inbytes, cudaMemcpyHostToDevice, e->stream));
+    e->stats.h2d_bytes += inbytes;
+    const int M = e->M, MS = e->MS;
+    // every view gets the CTAs its single call launches, sized from the view with the most rounds
+    const int list_ctas = std::max(1, std::min(4 * e->n_sm, (int)(((size_t)maxn * MS + 255) / 256)));
+    cudaEvent_t a = get_event(e), b = get_event(e);
+    cudaEventRecord(a, e->stream);
+    if (e->wide) {
+        k_w_order_rounds_views<<<dim3(maxn, A), 1024, (size_t)3 * M * sizeof(int), e->stream>>>(Pv);
+        k_w_order_cuts_views<<<dim3(1, A), 1024, (size_t)2 * M * sizeof(int), e->stream>>>(Pv);
+        k_w_order_list_views<<<dim3(list_ctas, A), 256, 0, e->stream>>>(Pv);
+        k_w_order_times_views<<<dim3(8 * e->n_sm, A), OW_WARPS * 32, (size_t)OW_WARPS * M * sizeof(u64), e->stream>>>(Pv);
+    } else {
+        k_order_rounds_views<<<dim3(maxn, A), 1024, 0, e->stream>>>(Pv);
+        k_order_cuts_views<<<dim3(1, A), 64, 0, e->stream>>>(Pv);
+        k_order_list_views<<<dim3(list_ctas, A), 256, 0, e->stream>>>(Pv);
+        k_order_times_views<<<dim3(4 * e->n_sm, A), 256, 0, e->stream>>>(Pv);
+    }
+    k_order_sort_views<<<dim3(maxn, A), 1024, 0, e->stream>>>(Pv);
+    k_views_gather<<<A, 32, 0, e->stream>>>(Pv, d_st, SC_COUNT);
+    CK(cudaGetLastError());
+    cudaEventRecord(b, e->stream);
+    e->spans.push_back(TimedSpan{a, b, 2});
+    e->stats.kernel_launches += 6;
+    if (views_leave(e, act.data(), A, h_st, d_st, sbytes) < 0) return SW_E_CUDA;
+    fold_spans(e);
+    int first_err = SW_OK;
+    for (int i = 0; i < A; i++) {
+        sw_engine *x = act[i];
+        memcpy(x->h_scal, h_st + (size_t)SC_COUNT * i, sizeof(int32_t) * SC_COUNT);
+        int r = device_error(x);
+        if (r == 0) { r = x->h_scal[SC_BATCH]; x->n_tx += r; }
+        count_out[act_v[i]] = r;
+        if (r < 0 && first_err == SW_OK) first_err = r;
+    }
+    return first_err;
 }
 
 int sw_members(const sw_engine *e) { return e ? e->M : SW_E_ARG; }

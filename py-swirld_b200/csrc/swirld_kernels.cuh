@@ -199,7 +199,7 @@ __device__ __forceinline__ void fame_collect(const FameParams &P, int max_c, int
     if (tid == 0) { P.scal[SC_NEWC] = s_base; P.scal[SC_MAXC] = max_c; }
 }
 
-__global__ void k_fame_begin(FameParams P) {                    // one warp
+__device__ __forceinline__ void fame_begin_body(const FameParams &P) {     // one warp
     const int lane = threadIdx.x;
     const int mc = fame_max_c(P, lane);
     if (lane == 0) { P.scal[SC_MAXC] = mc; P.scal[SC_NEWC] = 0; }
@@ -207,9 +207,12 @@ __global__ void k_fame_begin(FameParams P) {                    // one warp
     const int max_r = P.scal[SC_MAX_ROUND];
     for (int r = mc + lane; r <= max_r && r < P.Rcap; r += 32) { P.rem[r] = 0; P.done[r] = 0; }
 }
+__global__ void k_fame_begin(FameParams P) { fame_begin_body(P); }
 
-// M <= 64: each candidate round is one CTA's, which writes its rem / done whole
-__global__ void __launch_bounds__(256) k_fame_rounds(FameParams P) {
+// M <= 64: each candidate round is one CTA's, which writes its rem / done whole.  (A template so that each kernel gets
+// its own copy of the body's shared variables: k_fame_rounds then compiles as it did without the views kernel.)
+template <bool VIEWS>
+__device__ __forceinline__ void fame_rounds_body(const FameParams &P) {
     __shared__ u64 sv[2][64];
     __shared__ i64 vsum[2][64];
     __shared__ i64 stake_s[64];
@@ -303,10 +306,10 @@ __global__ void __launch_bounds__(256) k_fame_rounds(FameParams P) {
     if (tid == 0) P.scal[SC_TICKET] = 0;
     fame_collect(P, max_c, max_r);
 }
+__global__ void __launch_bounds__(256) k_fame_rounds(FameParams P) { fame_rounds_body<false>(P); }
 
-__global__ void __launch_bounds__(1024, 1) k_fame_finish(FameParams P) {
-    fame_collect(P, P.scal[SC_MAXC], P.scal[SC_MAX_ROUND]);
-}
+__device__ __forceinline__ void fame_finish_body(const FameParams &P) { fame_collect(P, P.scal[SC_MAXC], P.scal[SC_MAX_ROUND]); }
+__global__ void __launch_bounds__(1024, 1) k_fame_finish(FameParams P) { fame_finish_body(P); }
 
 // ---------------------------------------------------------------- K4: find_order
 struct OrderParams {
@@ -353,7 +356,7 @@ struct OrderParams {
 // A: everything about a consensus round that does not depend on what earlier rounds ordered -- one CTA
 // per round: famous witnesses, whitening XOR, and per member chain the received-threshold `thr` and the
 // reach over ALL famous witnesses (the usual case: none of them is ordered yet).
-__global__ void __launch_bounds__(1024, 1) k_order_rounds(OrderParams P) {
+__device__ __forceinline__ void order_rounds_body(const OrderParams &P) {
     __shared__ int fw[64];
     __shared__ int nf_s;
     __shared__ unsigned ball[2];
@@ -421,12 +424,13 @@ __global__ void __launch_bounds__(1024, 1) k_order_rounds(OrderParams P) {
         PLAN(3)[si * 64 + tid] = ua >= 0 ? P.seq[ua] : -1;
     }
 }
+__global__ void __launch_bounds__(1024, 1) k_order_rounds(OrderParams P) { order_rounds_body(P); }
 
 // B: the only sequential part -- round after round, what each chain still has to give: the events
 // (lastord[c], min(reach, thr)].  A famous witness that an earlier round already ordered does not seed
 // the search (swirld.py:288-289, `f_w & tbd`); then the reach is taken over the others.  One thread per
 // chain; the next round's vectors are fetched while this one is decided.
-__global__ void __launch_bounds__(64) k_order_cuts(OrderParams P) {
+__device__ __forceinline__ void order_cuts_body(const OrderParams &P) {
     __shared__ int lastord_s[64], tbd_s[64], wtot[2];
     const int c = threadIdx.x, lane = c & 31, M = P.M;
     int lo = c < M ? P.lastord[c] : -1;
@@ -475,9 +479,10 @@ __global__ void __launch_bounds__(64) k_order_cuts(OrderParams P) {
     if (c < M) P.lastord[c] = lo;
     if (c == 0) { P.seg_start[P.nrounds] = total; P.scal[SC_BATCH] = total; }
 }
+__global__ void __launch_bounds__(64) k_order_cuts(OrderParams P) { order_cuts_body(P); }
 
 // C: list the ordered events of every (round, chain): from the cut down the self-parent chain
-__global__ void k_order_list(OrderParams P) {
+__device__ __forceinline__ void order_list_body(const OrderParams &P) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < P.nrounds * 64; i += gridDim.x * blockDim.x) {
         const int cnt = PLAN(6)[i];
         if (cnt <= 0) continue;
@@ -490,13 +495,14 @@ __global__ void k_order_list(OrderParams P) {
         }
     }
 }
+__global__ void k_order_list(OrderParams P) { order_list_body(P); }
 
 // Consensus timestamp and sort key of each newly ordered event (swirld.py:295-306):
 // one warp per event, lane = famous witness.  For a witness that sees x the reference
 // walks down the witness's self-parent chain while the ancestor still sees x
 // (:298-302) and takes the timestamp of where it stops (the event before the first
 // seer, or the chain root -- quirk Q10); the lopsided median of :305 (quirk Q11).
-__global__ void __launch_bounds__(256) k_order_times(OrderParams P) {
+__device__ __forceinline__ void order_times_body(const OrderParams &P) {
     const int lane = threadIdx.x & 31;
     const int nbatch = P.scal[SC_BATCH];                 // (left on the device by k_order_cuts: no host round trip)
     const int gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), nw = gridDim.x * (blockDim.x >> 5);
@@ -556,6 +562,7 @@ __global__ void __launch_bounds__(256) k_order_times(OrderParams P) {
     }
     }
 }
+__global__ void __launch_bounds__(256) k_order_times(OrderParams P) { order_times_body(P); }
 
 __device__ __forceinline__ bool order_less(const OrderParams &P, int a, int b) {
     // a, b are batch slots (-1 = padding = +infinity); (ts, white ^ sig) ascending
@@ -575,7 +582,7 @@ __device__ __forceinline__ bool order_less(const OrderParams &P, int a, int b) {
 // One CTA per segment: bitonic sort of the segment's batch slots (padded to a power of
 // two with -1 = +infinity; P.perm holds 2 ints per batch slot so the padding is real),
 // then append to transactions / idx (swirld.py:306-309).
-__global__ void __launch_bounds__(1024) k_order_sort(OrderParams P) {
+__device__ __forceinline__ void order_sort_body(const OrderParams &P) {
     const int si = blockIdx.x;
     const int s0 = P.seg_start[si], cnt = P.seg_start[si + 1] - s0;
     if (cnt <= 0) return;
@@ -602,6 +609,45 @@ __global__ void __launch_bounds__(1024) k_order_sort(OrderParams P) {
         P.tx[P.tx_base + s0 + i] = x;
         P.idx[x] = P.tx_base + s0 + i;
     }
+}
+__global__ void __launch_bounds__(1024) k_order_sort(OrderParams P) { order_sort_body(P); }
+
+// ---------------------------------------------------------------- several node-views per launch
+// sw_batch_decide_fame / sw_batch_find_order run the bodies above for B independent node-views at once (the pattern of
+// k_rounds_batch_views): blockIdx.y is the view, Pv[blockIdx.y] its parameters, staged in shared memory; blockIdx.x and
+// gridDim.x are what they are in a single-view launch, so the grid-stride loops and k_fame_rounds' last-CTA ticket count
+// one view's CTAs.  The order grids are sized from the view with the most rounds: a CTA beyond its view's rounds exits.
+template <typename T>
+__device__ __forceinline__ const T &view_params(const T *Pv) {
+    __shared__ T Ps;
+    if (threadIdx.x == 0) Ps = Pv[blockIdx.y];
+    __syncthreads();
+    return Ps;
+}
+
+__global__ void k_fame_begin_views(const FameParams *Pv) { fame_begin_body(view_params(Pv)); }
+__global__ void __launch_bounds__(256) k_fame_rounds_views(const FameParams *Pv) { fame_rounds_body<true>(view_params(Pv)); }
+__global__ void __launch_bounds__(1024, 1) k_fame_finish_views(const FameParams *Pv) { fame_finish_body(view_params(Pv)); }
+
+__global__ void __launch_bounds__(1024, 1) k_order_rounds_views(const OrderParams *Pv) {
+    const OrderParams &P = view_params(Pv);
+    if ((int)blockIdx.x < P.nrounds) order_rounds_body(P);
+}
+__global__ void __launch_bounds__(64) k_order_cuts_views(const OrderParams *Pv) { order_cuts_body(view_params(Pv)); }
+__global__ void k_order_list_views(const OrderParams *Pv) { order_list_body(view_params(Pv)); }
+__global__ void __launch_bounds__(256) k_order_times_views(const OrderParams *Pv) { order_times_body(view_params(Pv)); }
+__global__ void __launch_bounds__(1024) k_order_sort_views(const OrderParams *Pv) {
+    const OrderParams &P = view_params(Pv);
+    if ((int)blockIdx.x < P.nrounds) order_sort_body(P);
+}
+
+// the first n ints of every view's scalar block (SC_*, and for decide_fame the new rounds behind them) into row v of
+// one staging array: one device-to-host copy brings back what B single calls copy one by one
+template <typename T>
+__global__ void k_views_gather(const T *Pv, int32_t *out, int n) {
+    const T &P = Pv[blockIdx.x];
+    const int m = min(n, SC_COUNT + P.Rcap);               // (the new rounds' array holds Rcap entries)
+    for (int i = threadIdx.x; i < m; i += blockDim.x) out[(size_t)blockIdx.x * n + i] = P.scal[i];
 }
 
 __global__ void k_fill_i32(int32_t *p, int32_t v, size_t n) {

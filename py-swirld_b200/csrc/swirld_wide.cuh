@@ -636,7 +636,7 @@ __device__ __forceinline__ i64 w_wsum(const unsigned (&m)[NJ], bool unit, const 
 // k_fame_begin cleared.
 #define FW_THREADS 256
 template <int NJ>
-__global__ void __launch_bounds__(FW_THREADS) k_w_fame_rounds(FameParams P) {
+__device__ __forceinline__ void w_fame_rounds_body(const FameParams &P) {
     extern __shared__ int fw_smem[];
     unsigned *sS = reinterpret_cast<unsigned *>(fw_smem);            // [32][NJ] staged voter sets
     int *vw = fw_smem + 32 * NJ;                                     // [32] voter present
@@ -724,13 +724,15 @@ __global__ void __launch_bounds__(FW_THREADS) k_w_fame_rounds(FameParams P) {
         if (tid == 0) { if (left) atomicAdd(&P.rem[r], left); if (dn) P.done[r] = 1; }
     }
 }
+template <int NJ>
+__global__ void __launch_bounds__(FW_THREADS) k_w_fame_rounds(FameParams P) { w_fame_rounds_body<NJ>(P); }
 
 // ------------------------------------------------------------------ find_order (swirld.py:280-311)
 // Same plan as swirld_kernels.cuh (A per round, B sequential cuts, C listing, times, sort) with per-round
 // arrays of M entries (OrderParams.seg_fw / plan strides are M instead of 64).
 #define WPLAN(k) (P.plan + (size_t)(k) * P.plan_stride)
 
-__global__ void __launch_bounds__(1024, 1) k_w_order_rounds(OrderParams P) {
+__device__ __forceinline__ void w_order_rounds_body(const OrderParams &P) {
     extern __shared__ int ow_smem[];
     i64 *st = reinterpret_cast<i64 *>(ow_smem);          // [M] stake of fw[i]'s creator
     int *fw = ow_smem + 2 * P.M;                         // [M]
@@ -795,8 +797,9 @@ __global__ void __launch_bounds__(1024, 1) k_w_order_rounds(OrderParams P) {
         WPLAN(3)[(size_t)si * M + c] = U >= 0 ? P.seq[U] : -1;
     }
 }
+__global__ void __launch_bounds__(1024, 1) k_w_order_rounds(OrderParams P) { w_order_rounds_body(P); }
 
-__global__ void __launch_bounds__(1024) k_w_order_cuts(OrderParams P) {
+__device__ __forceinline__ void w_order_cuts_body(const OrderParams &P) {
     extern __shared__ int oc_smem[];
     int *lastord_s = oc_smem, *tbd_s = oc_smem + P.M;
     __shared__ int wtot[32];
@@ -844,8 +847,9 @@ __global__ void __launch_bounds__(1024) k_w_order_cuts(OrderParams P) {
     if (c < M) P.lastord[c] = lo;
     if (c == 0) { P.seg_start[P.nrounds] = total; P.scal[SC_BATCH] = total; }
 }
+__global__ void __launch_bounds__(1024) k_w_order_cuts(OrderParams P) { w_order_cuts_body(P); }
 
-__global__ void k_w_order_list(OrderParams P) {
+__device__ __forceinline__ void w_order_list_body(const OrderParams &P) {
     const size_t tot = (size_t)P.nrounds * P.M;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < tot; i += (size_t)gridDim.x * blockDim.x) {
         const int cnt = WPLAN(6)[i];
@@ -859,6 +863,7 @@ __global__ void k_w_order_list(OrderParams P) {
         }
     }
 }
+__global__ void k_w_order_list(OrderParams P) { w_order_list_body(P); }
 
 __device__ __forceinline__ u64 dbl_key(double d) {       // order-preserving image of a double
     const u64 b = (u64)__double_as_longlong(d);
@@ -884,7 +889,7 @@ __device__ __forceinline__ u64 warp_select(const u64 *keys, int n, int k, int la
 }
 
 #define OW_WARPS 4
-__global__ void __launch_bounds__(OW_WARPS * 32) k_w_order_times(OrderParams P) {
+__device__ __forceinline__ void w_order_times_body(const OrderParams &P) {
     extern __shared__ u64 ot_smem[];
     const int nbatch = P.scal[SC_BATCH];                 // (left on the device by k_w_order_cuts: no host round trip)
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, M = P.M;
@@ -926,3 +931,15 @@ __global__ void __launch_bounds__(OW_WARPS * 32) k_w_order_times(OrderParams P) 
         }
     }
 }
+__global__ void __launch_bounds__(OW_WARPS * 32) k_w_order_times(OrderParams P) { w_order_times_body(P); }
+
+// several node-views per launch (swirld_kernels.cuh, view_params): blockIdx.y is the view
+template <int NJ>
+__global__ void __launch_bounds__(FW_THREADS) k_w_fame_rounds_views(const FameParams *Pv) { w_fame_rounds_body<NJ>(view_params(Pv)); }
+__global__ void __launch_bounds__(1024, 1) k_w_order_rounds_views(const OrderParams *Pv) {
+    const OrderParams &P = view_params(Pv);
+    if ((int)blockIdx.x < P.nrounds) w_order_rounds_body(P);
+}
+__global__ void __launch_bounds__(1024) k_w_order_cuts_views(const OrderParams *Pv) { w_order_cuts_body(view_params(Pv)); }
+__global__ void k_w_order_list_views(const OrderParams *Pv) { w_order_list_body(view_params(Pv)); }
+__global__ void __launch_bounds__(OW_WARPS * 32) k_w_order_times_views(const OrderParams *Pv) { w_order_times_body(view_params(Pv)); }

@@ -26,6 +26,7 @@ SYMBOLS = [
     "sw_get_witness_table", "sw_get_consensus", "sw_get_transactions", "sw_get_idx", "sw_get_height",
     "sw_sync", "sw_stats", "sw_flush_l2", "sw_version", "sw_debug_counters", "sw_peer_handle", "sw_peer_connect",
     "sw_save", "sw_load", "sw_members", "sw_ingest", "sw_lookup", "sw_batch_divide_rounds",
+    "sw_batch_decide_fame", "sw_batch_find_order",
 ]
 
 
@@ -88,6 +89,8 @@ def load_library(path: str = LIB_PATH):
     L.sw_ingest.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp]
     L.sw_lookup.argtypes = [vp, i32, vp, vp]
     L.sw_batch_divide_rounds.argtypes = [vp, i32, vp, vp]
+    L.sw_batch_decide_fame.argtypes = [vp, i32, vp, i32, vp]
+    L.sw_batch_find_order.argtypes = [vp, i32, vp, vp, vp]
     L.sw_save.argtypes = [vp, C.c_char_p]
     L.sw_load.argtypes = [C.c_char_p, i32, i32, P(vp)]
     _lib = L
@@ -143,14 +146,18 @@ class Engine:
         except Exception:
             pass
 
+    def _error(self, rc):
+        """The exception the single call would raise for the SW_E_* code rc."""
+        msg = (self._lib.sw_last_error(self._h) or b"").decode()
+        if rc == -2:
+            return IndexError(msg)
+        if rc == -3:
+            return KeyError(msg)
+        return EngineError(rc, msg)
+
     def _chk(self, rc):
         if rc < 0:
-            msg = (self._lib.sw_last_error(self._h) or b"").decode()
-            if rc == -2:
-                raise IndexError(msg)
-            if rc == -3:
-                raise KeyError(msg)
-            raise EngineError(rc, msg)
+            raise self._error(rc)
         return rc
 
     def reset(self):
@@ -319,6 +326,61 @@ def batch_divide_rounds(engines, firsts, counts):
     f = np.ascontiguousarray(firsts, np.int32)
     n = np.ascontiguousarray(counts, np.int32)
     engines[0]._chk(engines[0]._lib.sw_batch_divide_rounds(C.cast(arr, C.c_void_p), B, _ptr(f), _ptr(n)))
+
+
+def _handles(engines):
+    arr = (C.c_void_p * len(engines))(*[e._h for e in engines])
+    return C.cast(arr, C.c_void_p)
+
+
+def _per_view(what, engines, results, counts):
+    """Raise the views' own failures, after the whole batch has run, as one ExceptionGroup: each member is what the
+    single call would have raised, with .view set; the group's .results holds every view's result (None: failed)."""
+    errs = []
+    for v, rc in enumerate(counts):
+        if rc < 0:
+            ex = engines[v]._error(int(rc))
+            ex.view = v
+            errs.append(ex)
+            results[v] = None
+    if errs:
+        g = ExceptionGroup("%s: %d of %d views failed" % (what, len(errs), len(engines)), errs)
+        g.results = results
+        raise g
+    return results
+
+
+def batch_decide_fame(engines):
+    """sw_batch_decide_fame: decide_fame of several node-views (one member count, one kernel family, one device) in one
+    call.  Returns each view's new consensus rounds, as Engine.decide_fame does.  Argument errors raise at once;
+    failures the device finds in some views raise as an ExceptionGroup after every view has run (see _per_view)."""
+    B = len(engines)
+    if B == 0:
+        return []
+    cap = max(max(64, e.n_divided + 2) for e in engines)      # as Engine.decide_fame chooses it, for the largest view
+    out = np.empty((B, cap), np.int32)
+    cnt = np.zeros(B, np.int32)
+    rc = engines[0]._lib.sw_batch_decide_fame(_handles(engines), B, _ptr(out), cap, _ptr(cnt))
+    if rc < 0 and not (cnt < 0).any():
+        engines[0]._chk(rc)                # refused as a whole: nothing ran, count_out was not written
+    return _per_view("batch_decide_fame", engines, [out[v, :max(0, int(n))].tolist() for v, n in enumerate(cnt)], cnt)
+
+
+def batch_find_order(engines, new_cs):
+    """sw_batch_find_order: find_order(new_cs[v]) of every view in one call.  Returns the events each view appended
+    to its order; errors as batch_decide_fame."""
+    B = len(engines)
+    assert len(new_cs) == B
+    if B == 0:
+        return []
+    flat = np.ascontiguousarray(np.concatenate([np.asarray(sorted(nc), np.int32) for nc in new_cs]), np.int32)
+    offs = np.zeros(B + 1, np.int32)
+    offs[1:] = np.cumsum([len(nc) for nc in new_cs])
+    cnt = np.zeros(B, np.int32)
+    rc = engines[0]._lib.sw_batch_find_order(_handles(engines), B, _ptr(flat), _ptr(offs), _ptr(cnt))
+    if rc < 0 and not (cnt < 0).any():
+        engines[0]._chk(rc)
+    return _per_view("batch_find_order", engines, [int(n) for n in cnt], cnt)
 
 
 def run_engine(tr, K, stake=None, coin_period=6, device=0, find_order=True):
