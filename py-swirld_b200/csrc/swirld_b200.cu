@@ -47,11 +47,12 @@ struct sw_engine {
     std::vector<int32_t> h_creator, h_head, h_count;
     int32_t *h_height = nullptr, *h_seq = nullptr;   // pinned, cap entries: sources of asynchronous copies
     uint8_t *h_stale = nullptr;                      // pinned: the other-parent is not its member's latest event
-    // M <= 64: h_count as it stood after every SNAP-th event and at the end of every append, so that the per-member
-    // counts of any chunk cost O(M) plus fewer than SNAP events (round_batch_prep)
+    // h_count as it stood after every SNAP-th event and at the end of every append not yet divided, so that the
+    // per-member counts of any chunk cost O(M) plus fewer than SNAP events (chunk_prep)
     static constexpr int SNAP = 4096;
     std::vector<int> snap_at;                        // event counts of the snapshots, ascending
     std::vector<int32_t> snap_cnt;                   // [snapshot][M]
+    size_t snap_kept = 0;                            // snapshots [0, snap_kept) are all SNAP-event ones
     cudaStream_t copy_stream = nullptr;              // sw_append's copies run beside the kernels of earlier chunks
     struct PendingAppend { int base; cudaEvent_t done; };
     std::vector<PendingAppend> appends;              // copies (+ eager can_see scans) the compute stream has not waited for yet
@@ -71,7 +72,6 @@ struct sw_engine {
     int32_t *d_rsg = nullptr, *d_rccont = nullptr;
     size_t rsg_cap = 0;           // events d_rsg holds
     bool rc_ok = false;           // a 16-CTA cluster with its shared memory can be resident on this device
-    bool rc_mb = true;            // its exchanges by st.async + mbarrier (SW_RC_MB=0: plain stores + cluster barriers)
     int rc_min_n = 2048;          // shorter chunks go to the grid-wide kernel directly
     RcParams *d_rcviews = nullptr;
     RbParams *d_views = nullptr;  // sw_batch_divide_rounds: the views' parameters (owned by the first engine of a batch)
@@ -127,7 +127,7 @@ struct sw_engine {
     uint8_t *h_stage = nullptr, *d_stage = nullptr;
     cudaEvent_t stage_ev[STAGE_SLOTS] = {nullptr};
     int stage_next = 0;
-    int stream_n = 16;            // divide_rounds calls of at most this many events take the one-launch path (SW_STREAM_N)
+    static constexpr int STREAM_N = 16;              // divide_rounds calls of at most this many events take the one-launch path
     int32_t *h_scal = nullptr;    // pinned
     int32_t *h_newc = nullptr;    // pinned, Rcap: right behind h_scal (one copy brings both back)
     cudaStream_t stream = nullptr;
@@ -253,7 +253,7 @@ int reset_state(sw_engine *e, bool keep_events = false) {
         e->n_events = 0;
         std::fill(e->h_head.begin(), e->h_head.end(), -1);
         std::fill(e->h_count.begin(), e->h_count.end(), 0);
-        e->snap_at.clear(); e->snap_cnt.clear();
+        e->snap_at.clear(); e->snap_cnt.clear(); e->snap_kept = 0;
     }
     memset(e->h_scal, 0, sizeof(int32_t) * SC_COUNT);
     return 0;
@@ -273,9 +273,7 @@ int cansee_scan(sw_engine *e, cudaStream_t st, int upto) {
     C.meta = e->d_cs_meta; C.wr = e->d_cs_wr; C.xb = e->d_cs_xb; C.last = e->d_cs_last; C.Qtab = e->d_cs_Q;
     C.carry = e->d_cs_carry; C.slow_list = e->d_cs_slow; C.slow_cnt = e->d_cs_slowcnt; C.sflag = e->d_cs_sflag; C.xlist = e->d_cs_xlist; C.slow_blk = e->d_cs_slowblk; C.blk_cnt = e->d_cs_blkcnt;
     cudaEvent_t a = get_event(e), b = get_event(e);
-    int small_n = 24;
-    if (const char *v = getenv("SW_CS_SMALL")) small_n = atoi(v);
-    if (n <= small_n) {                                // the reference's own cadence: a handful of events per call
+    if (n <= 24) {                                     // the reference's own cadence: a handful of events per call
         cudaEventRecord(a, st);
         k_cs_small<<<1, std::min(1024, (M + 31) / 32 * 32), 0, st>>>(C);
         cudaEventRecord(b, st);
@@ -286,9 +284,8 @@ int cansee_scan(sw_engine *e, cudaStream_t st, int upto) {
         return 0;
     }
     // block length: >= 16 (32 above 64 members) events per member and block, so that nearly every member's last event of a
-    // block sees every block-start head (then the finality check passes; the rest goes through the waves); SW_CS_B overrides
+    // block sees every block-start head (then the finality check passes; the rest goes through the waves)
     int B = std::max(e->cs_min_B, std::min((M <= 64 ? 16 : 32) * M, 1 << 15));      // (above 64 members seeing every head takes more events per member)
-    if (const char *v = getenv("SW_CS_B")) B = std::max(e->cs_min_B, atoi(v));
     B = (B + 3) & ~3;
     C.B = B;
     C.first_al = first & ~3;
@@ -309,11 +306,9 @@ int cansee_scan(sw_engine *e, cudaStream_t st, int upto) {
             if (best < 0 || waves < best) { best = waves; CT = ct; }
         }
     }
-    if (const char *v = getenv("SW_CS_CT")) { const int x = atoi(v); if (x == 8 || x == 16 || x == 32) CT = x; }
     C.CT = CT;
     int tile_lo = 0, tile_hi = (M + CT - 1) / CT;
-    bool shard = e->nranks > 1;
-    if (const char *v = getenv("SW_CS_SHARD")) shard = shard && atoi(v) != 0;       // (0: every rank computes the whole table itself)
+    const bool shard = e->nranks > 1;
     if (shard) {                                          // the column tiles of this rank; every rank stores into every table
         const int nt = tile_hi;
         tile_lo = (int)((long long)nt * e->rank / e->nranks); tile_hi = (int)((long long)nt * (e->rank + 1) / e->nranks);
@@ -376,6 +371,25 @@ void push_snapshot(sw_engine *e, int at, const std::vector<int32_t> &cnt) {
     e->snap_cnt.insert(e->snap_cnt.end(), cnt.begin(), cnt.end());
 }
 
+// the snapshot at the end of an append.  The earlier end-of-append ones below n_divided go first: divides only go
+// forward, and after sw_rewind the SNAP-event ones keep counts_at exact.  So snapshots cost memory per event, not per
+// append (4 KB per append at M = 1024 otherwise).
+void push_append_snapshot(sw_engine *e) {
+    if (!e->snap_at.empty() && e->snap_at.back() == e->n_events) return;     // (the append ended on a SNAP-event one)
+    const int M = e->M;
+    size_t k = e->snap_kept, i = k;
+    for (; i < e->snap_at.size() && e->snap_at[i] < e->n_divided; i++)
+        if (e->snap_at[i] % sw_engine::SNAP == 0) {
+            e->snap_at[k] = e->snap_at[i];
+            std::copy_n(e->snap_cnt.begin() + i * M, M, e->snap_cnt.begin() + k * M);
+            k++;
+        }
+    e->snap_at.erase(e->snap_at.begin() + k, e->snap_at.begin() + i);
+    e->snap_cnt.erase(e->snap_cnt.begin() + k * M, e->snap_cnt.begin() + i * M);
+    e->snap_kept = k;
+    push_snapshot(e, e->n_events, e->h_count);
+}
+
 // events of each member among the first x appended events: the nearest snapshot at or below x, then the rest one by one
 void counts_at(const sw_engine *e, int x, int32_t *out) {
     const int M = e->M;
@@ -390,46 +404,73 @@ void counts_at(const sw_engine *e, int x, int32_t *out) {
     for (int i = from; i < x; i++) out[e->h_creator[i]]++;
 }
 
-// rounds of the chunk by the cooperative round-batch kernel (swirld_rounds.cuh), M <= 64: parameters + the kernel that
-// groups the chunk's events by creator and, for the cluster round kernel (`rows`), writes their seq-space rows
-// (`grid` = CTAs this view's round kernel will run on)
-int round_batch_prep(sw_engine *e, int first, int n, int grid, bool rows, RbParams &R, int min_L = 1) {
-    R = RbParams{};
+// d_rbmeta, one layout for both kernel families (MP = max(M, 64) members)
+struct RbMeta {
+    int32_t *ccnt, *cmin, *coff;  // [MP], [MP], [MP + 1]: the chunk's per-member counts, smallest seqs, offsets (k_rb_prep)
+    unsigned *bar;                // grid barrier counter of the round kernel
+    int32_t *wcnt;                // witnesses of the chunk (k_rb_finish)
+    unsigned *ticket;             // [3] k_rounds_wide's work counters
+};
+
+RbMeta rb_meta(const sw_engine *e) {
+    int32_t *m = e->d_rbmeta;
+    const int MP = e->MP;
+    return RbMeta{m, m + MP, m + 2 * MP, reinterpret_cast<unsigned *>(m + 3 * MP + 8), m + 3 * MP + 9,
+                  reinterpret_cast<unsigned *>(m + 3 * MP + 12)};
+}
+
+// what both kernel families read of the round-batch parameters: the chunk, its grouping by creator (k_rb_prep) and
+// the pass after the round kernel (k_rb_finish)
+RbParams chunk_params(const sw_engine *e, int first, int n) {
+    RbParams R{};
     R.M = e->M; R.first = first; R.n = n; R.Rcap = e->Rcap;
-    R.L = std::max(std::min(min_L, RB_LMAX), std::min(RB_LMAX, grid * (RB_THREADS / 32) / e->M));
-    R.maxmiss = RB_MAXMISS;
-    R.epoch = ++e->rb_epoch;
-    if (const char *v = getenv("SW_RB_L")) R.L = std::max(1, std::min(R.L, atoi(v)));          // tuning knobs
-    if (const char *v = getenv("SW_RB_MAXMISS")) R.maxmiss = std::max(0, atoi(v));
     R.row = e->d_row; R.p0 = e->d_p0; R.creator = e->d_creator; R.seq = e->d_seq; R.round = e->d_round;
-    R.Wf = e->d_Wf; R.sc = e->d_sc; R.cev = e->d_cev;
-    R.ccnt = e->d_rbmeta; R.cmin = e->d_rbmeta + 64; R.coff = e->d_rbmeta + 128; R.bar = reinterpret_cast<unsigned *>(e->d_rbmeta + 224);
-    R.ctot = e->d_rbtot; R.gchain = e->d_gchain;
-    R.res = e->d_res; R.stake = e->d_stake; R.tot2 = 2 * e->tot; R.scal = e->d_scal;
-    R.wit = e->d_wit; R.W = e->d_W; R.SM = e->d_SM; R.dbg = e->d_dbg;
-    R.wlist = e->d_cev + e->cap; R.wcnt = e->d_rbmeta + 225;
-    // the chunk's per-member counts from the host mirror: [first, first+n) holds seqs [lo[c], hi[c]) of member c
-    RbChunk K;
-    int32_t lo[64], hi[64];
-    counts_at(e, first, lo);
-    counts_at(e, first + n, hi);
+    R.cev = e->d_cev; R.ctot = e->d_rbtot; R.gchain = e->d_gchain; R.wit = e->d_wit; R.W = e->d_W;
+    const RbMeta m = rb_meta(e);
+    R.ccnt = m.ccnt; R.cmin = m.cmin; R.coff = m.coff; R.bar = m.bar;
+    R.wlist = e->d_cev + e->cap; R.wcnt = m.wcnt;
+    return R;
+}
+
+// the chunk's events grouped by creator (k_rb_prep) from the per-member counts of the host mirror: [first, first+n)
+// holds seqs [lo[c], hi[c]) of member c.  `rsg` (M <= 64): also the seq-space rows of the cluster round kernel.
+template <int CM>
+int chunk_prep(sw_engine *e, const RbParams &R, int32_t *rsg) {
+    RbChunk<CM> K;
+    int32_t lo[CM];
+    counts_at(e, R.first, lo);
+    counts_at(e, R.first + R.n, K.ctot);
     int o = 0;
-    for (int c = 0; c < 64; c++) {
-        const int cnt = c < e->M ? hi[c] - lo[c] : 0;
-        K.ccnt[c] = cnt; K.cmin[c] = cnt > 0 ? lo[c] : 0x7f7f7f7f; K.ctot[c] = c < e->M ? hi[c] : 0;
+    for (int c = 0; c < CM; c++) {
+        const int cnt = c < e->M ? K.ctot[c] - lo[c] : 0;
+        K.ccnt[c] = cnt; K.cmin[c] = cnt > 0 ? lo[c] : 0x7f7f7f7f;
+        if (c >= e->M) K.ctot[c] = 0;
         K.coff[c] = o; o += cnt;
     }
-    K.coff[64] = o;
+    K.coff[CM] = o;
+    k_rb_prep<CM><<<std::max(1, std::min(8 * e->n_sm, (R.n + 7) / 8)), 256, 0, e->stream>>>(R, K, rsg);
+    CK(cudaGetLastError());
+    e->stats.kernel_launches += 1;
+    return 0;
+}
+
+// rounds of the chunk by the cooperative round-batch kernel (swirld_rounds.cuh), M <= 64: parameters + the grouping of
+// the chunk, with the seq-space rows for the cluster round kernel (`rows`)
+// (`grid` = CTAs this view's round kernel will run on)
+int round_batch_prep(sw_engine *e, int first, int n, int grid, bool rows, RbParams &R, int min_L = 1) {
+    R = chunk_params(e, first, n);
+    R.L = std::max(std::min(min_L, RB_LMAX), std::min(RB_LMAX, grid * (RB_THREADS / 32) / e->M));
+    R.epoch = ++e->rb_epoch;
+    R.Wf = e->d_Wf; R.sc = e->d_sc;
+    R.res = e->d_res; R.stake = e->d_stake; R.tot2 = 2 * e->tot; R.scal = e->d_scal;
+    R.SM = e->d_SM; R.dbg = e->d_dbg;
     if (rows && (size_t)n > e->rsg_cap) {
         if (e->d_rsg) { CK(cudaStreamSynchronize(e->stream)); CK(cudaFree(e->d_rsg)); e->d_rsg = nullptr; e->rsg_cap = 0; }
         const size_t want = std::min<size_t>((size_t)e->cap, std::max<size_t>((size_t)n, 1 << 16));
         CK(dalloc(&e->d_rsg, want * 64));
         e->rsg_cap = want;
     }
-    k_rb_prep<<<std::max(1, std::min(8 * e->n_sm, (n + 7) / 8)), 256, 0, e->stream>>>(R, K, rows ? e->d_rsg : nullptr);
-    CK(cudaGetLastError());
-    e->stats.kernel_launches += 1;
-    return 0;
+    return chunk_prep<64>(e, R, rows ? e->d_rsg : nullptr);
 }
 
 // what follows the round kernel: ring of recent events, witness flags / table / list, seen-masks, strongly-seen sets
@@ -463,10 +504,7 @@ void rc_launch_config(cudaLaunchConfig_t &cfg, cudaLaunchAttribute *at, int clus
 // event record costs the stream a few microseconds)
 template <int NC, bool UNIT>
 int divide_round_batch(sw_engine *e, int first, int n, cudaEvent_t start) {
-    // a few SMs stay free for the can_see scan of the next chunk, which runs beside this kernel (SW_RB_FREE_SMS)
-    int free_sms = 16;
-    if (const char *v = getenv("SW_RB_FREE_SMS")) free_sms = std::max(0, atoi(v));
-    const int grid = std::max(e->n_sm / 2, e->n_sm - free_sms);
+    const int grid = std::max(e->n_sm / 2, e->n_sm - 16);       // 16 SMs stay free for the can_see scan of the next chunk
     const bool rc = e->rc_ok && n >= e->rc_min_n;
     RbParams R;
     void *args[] = {(void *)&R};
@@ -479,8 +517,7 @@ int divide_round_batch(sw_engine *e, int first, int n, cudaEvent_t start) {
             cudaLaunchConfig_t cfg;
             cudaLaunchAttribute at[1];
             rc_launch_config(cfg, at, 1, e->stream);
-            if (e->rc_mb) CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster<UNIT, true>, Q));
-            else CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster<UNIT, false>, Q));
+            CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster<UNIT>, Q));
             R.cont = e->d_rccont;
             e->stats.kernel_launches += 1;
             e->stats.rounds_cluster_launches += 1;
@@ -499,34 +536,25 @@ size_t rounds_wide_smem(int M) { return (size_t)(2 * M + 16 * M + 1 + 32 + (RW_T
 template <int NJ>
 int divide_rounds_wide(sw_engine *e, int first, int n) {
     const int M = e->M;
+    const RbParams T = chunk_params(e, first, n);       // the grouping and the finish kernel shared with the M <= 64 path
+    if (chunk_prep<SW_MAX_MEMBERS>(e, T, nullptr) < 0) return SW_E_CUDA;
     RwParams R{};
     R.M = M; R.first = first; R.n = n; R.Rcap = e->Rcap;
     const int grid = e->n_sm;
     const int nw = grid * (RW_THREADS / 32);
-    const int nown = (M + e->nranks - 1) / e->nranks;
     // events per member below a step's frontier: about three tests per warp and step, never more than half a window
     R.L = std::max(1, std::min(RW_LMAX / 2, 3 * nw * e->nranks / std::max(1, M)));
-    (void)nown;
-    if (const char *v = getenv("SW_RW_L")) R.L = std::max(1, std::min(RW_LMAX, atoi(v)));
     R.epoch = ++e->rb_epoch;
     R.row = e->d_row; R.p0 = e->d_p0; R.creator = e->d_creator; R.seq = e->d_seq; R.round = e->d_round;
-    R.Wf = e->d_Wf; R.scw = e->d_scw; R.sctag = e->d_sctag; R.cev = e->d_cev;
-    R.ccnt = e->d_rbmeta; R.cmin = e->d_rbmeta + M; R.coff = e->d_rbmeta + 2 * M; R.bar = reinterpret_cast<unsigned *>(e->d_rbmeta + 3 * M + 8);
-    int32_t *wcnt = e->d_rbmeta + 3 * M + 9, *wlist = e->d_cev + e->cap;
-    R.ctot = e->d_rbtot; R.gchain = e->d_gchain; R.hitmin = e->d_hitmin; R.ticket = reinterpret_cast<unsigned *>(e->d_rbmeta + 3 * M + 12);
+    R.Wf = e->d_Wf; R.scw = e->d_scw; R.sctag = e->d_sctag; R.cev = T.cev;
+    R.cmin = T.cmin; R.coff = T.coff; R.bar = T.bar; R.ticket = rb_meta(e).ticket;
+    R.ctot = T.ctot; R.gchain = T.gchain; R.hitmin = e->d_hitmin;
     R.stake = e->d_stake; R.tot2 = 2 * e->tot; R.unit = e->unit ? 1 : 0; R.scal = e->d_scal; R.dbg = e->d_dbg;
     R.rank = e->rank; R.nranks = e->nranks; R.xstep = e->d_xstep;
     for (int p = 0; p < e->nranks && p < 8; p++) {
         R.xflag[p] = reinterpret_cast<unsigned *>(e->x_peer[p]);
         R.xhit[p] = reinterpret_cast<u64 *>(reinterpret_cast<char *>(e->x_peer[p]) + 256);
     }
-    CK(cudaMemsetAsync(R.ccnt, 0, sizeof(int32_t) * M, e->stream));
-    CK(cudaMemsetAsync(R.cmin, 0x7f, sizeof(int32_t) * M, e->stream));
-    const int blocks = std::max(1, std::min(2 * e->n_sm, (n + 255) / 256));
-    k_rw_count<<<blocks, 256, 0, e->stream>>>(R);
-    k_rw_offsets<<<1, 1024, 0, e->stream>>>(R, wcnt);
-    k_rw_scatter<<<blocks, 256, 0, e->stream>>>(R);
-    CK(cudaGetLastError());
     const size_t smem = rounds_wide_smem(M);
     CK(cudaFuncSetAttribute(k_rounds_wide<NJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     void *args[] = {(void *)&R};
@@ -537,23 +565,19 @@ int divide_rounds_wide(sw_engine *e, int first, int n) {
         cudaEventRecord(b, e->stream);
         e->spans.push_back(TimedSpan{a, b, 4});
     }
-    RbParams T{};                                      // the finish kernels shared with the M <= 64 path
-    T.M = M; T.first = first; T.n = n; T.Rcap = e->Rcap; T.p0 = e->d_p0; T.creator = e->d_creator; T.seq = e->d_seq;
-    T.round = e->d_round; T.ctot = e->d_rbtot; T.gchain = e->d_gchain; T.wit = e->d_wit; T.W = e->d_W;
-    T.wlist = wlist; T.wcnt = wcnt;
-    k_rb_finish<<<blocks, 256, 0, e->stream>>>(T);
+    k_rb_finish<<<std::max(1, std::min(2 * e->n_sm, (n + 255) / 256)), 256, 0, e->stream>>>(T);
     k_w_seenmask<NJ><<<std::max(1, std::min(8 * e->n_sm, (n + 7) / 8)), 256, 0, e->stream>>>(M, first, n, e->Rcap, e->d_row, e->d_round, e->d_W, e->d_SMw);
     CK(cudaGetLastError());
     StrongParams Q{};
     Q.M = M; Q.first = first; Q.n = n; Q.Rcap = e->Rcap; Q.creator = e->d_creator; Q.row = e->d_row;
     Q.round = e->d_round; Q.wit = e->d_wit; Q.stake = e->d_stake; Q.tot2 = 2 * e->tot;
-    Q.coin = e->d_coin; Q.sig = e->d_sig; Q.unit = e->unit ? 1 : 0; Q.list = wlist; Q.list_n = wcnt;
+    Q.coin = e->d_coin; Q.sig = e->d_sig; Q.unit = e->unit ? 1 : 0; Q.list = T.wlist; Q.list_n = T.wcnt;
     Q.SMw = e->d_SMw; Q.Sw = e->d_Sw;
     const size_t ssm = (size_t)(2 * M + 8 * M) * sizeof(int);
     CK(cudaFuncSetAttribute(k_w_strong<NJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssm));
     k_w_strong<NJ><<<std::max(1, std::min(4 * e->n_sm, (n + 7) / 8)), 256, ssm, e->stream>>>(Q);
     CK(cudaGetLastError());
-    e->stats.kernel_launches += 7;
+    e->stats.kernel_launches += 4;
     return 0;
 }
 
@@ -667,16 +691,9 @@ int views_leave(sw_engine *e, sw_engine *const *views, int B, void *h_dst, const
     return 0;
 }
 
-}  // namespace
-
-extern "C" {
-
-int sw_version(void) { return 202; }
-
-const char *sw_last_error(const sw_engine *e) { return e ? e->err.c_str() : g_create_error.c_str(); }
-
-int sw_create(int M, int capacity_events, const int64_t *stake, int coin_period, int device,
-              sw_engine **out) {
+// sw_create and sw_load: `wide` selects the any-M kernels (swirld_wide.cuh), required above 64 members.  Nothing here
+// changes state that other engines of the process share.
+int create(int M, int capacity_events, const int64_t *stake, int coin_period, int device, bool wide, sw_engine **out) {
     sw_engine *e = nullptr;
     if (!out) return fail(e, SW_E_ARG, "out is NULL");
     *out = nullptr;
@@ -688,8 +705,7 @@ int sw_create(int M, int capacity_events, const int64_t *stake, int coin_period,
     if (device < 0 || device >= ndev) return fail(e, SW_E_ARG, "device %d out of range (%d devices)", device, ndev);
     e = new sw_engine();
     e->M = M; e->NC = (M + 31) / 32; e->cap = capacity_events; e->C = coin_period; e->device = device;
-    e->wide = M > 64;
-    if (const char *v = getenv("SW_FORCE_WIDE")) if (atoi(v)) e->wide = true;
+    e->wide = wide;
     e->NJ = 1;
     while (e->NJ * 32 < M) e->NJ *= 2;
     e->MS = e->wide ? M : 64;
@@ -722,7 +738,6 @@ int sw_create(int M, int capacity_events, const int64_t *stake, int coin_period,
         CK(dalloc(&e->d_t, cap)); CK(dalloc(&e->d_sig, cap * 64)); CK(dalloc(&e->d_height, cap)); CK(dalloc(&e->d_stale, cap));
         // can_see scan scratch: per-event meta / flags / slow list, per-block tables (blocks are >= cs_min_B events)
         e->cs_min_B = std::max(256, std::min((M <= 64 ? 16 : 32) * M, 1 << 15));
-        if (const char *v = getenv("SW_CS_B")) e->cs_min_B = std::max(64, std::min(e->cs_min_B, atoi(v)));
         const size_t nbmax = cap / e->cs_min_B + 3;
         CK(dalloc(&e->d_cs_meta, cap)); CK(dalloc(&e->d_cs_wr, cap)); CK(dalloc(&e->d_cs_xb, cap)); CK(dalloc(&e->d_cs_slow, cap + 4));
         CK(dalloc(&e->d_cs_last, nbmax * M)); CK(dalloc(&e->d_cs_Q, (nbmax + 1) * M)); CK(dalloc(&e->d_cs_slowcnt, (size_t)4)); CK(dalloc(&e->d_cs_sflag, cap)); CK(dalloc(&e->d_cs_xlist, cap + 4)); CK(dalloc(&e->d_cs_slowblk, cap + 4)); CK(dalloc(&e->d_cs_blkcnt, nbmax + 1));
@@ -750,14 +765,11 @@ int sw_create(int M, int capacity_events, const int64_t *stake, int coin_period,
             if (const char *v = getenv("SW_RC_MIN_N")) e->rc_min_n = std::max(1, atoi(v));
             if (want) {
                 int ncl = 0;
-                if (const char *v = getenv("SW_RC_MB")) e->rc_mb = atoi(v) != 0;
-                const void *fn = e->unit ? (e->rc_mb ? (const void *)k_rounds_cluster<true, true> : (const void *)k_rounds_cluster<true, false>)
-                                         : (e->rc_mb ? (const void *)k_rounds_cluster<false, true> : (const void *)k_rounds_cluster<false, false>);
+                const void *fn = e->unit ? (const void *)k_rounds_cluster<true> : (const void *)k_rounds_cluster<false>;
                 cudaError_t er = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RC_SMEM_BYTES);
                 if (er == cudaSuccess) er = cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
                 if (er == cudaSuccess) {
-                    const void *fv = e->unit ? (e->rc_mb ? (const void *)k_rounds_cluster_views<true, true> : (const void *)k_rounds_cluster_views<true, false>)
-                                             : (e->rc_mb ? (const void *)k_rounds_cluster_views<false, true> : (const void *)k_rounds_cluster_views<false, false>);
+                    const void *fv = e->unit ? (const void *)k_rounds_cluster_views<true> : (const void *)k_rounds_cluster_views<false>;
                     er = cudaFuncSetAttribute(fv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RC_SMEM_BYTES);
                     if (er == cudaSuccess) er = cudaFuncSetAttribute(fv, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
                     cudaLaunchConfig_t cfg;
@@ -767,7 +779,6 @@ int sw_create(int M, int capacity_events, const int64_t *stake, int coin_period,
                 }
                 e->rc_ok = er == cudaSuccess && ncl >= 1;
                 if (er != cudaSuccess) (void)cudaGetLastError();
-                if (getenv("SW_DEBUG")) fprintf(stderr, "swirld_b200: cluster round kernel %s (%s, %d clusters of %d CTAs resident)\n", e->rc_ok ? "on" : "off", cudaGetErrorString(er), ncl, RC_CS);
             }
         }
         CK(dalloc(&e->d_round, cap)); CK(dalloc(&e->d_wit, cap)); CK(dalloc(&e->d_famous_ev, cap));
@@ -783,13 +794,13 @@ int sw_create(int M, int capacity_events, const int64_t *stake, int coin_period,
         CK(cudaMallocHost((void **)&e->h_stage, slot * sw_engine::STAGE_SLOTS));
         CK(cudaMalloc((void **)&e->d_stage, slot * sw_engine::STAGE_SLOTS));
         for (auto &ev : e->stage_ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        if (const char *v = getenv("SW_STREAM_N")) e->stream_n = std::max(0, std::min(1024, atoi(v)));
         CK(cudaFuncSetAttribute(k_stream_divide<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
         CK(cudaMallocHost((void **)&e->h_scal, sizeof(int32_t) * ((size_t)SC_COUNT + e->Rcap)));
         e->h_newc = e->h_scal + SC_COUNT;
         CK(cudaMemcpyAsync(e->d_stake, e->h_stake.data(), sizeof(i64) * M, cudaMemcpyHostToDevice, e->stream));
-        // kernels that need more than the default 48 KB of dynamic shared memory
-        const size_t cs_smem = (size_t)(M + CS_SV) * CS_CT * sizeof(int) + CS_TILE * sizeof(int4) + 3 * CS_TILE;
+        // kernels that need more than the default 48 KB of dynamic shared memory: the limit is a property of the kernel in
+        // the whole process, so it is what the largest member count needs, whatever M this engine has
+        const size_t cs_smem = (size_t)(SW_MAX_MEMBERS + CS_SV) * CS_CT * sizeof(int) + CS_TILE * sizeof(int4) + 3 * CS_TILE;
         CK(cudaFuncSetAttribute(k_cs_pass<1, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs_smem));
         CK(cudaFuncSetAttribute(k_cs_pass<2, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs_smem));
         CK(cudaFuncSetAttribute(k_cs_pass<1, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs_smem));
@@ -798,14 +809,28 @@ int sw_create(int M, int capacity_events, const int64_t *stake, int coin_period,
         CK(cudaFuncSetAttribute(k_cs_pass<2, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs_smem));
         CK(cudaFuncSetAttribute(k_cs_pass<1, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs_smem));
         CK(cudaFuncSetAttribute(k_cs_pass<2, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs_smem));
-        CK(cudaFuncSetAttribute(k_cs_slow_wave, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)CS_SLOW_WARPS * M * sizeof(int))));
-        CK(cudaFuncSetAttribute(k_cs_slow_rest, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)CS_REST_WARPS * M * sizeof(int))));
+        CK(cudaFuncSetAttribute(k_cs_slow_wave, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)CS_SLOW_WARPS * SW_MAX_MEMBERS * sizeof(int))));
+        CK(cudaFuncSetAttribute(k_cs_slow_rest, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)CS_REST_WARPS * SW_MAX_MEMBERS * sizeof(int))));
         return reset_state(e);
     }();
     if (rc < 0) { g_create_error = e->err; sw_destroy(e); return rc; }
     memset(&e->stats, 0, sizeof e->stats);
     *out = e;
     return SW_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sw_version(void) { return 202; }
+
+const char *sw_last_error(const sw_engine *e) { return e ? e->err.c_str() : g_create_error.c_str(); }
+
+int sw_create(int M, int capacity_events, const int64_t *stake, int coin_period, int device, sw_engine **out) {
+    bool force_wide = false;                           // SW_FORCE_WIDE=1: the any-M kernels at M <= 64 too
+    if (const char *v = getenv("SW_FORCE_WIDE")) force_wide = atoi(v) != 0;
+    return create(M, capacity_events, stake, coin_period, device, M > 64 || force_wide, out);
 }
 
 void sw_destroy(sw_engine *e) {
@@ -899,7 +924,7 @@ int sw_append(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const i
     std::vector<int32_t> head_save(e->h_head), count_save(e->h_count);
     e->h_creator.resize((size_t)base + n);
     int rc = SW_OK;
-    int next_snap = e->wide ? INT32_MAX : (base / sw_engine::SNAP + 1) * sw_engine::SNAP;
+    int next_snap = (base / sw_engine::SNAP + 1) * sw_engine::SNAP;
     for (int j = 0; j < n && rc == SW_OK; j++) {
         const int i = base + j, c = creator[j], a = p0[j], b = p1[j];
         if (c < 0 || c >= e->M) { rc = fail(e, SW_E_ARG, "event %d: creator %d out of range", i, c); break; }
@@ -923,7 +948,6 @@ int sw_append(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const i
     if (rc == SW_OK) {
         e->h_stale_cum.resize((size_t)base + n + 1);
         for (int j = 0; j < n; j++) e->h_stale_cum[base + j + 1] = e->h_stale_cum[base + j] + e->h_stale[base + j];
-        if (!e->wide && (e->snap_at.empty() || e->snap_at.back() != base + n)) push_snapshot(e, base + n, e->h_count);
     }
     if (rc != SW_OK) {
         e->h_head = head_save; e->h_count = count_save;
@@ -971,6 +995,7 @@ int sw_append(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const i
     e->stats.h2d_bytes += (i64)n * (5 * 4 + 1 + 8 + 64);
     e->stats.events += n;
     e->n_events += n;
+    push_append_snapshot(e);
     if (eager) {
         if (e->scan_ev_set) CK(cudaStreamWaitEvent(cs, e->scan_ev, 0));     // never beside a scan on the compute stream
         int rc2 = cansee_scan(e, cs, e->n_events);
@@ -989,7 +1014,7 @@ int sw_divide_rounds(sw_engine *e, int first, int n) {
     if (first != e->n_divided) return fail(e, SW_E_ARG, "divide_rounds: first=%d but %d events are divided (events must arrive in order)", first, e->n_divided);
     if (first + n > e->n_events) return fail(e, SW_E_KEY, "divide_rounds: events [%d,%d) not appended", first, first + n);
     CK(cudaSetDevice(e->device));
-    if (n <= e->stream_n && e->n_rowed == first) {
+    if (n <= sw_engine::STREAM_N && e->n_rowed == first) {
         // the reference's own cadence (one sync per call): the whole of divide_rounds in ONE launch (swirld_stream.cuh)
         if (wait_appends(e, first + n) < 0) return SW_E_CUDA;
         const int M = e->M;
@@ -1050,8 +1075,7 @@ int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, c
             return fail(e, SW_E_ARG, "sw_batch_divide_rounds: view %d: bad range [%d,%d)", v, first[v], first[v] + n[v]);
     }
     CK(cudaSetDevice(e->device));
-    const int gmin = 1;                                     // (a view's warps loop over its (chain, position) pairs)
-    const int per_launch = std::max(1, e->n_sm / gmin);
+    const int per_launch = e->n_sm;                         // (one CTA per view at least: its warps loop over its chains)
     if (B > e->views_cap) {
         if (e->d_views) cudaFree(e->d_views);
         if (e->d_rcviews) cudaFree(e->d_rcviews);
@@ -1062,12 +1086,12 @@ int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, c
     }
     // one thread-block cluster per view first (swirld_rcluster.cuh); the grid-wide kernel then takes what they hand back
     bool use_rc = true;
-    for (int v = 0; v < B; v++) use_rc = use_rc && engines[v]->rc_ok && engines[v]->rc_mb == e->rc_mb && n[v] >= e->rc_min_n;
+    for (int v = 0; v < B; v++) use_rc = use_rc && engines[v]->rc_ok && n[v] >= e->rc_min_n;
     std::vector<RcParams> Qv(B);
     if (!e->view_ev) CK(cudaEventCreateWithFlags(&e->view_ev, cudaEventDisableTiming));
     std::vector<RbParams> Rv(B);
     for (int v0 = 0; v0 < B; v0 += per_launch) {
-        const int nv = std::min(per_launch, B - v0), G = std::max(gmin, e->n_sm / nv);
+        const int nv = std::min(per_launch, B - v0), G = e->n_sm / nv;
         for (int v = v0; v < v0 + nv; v++) {
             sw_engine *x = engines[v];
             if (first[v] + n[v] > x->n_rowed) {
@@ -1100,8 +1124,8 @@ int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, c
                 cudaLaunchAttribute at[1];
                 rc_launch_config(cfg, at, nv, e->stream);
                 const RcParams *qv = e->d_rcviews + v0;
-                if (e->unit) { if (e->rc_mb) CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster_views<true, true>, qv)); else CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster_views<true, false>, qv)); }
-                else { if (e->rc_mb) CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster_views<false, true>, qv)); else CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster_views<false, false>, qv)); }
+                if (e->unit) CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster_views<true>, qv));
+                else CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster_views<false>, qv));
                 e->stats.kernel_launches += 1;
                 e->stats.rounds_cluster_launches += 1;
             }
@@ -1642,17 +1666,16 @@ int sw_load(const char *path, int device, int capacity_events, sw_engine **out) 
     FILE *f = fopen(path, "rb");
     if (!f) return fail(e, SW_E_ARG, "sw_load: cannot open %s", path);
     CkptHeader H{};
-    if (fread(&H, sizeof H, 1, f) != 1 || memcmp(H.magic, CKPT_MAGIC, 8) != 0 || H.version != 1 || H.M < 1 || H.M > SW_MAX_MEMBERS) {
+    if (fread(&H, sizeof H, 1, f) != 1 || memcmp(H.magic, CKPT_MAGIC, 8) != 0 || H.version != 1 || H.M < 1 || H.M > SW_MAX_MEMBERS
+        || (H.M > 64 && !H.wide)) {
         fclose(f);
         return fail(e, SW_E_ARG, "sw_load: %s is not a swirld_b200 checkpoint", path);
     }
     std::vector<i64> stake(H.M);
     if (!get_host(f, stake.data(), sizeof(i64) * H.M)) { fclose(f); return fail(e, SW_E_ARG, "sw_load: truncated file"); }
     const int cap = std::max(capacity_events > 0 ? capacity_events : H.cap, H.n_events);
-    // the saved engine's path (wide or not) is restored whatever SW_FORCE_WIDE says now
-    setenv("SW_FORCE_WIDE", H.wide ? "1" : "0", 1);
-    int rc = sw_create(H.M, cap, reinterpret_cast<const int64_t *>(stake.data()), H.C, device, &e);
-    unsetenv("SW_FORCE_WIDE");
+    // the saved engine's kernel family, whatever SW_FORCE_WIDE says now
+    int rc = create(H.M, cap, reinterpret_cast<const int64_t *>(stake.data()), H.C, device, H.wide != 0, &e);
     if (rc < 0) { fclose(f); return rc; }
     const int M = H.M, n = H.n_events, nd = H.n_divided, nr = H.n_rowed, R = H.rounds;
     if (R > e->Rcap || (int)e->wide != H.wide || e->NJ != H.NJ) { fclose(f); sw_destroy(e); return fail(nullptr, SW_E_ARG, "sw_load: checkpoint does not fit the engine"); }
@@ -1692,12 +1715,10 @@ int sw_load(const char *path, int device, int capacity_events, sw_engine **out) 
     e->n_events = n; e->n_divided = nd; e->n_tx = H.n_tx; e->n_rowed = nr; e->rb_epoch = H.rb_epoch;
     e->h_stale_cum.assign((size_t)n + 1, 0);
     for (int i = 0; i < n; i++) e->h_stale_cum[i + 1] = e->h_stale_cum[i] + e->h_stale[i];
-    if (!e->wide) {
-        std::vector<int32_t> cnt(M, 0);
-        for (int i = 0; i < n; i++) {
-            cnt[e->h_creator[i]]++;
-            if ((i + 1) % sw_engine::SNAP == 0 || i + 1 == n) push_snapshot(e, i + 1, cnt);
-        }
+    std::vector<int32_t> cnt(M, 0);
+    for (int i = 0; i < n; i++) {
+        cnt[e->h_creator[i]]++;
+        if ((i + 1) % sw_engine::SNAP == 0 || i + 1 == n) push_snapshot(e, i + 1, cnt);
     }
     e->stats.events = n; e->stats.events_divided = nd;
     *out = e;

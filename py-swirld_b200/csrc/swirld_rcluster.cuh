@@ -27,8 +27,8 @@
 //          a chain), one test of swirld_rounds.cuh's kind per warp and pass;
 //       c  (first position, kind) of every chain to every CTA, again by st.async + mbarrier;
 //       d  identical bookkeeping in every CTA; the owner stores the final rounds and Wf, the window slides.
-//     With MB = false the two exchanges use plain DSMEM stores and barrier.cluster instead (the release fence of the
-//     barrier also waits for the step's global stores: slower; kept for A/B, SW_RC_MB=0).
+//     (Plain DSMEM stores and barrier.cluster instead of st.async + mbarrier are slower: the release fence of the
+//     barrier also waits for the step's global stores.)
 //   * whatever the windows cannot decide -- no progress for RC_STALL steps, a chain more than RB_WR rounds behind,
 //     rows further before the chunk than RC_REACH -- hands the REST of the chunk to k_rounds_batch through `cont`
 //     (positions and rounds per chain).  tests/test_rounds_cluster_model.py is the executable model.
@@ -71,16 +71,12 @@ __device__ __forceinline__ unsigned rc_map(const void *p, unsigned rank) {
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
     return r;
 }
-__device__ __forceinline__ void rc_st_u32(unsigned addr, unsigned v) { asm volatile("st.shared::cluster.u32 [%0], %1;" :: "r"(addr), "r"(v) : "memory"); }
 __device__ __forceinline__ void rc_cp16(void *dst, const void *src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
 }
 
 __device__ __forceinline__ void rc_cp4(void *dst, const void *src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" :: "r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
-}
-__device__ __forceinline__ void rc_st_v4(unsigned addr, uint4 v) {
-    asm volatile("st.shared::cluster.v4.u32 [%0], {%1, %2, %3, %4};" :: "r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 // carry-save adder over 64 bit columns: a + b + c = 2 * h + l
 __device__ __forceinline__ void rc_csa(u64 &h, u64 &l, u64 a, u64 b, u64 c) {
@@ -126,8 +122,7 @@ __device__ __forceinline__ void rc_sta_u32(unsigned addr, unsigned v, unsigned m
     asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" :: "r"(addr), "r"(v), "r"(mbar) : "memory");
 }
 
-// MB: the two exchanges of a step (masks, results) by st.async + mbarrier instead of stores + cluster barriers
-template <bool UNIT, bool MB>
+template <bool UNIT>
 __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
     const RbParams &P = Q.R;
     extern __shared__ __align__(16) unsigned char rc_smem[];
@@ -186,7 +181,7 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
     if (tid < 64 && xres[tid] && rtop < RB_WR) Wls[0][tid] = 0;
     __syncthreads();
 
-    if (MB && tid == 0) {
+    if (tid == 0) {
         rc_mbar_init(mbar0, 1); rc_mbar_init(mbar0 + 8, 1); rc_mbar_init(mbar0 + 16, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -250,14 +245,12 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
     unsigned it = 0;                                            // steps so far (mbarrier phases)
     for (; !handed; ++it) {
         const long long t0 = clock64();
-        u64 (*maskbuf)[RC_MRS] = maskbuf0 + (MB ? (it & 1) * 64 : 0);
+        u64 (*maskbuf)[RC_MRS] = maskbuf0 + (it & 1) * 64;
         // ---- the results of the last step (every CTA holds all of them): positions, rounds, the mirror of Wf; then
         //      this step's ranges and windows.  One warp, no block-wide barrier inside.
         bool late = false;
-        if (MB) {
-            if (have_res) late = !rc_mbar_wait(mbar0 + 16, (it - 1) & 1);
-            if (tid == 0) rc_mbar_expect(mbar0 + 16, 64 * 4);  // this step's results: one word per chain
-        }
+        if (have_res) late = !rc_mbar_wait(mbar0 + 16, (it - 1) & 1);
+        if (tid == 0) rc_mbar_expect(mbar0 + 16, 64 * 4);      // this step's results: one word per chain
         asm volatile("cp.async.wait_all;" ::: "memory");        // (the rows issued a step ago)
         if (warp == 0) {
             bool hit[2] = {false, false}, prog = false;
@@ -315,7 +308,7 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
                 const bool anymoved = __any_sync(0xffffffffu, moved);
                 if (have_res) stall = (anyprog || anymoved) ? 0 : stall + 1;
                 if (stall >= RC_STALL) status = 2;
-                else if (MB) {                                  // the bytes the other CTAs will store into my mask table
+                else {                                          // the bytes the other CTAs will store into my mask table
                     int by = 0;
 #pragma unroll
                     for (int j = 0; j < 2; j++) { const int m = lane + 32 * j; if (m / RC_CPC != bx) by += ((cnts[m] + 1) >> 1) * 16; }
@@ -369,12 +362,10 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
                 const int cl2 = pair & (RC_CPC - 1), r = pair / RC_CPC, c2 = bx * RC_CPC + cl2;
                 if (r == bx || 2 * lane >= cnts[c2]) continue;
                 const uint4 val = *reinterpret_cast<const uint4 *>(&maskbuf[c2][2 * lane]);
-                if (MB) rc_sta_v4(rc_map(&maskbuf[c2][2 * lane], (unsigned)r), val, rc_map(iv + 2304 + 2 * (it & 1), (unsigned)r));
-                else rc_st_v4(rc_map(&maskbuf[c2][2 * lane], (unsigned)r), val);
+                rc_sta_v4(rc_map(&maskbuf[c2][2 * lane], (unsigned)r), val, rc_map(iv + 2304 + 2 * (it & 1), (unsigned)r));
             }
         }
         const long long t2 = clock64();
-        if (!MB) rc_cluster_arrive();
         // off the path the other CTAs wait on: the final rounds of the last step, the next rows of my chains' windows
         if (have_res && tid < RC_CPC * RC_LW) {
             const int cl = tid / RC_LW, j = tid % RC_LW, c = bx * RC_CPC + cl;
@@ -423,8 +414,7 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
             unk = ((ub >> (lane & ~3)) & 0xfu) != 0;
             const bool need = act && lv > thr_i && !unk;       // (lv <= thr: hits[c_] <= the live members)
             int v = (act && lv > thr_i && unk) ? 2 : 0;
-            if (MB) late = !rc_mbar_wait(mbar0 + 8 * (it & 1), (it >> 1) & 1);
-            else rc_cluster_wait();
+            late = !rc_mbar_wait(mbar0 + 8 * (it & 1), (it >> 1) & 1);
             t3 = clock64();
             if (__any_sync(0xffffffffu, need)) {
                 c_tests++;
@@ -471,13 +461,11 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
                 const int vf = nz ? __shfl_sync(0xffffffffu, x, f & 31) : 0;
                 if (lane < RC_CS) {
                     const unsigned xv = w2 >= 0 ? (unsigned)(f << 2 | vf) : 0u;
-                    if (MB) rc_sta_u32(rc_map(&xres[c2], (unsigned)lane), xv, rc_map(iv + 2304 + 4, (unsigned)lane));
-                    else rc_st_u32(rc_map(&xres[c2], (unsigned)lane), xv);
+                    rc_sta_u32(rc_map(&xres[c2], (unsigned)lane), xv, rc_map(iv + 2304 + 4, (unsigned)lane));
                 }
             }
         } else {
-            if (MB) late = !rc_mbar_wait(mbar0 + 8 * (it & 1), (it >> 1) & 1);
-            else rc_cluster_wait();
+            late = !rc_mbar_wait(mbar0 + 8 * (it & 1), (it >> 1) & 1);
             if (__syncthreads_or(late)) {
                 if (tid == 0 && lead) atomicMin(&P.scal[SC_ERR], -4);
                 handed = 1;
@@ -560,12 +548,10 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
                 const int cl = tid & (RC_CPC - 1), rank = tid / RC_CPC, c = bx * RC_CPC + cl;
                 unsigned x = 0;
                 if (swin[c] >= 0) { const int f = sb[cl]; x = (unsigned)(f << 2 | (f < swin[c] ? svb[cl] : 0)); }
-                if (MB) rc_sta_u32(rc_map(&xres[c], (unsigned)rank), x, rc_map(iv + 2304 + 4, (unsigned)rank));
-                else rc_st_u32(rc_map(&xres[c], (unsigned)rank), x);
+                rc_sta_u32(rc_map(&xres[c], (unsigned)rank), x, rc_map(iv + 2304 + 4, (unsigned)rank));
             }
         }
         const long long t4 = clock64();
-        if (!MB) rc_cluster_sync();
         const long long t5 = clock64();
         have_res = true;
         c_t[0] += t1 - t0; c_t[1] += t2 - t1; c_t[2] += t3 - t2; c_t[3] += t4 - t3; c_t[4] += t5 - t4;
@@ -597,15 +583,15 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
     rc_cluster_sync();                                          // nobody leaves while its shared memory may still be written
 }
 
-template <bool UNIT, bool MB>
-__global__ void __launch_bounds__(RC_THREADS, 1) k_rounds_cluster(RcParams Q) { rounds_cluster_body<UNIT, MB>(Q); }
+template <bool UNIT>
+__global__ void __launch_bounds__(RC_THREADS, 1) k_rounds_cluster(RcParams Q) { rounds_cluster_body<UNIT>(Q); }
 
 // several independent node-views (swirld_rounds.cuh, k_rounds_batch_views): one cluster per view, as many side by side
 // as the device holds -- the clusters never talk to each other, so this is an ordinary (non-cooperative) launch
-template <bool UNIT, bool MB>
+template <bool UNIT>
 __global__ void __launch_bounds__(RC_THREADS, 1) k_rounds_cluster_views(const RcParams *Qv) {
     __shared__ RcParams Qs;
     if (threadIdx.x == 0) Qs = Qv[blockIdx.x / RC_CS];
     __syncthreads();
-    rounds_cluster_body<UNIT, MB>(Qs);
+    rounds_cluster_body<UNIT>(Qs);
 }

@@ -42,18 +42,18 @@
 #define RB_MAXMISS 0         // an event with more unprepared S_r masks than this waits for a later step
 
 struct RbParams {
-    int M, first, n, Rcap, L, maxmiss;
+    int M, first, n, Rcap, L;
     unsigned epoch;             // launch counter (part of the mask-cache key)
     const int32_t *row, *p0, *creator, *seq;
     int32_t *round;             // [cap] out
     int32_t *Wf;                // [Rcap][M] first event of round >= r per member
     ulonglong2 *sc;             // [cap] {S_r(k), S_r(k) ^ key(r)}
     int32_t *cev;               // [cap] chunk events grouped by creator, region [first, first+n)
-    int32_t *ccnt, *cmin;       // [64] per-member count / smallest seq inside the chunk
-    int32_t *ctot;              // [64] events of the member so far (1 + its largest seq)
-    int32_t *gchain;            // [64][RB_RING] the member's most recent events by seq % RB_RING
-    int32_t *coff;              // [65]
-    unsigned *bar;              // grid barrier counter of k_rounds_batch (zeroed by k_rb_prep)
+    int32_t *ccnt, *cmin;       // [MP] per-member count / smallest seq inside the chunk (MP = max(M, 64))
+    int32_t *ctot;              // [M] events of the member so far (1 + its largest seq)
+    int32_t *gchain;            // [M][RB_RING] the member's most recent events by seq % RB_RING
+    int32_t *coff;              // [MP + 1]
+    unsigned *bar;              // grid barrier counter of the round kernel (zeroed by k_rb_prep)
     uint8_t *res;               // per-step results of k_rounds_batch, 2 x (64 x u64 + 64 x int)
     const i64 *stake;
     i64 tot2;
@@ -68,20 +68,27 @@ struct RbParams {
 };
 
 // ---- per-member event lists of the chunk.  Events are divided in arrival order and seq[h] counts the earlier events
-// of h's creator, so the per-member counts of a chunk are known on the host (round_batch_prep) and arrive by value.
+// of h's creator, so the per-member counts of a chunk are known on the host (chunk_prep) and arrive by value.
+// CM members at most: 64 for the M <= 64 kernels, SW_MAX_MEMBERS (16 KB of parameters) for the any-M kernels.
+template <int CM>
 struct RbChunk {
-    int ccnt[64];               // events of the member in the chunk
-    int cmin[64];               // the smallest seq among them (0x7f7f7f7f: none)
-    int ctot[64];               // events of the member up to the end of the chunk
-    int coff[65];               // exclusive prefix sum of ccnt
+    int ccnt[CM];               // events of the member in the chunk
+    int cmin[CM];               // the smallest seq among them (0x7f7f7f7f: none)
+    int ctot[CM];               // events of the member up to the end of the chunk
+    int coff[CM + 1];           // exclusive prefix sum of ccnt
 };
 
-// the chunk's meta arrays, cev, and (rsg != NULL) the seq-space rows of swirld_rcluster.cuh in cev order: one warp per event
-__global__ void __launch_bounds__(256) k_rb_prep(RbParams P, const __grid_constant__ RbChunk K, int32_t *rsg) {
+// the chunk's meta arrays, cev, and (rsg != NULL, M <= 64) the seq-space rows of swirld_rcluster.cuh in cev order: one
+// warp per event
+template <int CM>
+__global__ void __launch_bounds__(256) k_rb_prep(RbParams P, const __grid_constant__ RbChunk<CM> K, int32_t *rsg) {
     const int tid = threadIdx.x, lane = tid & 31;
     if (blockIdx.x == 0) {
-        if (tid < 64) { P.ccnt[tid] = K.ccnt[tid]; P.cmin[tid] = K.cmin[tid]; if (tid < P.M) P.ctot[tid] = K.ctot[tid]; }
-        if (tid <= 64) P.coff[tid] = K.coff[tid];
+        const int mp = min(CM, max(P.M, 64));                 // (the meta arrays hold max(M, 64) members)
+        for (int c = tid; c <= mp; c += blockDim.x) {
+            if (c < mp) { P.ccnt[c] = K.ccnt[c]; P.cmin[c] = K.cmin[c]; if (c < P.M) P.ctot[c] = K.ctot[c]; }
+            P.coff[c] = K.coff[c];
+        }
         if (tid == 0) { *P.bar = 0; *P.wcnt = 0; }
     }
     for (int j = blockIdx.x * 8 + (tid >> 5); j < P.n; j += gridDim.x * 8) {
@@ -249,7 +256,7 @@ __device__ __forceinline__ void rounds_batch_body(const RbParams &P, const int b
 #pragma unroll
             for (int j = 0; j < NC; j++) nm += __popc(__ballot_sync(0xffffffffu, live[j] && !valid[j]));
             tG1 = clock64();
-            if (may_defer && nm > P.maxmiss) return 2;       // (never the chain's first pending event: progress)
+            if (may_defer && nm > RB_MAXMISS) return 2;       // (never the chain's first pending event: progress)
         }
 #pragma unroll
         for (int jj = 0; jj < NC; jj++) {                     // cache misses: compute S_r(k) together,

@@ -160,8 +160,8 @@ struct RwParams {
     int32_t *Wf;                // [Rcap][M]
     unsigned *scw;              // [cap][NJ] mask cache
     u64 *sctag;                 // [cap] (epoch << 32 | round + 1) of the cached mask
-    int32_t *cev;               // chunk events grouped by creator at [first, first+n)
-    int32_t *ccnt, *cmin, *coff, *ctot, *gchain;
+    int32_t *cev;               // chunk events grouped by creator at [first, first+n) (k_rb_prep, like cmin, coff, ctot, bar)
+    int32_t *cmin, *coff, *ctot, *gchain;
     unsigned *bar;
     u64 *hitmin;                // [3][M]
     unsigned *ticket;           // [3] work counter of a step's tests (cleared like hitmin)
@@ -177,44 +177,6 @@ struct RwParams {
                                 // because the step count of a launch is data dependent)
     long long *dbg;
 };
-
-__global__ void __launch_bounds__(256) k_rw_count(RwParams P) {
-    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < P.n; j += gridDim.x * blockDim.x) {
-        const int h = P.first + j, c = P.creator[h], sq = P.seq[h];
-        atomicAdd(&P.ccnt[c], 1);
-        atomicMin(&P.cmin[c], sq);
-        atomicMax(&P.ctot[c], sq + 1);
-    }
-}
-__global__ void __launch_bounds__(1024) k_rw_offsets(RwParams P, int32_t *wcnt) {     // one CTA: exclusive scan of ccnt
-    __shared__ int wsum_s[32];
-    __shared__ int base_s;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) { base_s = 0; *P.bar = 0; *wcnt = 0; }
-    __syncthreads();
-    for (int c0 = 0; c0 < P.M; c0 += 1024) {
-        const int c = c0 + tid;
-        const int a = c < P.M ? P.ccnt[c] : 0;
-        int inc = a;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int x = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += x; }
-        if (lane == 31) wsum_s[warp] = inc;
-        __syncthreads();
-        int before = base_s;
-        for (int w2 = 0; w2 < warp; w2++) before += wsum_s[w2];
-        if (c < P.M) P.coff[c] = before + inc - a;
-        __syncthreads();
-        if (tid == 1023) base_s = before + inc;
-        __syncthreads();
-    }
-    if (tid == 0) P.coff[P.M] = base_s;
-}
-__global__ void k_rw_scatter(RwParams P) {
-    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < P.n; j += gridDim.x * blockDim.x) {
-        const int h = P.first + j, c = P.creator[h];
-        P.cev[P.first + P.coff[c] + P.seq[h] - P.cmin[c]] = h;
-    }
-}
 
 __device__ __forceinline__ void rw_grid_barrier(unsigned *ctr, unsigned &target) {
     __syncthreads();

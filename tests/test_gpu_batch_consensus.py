@@ -284,15 +284,14 @@ def test_refusals_change_nothing(monkeypatch):
     from swirld_b200.engine import EngineError
     cases = [_gossip(8, 3000, 41, 500), _gossip(8, 2500, 42, 500), _gossip(8, 3000, 43, 700)]
     trs = [c.trace() for c in cases]
+    odd = _gossip(9, 2000, 44, 500)
+    e9 = engine.Engine(9, 2000)
     engs = [engine.Engine(8, tr.N) for tr in trs]
     monkeypatch.setenv("SW_FORCE_WIDE", "1")
     ew = engine.Engine(8, trs[0].N)
     monkeypatch.delenv("SW_FORCE_WIDE")
     undiv = engine.Engine(8, trs[0].N)
     undiv.append_trace(trs[0])
-    # (created last: sw_create sets the can_see kernels' dynamic shared memory limit for its own M, process-wide)
-    odd = _gossip(9, 2000, 44, 500)
-    e9 = engine.Engine(9, 2000)
     scheds = [c.schedule(tr.N) for c, tr in zip(cases, trs)]
     for e, tr, s in zip(engs + [ew], trs + [trs[0]], scheds + [scheds[0]]):
         e.append_trace(tr)
