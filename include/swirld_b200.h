@@ -84,6 +84,21 @@ const char *sw_last_error(const sw_engine *e);   /* e may be NULL: last create e
 int sw_append(sw_engine *e, int n, const int32_t *p0, const int32_t *p1,
               const int32_t *creator, const double *t, const uint8_t *sig);
 
+/* Node.add_event for B independent node-views in one call (each node of the simulation receives the events of its
+ * sync, swirld.py:319-324): view v appends rows offsets[v] .. offsets[v+1] of the concatenated columns (as sw_append).
+ * The views may differ in M; they share one device.  The views of at most 64 events go over packed in ONE copy and are
+ * scattered by ONE kernel on the first engine's copy stream (charged to the first engine): the caller's arrays are free
+ * again when the call returns.  Larger views make the copies (and can_see scan) their sw_append makes, under its
+ * page-locked memory contract.
+ * Argument errors refuse the whole call before anything runs, leave rc_out unwritten and put the message in the first
+ * engine's sw_last_error: B < 1, a NULL or repeated engine, views on different devices or peer-connected to other GPUs
+ * (SW_E_UNSUPPORTED), offsets that are not monotone (SW_E_ARG).  A view whose events sw_append would refuse (SW_E_PARENT,
+ * SW_E_FORK, SW_E_CAPACITY, SW_E_ARG for a creator out of range) appends nothing: rc_out[v] gets that code and the
+ * message is in that view's sw_last_error; the other views append normally (rc_out[v] = SW_OK).  Returns SW_OK when
+ * every view appended, else the first failing view's code. */
+int sw_batch_append(sw_engine *const *engines, int B, const int *offsets, const int32_t *p0, const int32_t *p1,
+                    const int32_t *creator, const double *t, const uint8_t *sig, int32_t *rc_out);
+
 /* Node.divide_rounds(events) (swirld.py:187-222) for the topologically sorted
  * events [first, first+n): can_see rows, round numbers, witness registration.
  * `first` must equal the number of events already divided. Asynchronous. */
@@ -91,10 +106,17 @@ int sw_divide_rounds(sw_engine *e, int first, int n);
 
 /* Node.divide_rounds for B independent node-views in one call (the simulation's M nodes each recompute consensus on
  * nearly the same graph, swirld.py:331-345 / viz.py:35-46): engines[v] divides its events [first[v], first[v]+n[v]).
- * M <= 64, same member count and stake shape, same device.  The views' round kernels advance side by side -- one
- * thread-block cluster per view (chunks of >= 2048 events), then ONE cooperative launch, each view on its own group of
- * CTAs, for what is left: the path is latency-bound, so this is what fills the GPU.
- * Results per view are identical to B separate sw_divide_rounds calls. */
+ * The views share one member count, kernel family and device (as sw_batch_decide_fame), and each takes the path its
+ * single call would take:
+ *  - a call of at most 16 events whose can_see rows are not behind (the reference's cadence): every such view in ONE
+ *    launch, one thread block per view, at any M; stakes and coin periods may differ.  Asynchronous, like
+ *    sw_divide_rounds: each view's stream waits for the launch, and nothing synchronises the host.
+ *  - the other calls (M <= 64 only, one stake shape among them): the views' round kernels advance side by side -- one
+ *    thread-block cluster per view (chunks of >= 2048 events), then ONE cooperative launch, each view on its own group
+ *    of CTAs, for what is left: the path is latency-bound, so this is what fills the GPU.
+ * A batch whose chunk-path views break those rules is refused as a whole before anything runs (SW_E_UNSUPPORTED), as are
+ * views that differ in M, kernel family or device, a NULL or repeated engine and a bad range (SW_E_ARG).  Timings and
+ * launches are charged to the first engine.  Results per view are identical to B separate sw_divide_rounds calls. */
 int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, const int *n);
 
 /* Node.decide_fame() (swirld.py:224-277).  Writes the new consensus rounds

@@ -127,7 +127,16 @@ struct sw_engine {
     uint8_t *h_stage = nullptr, *d_stage = nullptr;
     cudaEvent_t stage_ev[STAGE_SLOTS] = {nullptr};
     int stage_next = 0;
+    // sw_batch_append (owned by the first engine of a batch): the packed small views of one call, [parameters][columns],
+    // in a ring of its own.  h_vbuf cannot hold them: the batched fame and order calls of the same turn rewrite it on
+    // the host before the asynchronous copy from it would have run.
+    uint8_t *h_bstage = nullptr, *d_bstage = nullptr;
+    size_t bstage_slot = 0;       // bytes per slot
+    cudaEvent_t bstage_ev[STAGE_SLOTS] = {nullptr};
+    int bstage_next = 0;
     static constexpr int STREAM_N = 16;              // divide_rounds calls of at most this many events take the one-launch path
+    StreamParams *d_stviews = nullptr;               // sw_batch_divide_rounds: the parameters of the views on that path
+    int stviews_cap = 0;
     int32_t *h_scal = nullptr;    // pinned
     int32_t *h_newc = nullptr;    // pinned, Rcap: right behind h_scal (one copy brings both back)
     cudaStream_t stream = nullptr;
@@ -633,10 +642,10 @@ OrderParams order_params(const sw_engine *e, int n, const int32_t *rounds) {
     return P;
 }
 
-// ---- several node-views per call (sw_batch_decide_fame / sw_batch_find_order)
-// The shape checks shared by both calls: they refuse the whole batch before anything runs (the message goes to the first
-// engine).
-int check_views(sw_engine *const *engines, int B, const char *what) {
+// ---- several node-views per call (sw_batch_*)
+// The checks shared by the batched calls: they refuse the whole batch before anything runs (the message goes to the first
+// engine).  `same_shape`: the views must also share M and the kernel family (all but sw_batch_append).
+int check_views(sw_engine *const *engines, int B, const char *what, bool same_shape) {
     sw_engine *e = engines[0];
     std::vector<const sw_engine *> seen(engines, engines + B);
     for (int v = 0; v < B; v++)
@@ -645,8 +654,9 @@ int check_views(sw_engine *const *engines, int B, const char *what) {
     if (std::adjacent_find(seen.begin(), seen.end()) != seen.end()) return fail(e, SW_E_ARG, "%s: an engine appears twice", what);
     for (int v = 0; v < B; v++) {
         const sw_engine *x = engines[v];
-        if (x->device != e->device || x->M != e->M || x->wide != e->wide)
-            return fail(e, SW_E_UNSUPPORTED, "%s: view %d: the views must have one member count and one kernel family on one device", what, v);
+        if (x->device != e->device || (same_shape && (x->M != e->M || x->wide != e->wide)))
+            return fail(e, SW_E_UNSUPPORTED, "%s: view %d: the views must %s on one device", what, v,
+                        same_shape ? "have one member count and one kernel family" : "be");
         if (x->nranks > 1) return fail(e, SW_E_UNSUPPORTED, "%s: view %d is one rank of a multi-GPU engine", what, v);
     }
     return 0;
@@ -795,6 +805,7 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
         CK(cudaMalloc((void **)&e->d_stage, slot * sw_engine::STAGE_SLOTS));
         for (auto &ev : e->stage_ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
         CK(cudaFuncSetAttribute(k_stream_divide<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
+        CK(cudaFuncSetAttribute(k_stream_divide_views<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
         CK(cudaMallocHost((void **)&e->h_scal, sizeof(int32_t) * ((size_t)SC_COUNT + e->Rcap)));
         e->h_newc = e->h_scal + SC_COUNT;
         CK(cudaMemcpyAsync(e->d_stake, e->h_stake.data(), sizeof(i64) * M, cudaMemcpyHostToDevice, e->stream));
@@ -819,11 +830,132 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
     return SW_OK;
 }
 
+// ---- the parts of sw_append, shared with sw_batch_append
+// The graph-shape checks of is_valid_event (swirld.py:104-108) and the fork-free contract for the n events that follow
+// the engine's last one, updating the host mirrors; on an error the mirrors are as they were and the message is the
+// engine's.
+int append_validate(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const int32_t *creator) {
+    if ((i64)e->n_events + n > e->cap) return fail(e, SW_E_CAPACITY, "capacity_events=%d exceeded", e->cap);
+    const int base = e->n_events;
+    std::vector<int32_t> head_save(e->h_head), count_save(e->h_count);
+    e->h_creator.resize((size_t)base + n);
+    int rc = SW_OK;
+    int next_snap = (base / sw_engine::SNAP + 1) * sw_engine::SNAP;
+    for (int j = 0; j < n && rc == SW_OK; j++) {
+        const int i = base + j, c = creator[j], a = p0[j], b = p1[j];
+        if (c < 0 || c >= e->M) { rc = fail(e, SW_E_ARG, "event %d: creator %d out of range", i, c); break; }
+        e->h_stale[i] = 0;
+        if (a < 0 && b < 0) {
+            if (e->h_head[c] >= 0) { rc = fail(e, SW_E_FORK, "event %d: second root of member %d", i, c); break; }
+            e->h_height[i] = 0;                                          // swirld.py:117-118
+        } else {
+            if (a < 0 || b < 0 || a >= i || b >= i) { rc = fail(e, SW_E_PARENT, "event %d: parents (%d,%d) unknown", i, a, b); break; }
+            if (e->h_creator[a] != c) { rc = fail(e, SW_E_PARENT, "event %d: self-parent %d has another creator", i, a); break; }
+            if (e->h_creator[b] == c) { rc = fail(e, SW_E_PARENT, "event %d: other-parent %d has the same creator", i, b); break; }
+            if (e->h_head[c] != a) { rc = fail(e, SW_E_FORK, "event %d: self-parent %d is not member %d's latest event (fork)", i, a, c); break; }
+            e->h_height[i] = std::max(e->h_height[a], e->h_height[b]) + 1;   // swirld.py:120
+            e->h_stale[i] = e->h_head[e->h_creator[b]] != b;             // "near fork": an older event of the peer
+        }
+        e->h_creator[i] = c;
+        e->h_head[c] = i;
+        e->h_seq[i] = e->h_count[c]++;
+        if (i + 1 == next_snap) { push_snapshot(e, i + 1, e->h_count); next_snap += sw_engine::SNAP; }
+    }
+    if (rc != SW_OK) {
+        e->h_head = head_save; e->h_count = count_save;
+        e->h_creator.resize(base);
+        while (!e->snap_at.empty() && e->snap_at.back() > base) { e->snap_at.pop_back(); e->snap_cnt.resize(e->snap_at.size() * e->M); }
+        return rc;
+    }
+    e->h_stale_cum.resize((size_t)base + n + 1);
+    for (int j = 0; j < n; j++) e->h_stale_cum[base + j + 1] = e->h_stale_cum[base + j] + e->h_stale[base + j];
+    return SW_OK;
+}
+
+// A handful of events (at most STAGE_EVENTS): the eight columns packed at `hs` (unpack_bytes(n) bytes, which go to
+// `ds` on the device), and what k_unpack needs to scatter them.  The caller's arrays are free once this returns.
+UnpackParams append_pack(const sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const int32_t *creator,
+                         const double *t, const uint8_t *sig, uint8_t *hs, const uint8_t *ds) {
+    const int base = e->n_events;
+    int32_t *ints = reinterpret_cast<int32_t *>(hs);
+    memcpy(ints, p0, sizeof(int32_t) * n); memcpy(ints + n, p1, sizeof(int32_t) * n); memcpy(ints + 2 * n, creator, sizeof(int32_t) * n);
+    memcpy(ints + 3 * n, e->h_seq + base, sizeof(int32_t) * n); memcpy(ints + 4 * n, e->h_height + base, sizeof(int32_t) * n);
+    uint8_t *pt = hs + unpack_off_t(n);
+    memcpy(pt, t, sizeof(double) * n); memcpy(pt + (size_t)8 * n, sig, (size_t)64 * n); memcpy(pt + (size_t)72 * n, e->h_stale + base, (size_t)n);
+    UnpackParams U{};
+    U.base = base; U.n = n; U.stage = ds; U.p0 = e->d_p0; U.p1 = e->d_p1; U.creator = e->d_creator; U.seq = e->d_seq;
+    U.height = e->d_height; U.t = e->d_t; U.sig = e->d_sig; U.stale = e->d_stale;
+    return U;
+}
+
+// More events: one copy per column on the engine's copy stream (from pinned memory, asynchronous)
+int append_copy(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const int32_t *creator, const double *t,
+                const uint8_t *sig) {
+    const int base = e->n_events;
+    cudaStream_t cs = e->copy_stream;
+    CK(cudaMemcpyAsync(e->d_p0 + base, p0, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_p1 + base, p1, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_creator + base, creator, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_t + base, t, sizeof(double) * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_sig + (size_t)base * 64, sig, (size_t)64 * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_seq + base, e->h_seq + base, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_height + base, e->h_height + base, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_stale + base, e->h_stale + base, (size_t)n, cudaMemcpyHostToDevice, cs));
+    return 0;
+}
+
+// The n validated events are queued on `st` (the engine's copy stream, or the first engine's for a packed batch): count
+// them, and start their can_see rows when the batch is big.  Later calls wait for `st` at this point (wait_appends).
+int append_commit(sw_engine *e, int n, cudaStream_t st) {
+    const int base = e->n_events;
+    // rows are up to date and the batch is big: scan it now, beside the kernels of the previous chunk
+    // (several ranks: the scan holds cross-GPU barriers; it must not run beside a round kernel that fills every SM while
+    //  waiting for the same peer -- scans stay on the compute stream then)
+    const bool eager = e->n_rowed == base && n >= 4096 && e->nranks == 1;
+    e->stats.h2d_bytes += (i64)n * (5 * 4 + 1 + 8 + 64);
+    e->stats.events += n;
+    e->n_events += n;
+    push_append_snapshot(e);
+    if (eager) {
+        if (e->scan_ev_set) CK(cudaStreamWaitEvent(st, e->scan_ev, 0));     // never beside a scan on the compute stream
+        int rc2 = cansee_scan(e, st, e->n_events);
+        if (rc2 < 0) return rc2;
+    }
+    // the compute stream waits for this batch only when a call first touches it (wait_appends)
+    cudaEvent_t done = get_event(e);
+    CK(cudaEventRecord(done, st));
+    e->appends.push_back({base, done});
+    return 0;
+}
+
+// divide_rounds of [first, first+n) in one launch of k_stream_divide (swirld_stream.cuh)
+StreamParams stream_params(const sw_engine *e, int first, int n) {
+    StreamParams S{};
+    S.M = e->M; S.first = first; S.n = n; S.Rcap = e->Rcap; S.NJ = e->NJ;
+    S.p0 = e->d_p0; S.p1 = e->d_p1; S.creator = e->d_creator; S.seq = e->d_seq; S.row = e->d_row; S.round = e->d_round;
+    S.wit = e->d_wit; S.W = e->d_W; S.Wf = e->d_Wf; S.SM = e->d_SM; S.S = e->d_S; S.SMw = e->d_SMw; S.Sw = e->d_Sw;
+    S.coin = e->d_coin; S.sig = e->d_sig; S.stake = e->d_stake; S.tot2 = 2 * e->tot; S.scal = e->d_scal;
+    S.ctot = e->d_rbtot; S.gchain = e->d_gchain; S.carry = e->d_cs_carry; S.ring = RB_RING;
+    return S;
+}
+int stream_threads(int M) { return std::min(1024, std::max(32, (M + 31) / 32 * 32)); }
+size_t stream_smem(int M) { return (size_t)M * 8 + 32 * 8 + (size_t)3 * M * 4 + 32 * 4; }
+
+// what a call on the streaming path leaves behind: its rows are complete (written on the compute stream)
+int stream_divided(sw_engine *e, int n) {
+    e->n_rowed = e->n_divided + n;
+    CK(cudaEventRecord(e->scan_ev, e->stream));
+    e->scan_ev_set = true;
+    e->stats.events_divided += n;
+    e->n_divided += n;
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
 
-int sw_version(void) { return 202; }
+int sw_version(void) { return 203; }
 
 const char *sw_last_error(const sw_engine *e) { return e ? e->err.c_str() : g_create_error.c_str(); }
 
@@ -845,6 +977,10 @@ void sw_destroy(sw_engine *e) {
     if (e->view_ev) cudaEventDestroy(e->view_ev);
     if (e->d_views) cudaFree(e->d_views);
     if (e->d_rcviews) cudaFree(e->d_rcviews);
+    if (e->d_stviews) cudaFree(e->d_stviews);
+    for (auto ev : e->bstage_ev) if (ev) cudaEventDestroy(ev);
+    if (e->h_bstage) cudaFreeHost(e->h_bstage);
+    if (e->d_bstage) cudaFree(e->d_bstage);
     if (e->d_vbuf) cudaFree(e->d_vbuf);
     if (e->h_vbuf) cudaFreeHost(e->h_vbuf);
     for (auto ev : e->stage_ev) if (ev) cudaEventDestroy(ev);
@@ -919,42 +1055,8 @@ int sw_append(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const i
     if (n == 0) return SW_OK;
     if ((i64)e->n_events + n > e->cap) return fail(e, SW_E_CAPACITY, "capacity_events=%d exceeded", e->cap);
     CK(cudaSetDevice(e->device));
-    const int base = e->n_events;
-    // graph-shape checks of is_valid_event (swirld.py:104-108) + the fork-free contract
-    std::vector<int32_t> head_save(e->h_head), count_save(e->h_count);
-    e->h_creator.resize((size_t)base + n);
-    int rc = SW_OK;
-    int next_snap = (base / sw_engine::SNAP + 1) * sw_engine::SNAP;
-    for (int j = 0; j < n && rc == SW_OK; j++) {
-        const int i = base + j, c = creator[j], a = p0[j], b = p1[j];
-        if (c < 0 || c >= e->M) { rc = fail(e, SW_E_ARG, "event %d: creator %d out of range", i, c); break; }
-        e->h_stale[i] = 0;
-        if (a < 0 && b < 0) {
-            if (e->h_head[c] >= 0) { rc = fail(e, SW_E_FORK, "event %d: second root of member %d", i, c); break; }
-            e->h_height[i] = 0;                                          // swirld.py:117-118
-        } else {
-            if (a < 0 || b < 0 || a >= i || b >= i) { rc = fail(e, SW_E_PARENT, "event %d: parents (%d,%d) unknown", i, a, b); break; }
-            if (e->h_creator[a] != c) { rc = fail(e, SW_E_PARENT, "event %d: self-parent %d has another creator", i, a); break; }
-            if (e->h_creator[b] == c) { rc = fail(e, SW_E_PARENT, "event %d: other-parent %d has the same creator", i, b); break; }
-            if (e->h_head[c] != a) { rc = fail(e, SW_E_FORK, "event %d: self-parent %d is not member %d's latest event (fork)", i, a, c); break; }
-            e->h_height[i] = std::max(e->h_height[a], e->h_height[b]) + 1;   // swirld.py:120
-            e->h_stale[i] = e->h_head[e->h_creator[b]] != b;             // "near fork": an older event of the peer
-        }
-        e->h_creator[i] = c;
-        e->h_head[c] = i;
-        e->h_seq[i] = e->h_count[c]++;
-        if (i + 1 == next_snap) { push_snapshot(e, i + 1, e->h_count); next_snap += sw_engine::SNAP; }
-    }
-    if (rc == SW_OK) {
-        e->h_stale_cum.resize((size_t)base + n + 1);
-        for (int j = 0; j < n; j++) e->h_stale_cum[base + j + 1] = e->h_stale_cum[base + j] + e->h_stale[base + j];
-    }
-    if (rc != SW_OK) {
-        e->h_head = head_save; e->h_count = count_save;
-        e->h_creator.resize(base);
-        while (!e->snap_at.empty() && e->snap_at.back() > base) { e->snap_at.pop_back(); e->snap_cnt.resize(e->snap_at.size() * e->M); }
-        return rc;
-    }
+    int rc = append_validate(e, n, p0, p1, creator);
+    if (rc < 0) return rc;
     // The copies go to their own stream: they touch only the new rows, so they overlap the kernels of
     // earlier chunks still running on the compute stream; later compute work waits for them.
     cudaStream_t cs = e->copy_stream;
@@ -965,47 +1067,84 @@ int sw_append(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const i
         e->stage_next = (si + 1) % sw_engine::STAGE_SLOTS;
         CK(cudaEventSynchronize(e->stage_ev[si]));                       // (the copy that used this slot eight appends ago)
         uint8_t *hs = e->h_stage + slot * si, *ds = e->d_stage + slot * si;
-        int32_t *ints = reinterpret_cast<int32_t *>(hs);
-        memcpy(ints, p0, sizeof(int32_t) * n); memcpy(ints + n, p1, sizeof(int32_t) * n); memcpy(ints + 2 * n, creator, sizeof(int32_t) * n);
-        memcpy(ints + 3 * n, e->h_seq + base, sizeof(int32_t) * n); memcpy(ints + 4 * n, e->h_height + base, sizeof(int32_t) * n);
-        uint8_t *pt = hs + unpack_off_t(n);
-        memcpy(pt, t, sizeof(double) * n); memcpy(pt + (size_t)8 * n, sig, (size_t)64 * n); memcpy(pt + (size_t)72 * n, e->h_stale + base, (size_t)n);
+        const UnpackParams U = append_pack(e, n, p0, p1, creator, t, sig, hs, ds);
         CK(cudaMemcpyAsync(ds, hs, unpack_bytes(n), cudaMemcpyHostToDevice, cs));
         CK(cudaEventRecord(e->stage_ev[si], cs));
-        UnpackParams U{};
-        U.base = base; U.n = n; U.stage = ds; U.p0 = e->d_p0; U.p1 = e->d_p1; U.creator = e->d_creator; U.seq = e->d_seq;
-        U.height = e->d_height; U.t = e->d_t; U.sig = e->d_sig; U.stale = e->d_stale;
         k_unpack<<<1, 256, 0, cs>>>(U);
         CK(cudaGetLastError());
         e->stats.kernel_launches += 1;
-    } else {
-        CK(cudaMemcpyAsync(e->d_p0 + base, p0, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
-        CK(cudaMemcpyAsync(e->d_p1 + base, p1, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
-        CK(cudaMemcpyAsync(e->d_creator + base, creator, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
-        CK(cudaMemcpyAsync(e->d_t + base, t, sizeof(double) * n, cudaMemcpyHostToDevice, cs));
-        CK(cudaMemcpyAsync(e->d_sig + (size_t)base * 64, sig, (size_t)64 * n, cudaMemcpyHostToDevice, cs));
-        CK(cudaMemcpyAsync(e->d_seq + base, e->h_seq + base, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
-        CK(cudaMemcpyAsync(e->d_height + base, e->h_height + base, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
-        CK(cudaMemcpyAsync(e->d_stale + base, e->h_stale + base, (size_t)n, cudaMemcpyHostToDevice, cs));
+    } else if (append_copy(e, n, p0, p1, creator, t, sig) < 0) return SW_E_CUDA;
+    return append_commit(e, n, cs);
+}
+
+// Node.add_event for B node-views in one call.  Every view is validated as sw_append validates it; the views of at most
+// STAGE_EVENTS events go over packed in ONE block (their parameters first) and are scattered by ONE k_unpack_views, on
+// the first engine's copy stream; larger views make the copies their sw_append makes, on their own copy streams.
+int sw_batch_append(sw_engine *const *engines, int B, const int *offsets, const int32_t *p0, const int32_t *p1,
+                    const int32_t *creator, const double *t, const uint8_t *sig, int32_t *rc_out) {
+    sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
+    if (!e || !offsets || !rc_out) return fail(e, SW_E_ARG, "bad argument");
+    int rc = check_views(engines, B, "sw_batch_append", false);
+    if (rc < 0) return rc;
+    if (offsets[0] < 0) return fail(e, SW_E_ARG, "sw_batch_append: offsets[0] = %d", offsets[0]);
+    for (int v = 0; v < B; v++)
+        if (offsets[v + 1] < offsets[v])
+            return fail(e, SW_E_ARG, "sw_batch_append: offsets[%d] = %d > offsets[%d] = %d", v, offsets[v], v + 1, offsets[v + 1]);
+    if (offsets[B] > offsets[0] && (!p0 || !p1 || !creator || !t || !sig)) return fail(e, SW_E_ARG, "bad argument");
+    CK(cudaSetDevice(e->device));
+    // 1. every view's checks; a view that fails them keeps its state and its error
+    std::vector<int> packed;
+    size_t bytes = 0;
+    int first_err = SW_OK;
+    for (int v = 0; v < B; v++) {
+        sw_engine *x = engines[v];
+        const int o = offsets[v], n = offsets[v + 1] - o;
+        int r = n > 0 ? append_validate(x, n, p0 + o, p1 + o, creator + o) : SW_OK;
+        rc_out[v] = r;
+        if (r < 0) { if (first_err == SW_OK) first_err = r; continue; }
+        if (n == 0) continue;
+        if (n <= sw_engine::STAGE_EVENTS) { packed.push_back(v); bytes += (unpack_bytes(n) + 15) & ~(size_t)15; }
+        else if (append_copy(x, n, p0 + o, p1 + o, creator + o, t + o, sig + (size_t)64 * o) < 0 || append_commit(x, n, x->copy_stream) < 0) {
+            e->err = x->err;
+            return SW_E_CUDA;
+        }
     }
-    // rows are up to date and the batch is big: scan it now, beside the kernels of the previous chunk
-    // (several ranks: the scan holds cross-GPU barriers; it must not run beside a round kernel that fills every SM while
-    //  waiting for the same peer -- scans stay on the compute stream then)
-    const bool eager = e->n_rowed == base && n >= 4096 && e->nranks == 1;
-    e->stats.h2d_bytes += (i64)n * (5 * 4 + 1 + 8 + 64);
-    e->stats.events += n;
-    e->n_events += n;
-    push_append_snapshot(e);
-    if (eager) {
-        if (e->scan_ev_set) CK(cudaStreamWaitEvent(cs, e->scan_ev, 0));     // never beside a scan on the compute stream
-        int rc2 = cansee_scan(e, cs, e->n_events);
-        if (rc2 < 0) return rc2;
+    if (packed.empty()) return first_err;
+    bytes += align256(sizeof(UnpackParams) * packed.size());
+    // 2. the packed views: one slot of the first engine's ring, one copy, one scatter kernel
+    cudaStream_t cs = e->copy_stream;
+    if (bytes > e->bstage_slot) {
+        CK(cudaStreamSynchronize(cs));                                   // (the copies and kernels that read the old ring)
+        if (e->h_bstage) { CK(cudaFreeHost(e->h_bstage)); e->h_bstage = nullptr; }
+        if (e->d_bstage) { CK(cudaFree(e->d_bstage)); e->d_bstage = nullptr; }
+        const size_t slot = align256(std::max(bytes, 2 * e->bstage_slot));
+        e->bstage_slot = 0;
+        CK(cudaMallocHost((void **)&e->h_bstage, slot * sw_engine::STAGE_SLOTS));
+        CK(cudaMalloc((void **)&e->d_bstage, slot * sw_engine::STAGE_SLOTS));
+        e->bstage_slot = slot;
+        for (auto &ev : e->bstage_ev) if (!ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     }
-    // the compute stream waits for this batch only when a call first touches it (wait_appends)
-    cudaEvent_t done = get_event(e);
-    CK(cudaEventRecord(done, cs));
-    e->appends.push_back({base, done});
-    return SW_OK;
+    const int si = e->bstage_next;
+    e->bstage_next = (si + 1) % sw_engine::STAGE_SLOTS;
+    CK(cudaEventSynchronize(e->bstage_ev[si]));                          // (the copy that used this slot eight calls ago)
+    uint8_t *hs = e->h_bstage + e->bstage_slot * si, *ds = e->d_bstage + e->bstage_slot * si;
+    UnpackParams *U = reinterpret_cast<UnpackParams *>(hs);
+    size_t off = align256(sizeof(UnpackParams) * packed.size());
+    for (size_t i = 0; i < packed.size(); i++) {
+        sw_engine *x = engines[packed[i]];
+        const int o = offsets[packed[i]], n = offsets[packed[i] + 1] - o;
+        U[i] = append_pack(x, n, p0 + o, p1 + o, creator + o, t + o, sig + (size_t)64 * o, hs + off, ds + off);
+        off += (unpack_bytes(n) + 15) & ~(size_t)15;
+    }
+    CK(cudaMemcpyAsync(ds, hs, off, cudaMemcpyHostToDevice, cs));
+    CK(cudaEventRecord(e->bstage_ev[si], cs));
+    k_unpack_views<<<(int)packed.size(), 256, 0, cs>>>(reinterpret_cast<const UnpackParams *>(ds));
+    CK(cudaGetLastError());
+    e->stats.kernel_launches += 1;
+    // each view's pending-append event comes from its own pool (wait_appends returns it there)
+    for (int v : packed)
+        if (append_commit(engines[v], offsets[v + 1] - offsets[v], cs) < 0) { e->err = engines[v]->err; return SW_E_CUDA; }
+    return first_err;
 }
 
 int sw_divide_rounds(sw_engine *e, int first, int n) {
@@ -1017,28 +1156,17 @@ int sw_divide_rounds(sw_engine *e, int first, int n) {
     if (n <= sw_engine::STREAM_N && e->n_rowed == first) {
         // the reference's own cadence (one sync per call): the whole of divide_rounds in ONE launch (swirld_stream.cuh)
         if (wait_appends(e, first + n) < 0) return SW_E_CUDA;
-        const int M = e->M;
-        StreamParams S{};
-        S.M = M; S.first = first; S.n = n; S.Rcap = e->Rcap; S.NJ = e->NJ;
-        S.p0 = e->d_p0; S.p1 = e->d_p1; S.creator = e->d_creator; S.seq = e->d_seq; S.row = e->d_row; S.round = e->d_round;
-        S.wit = e->d_wit; S.W = e->d_W; S.Wf = e->d_Wf; S.SM = e->d_SM; S.S = e->d_S; S.SMw = e->d_SMw; S.Sw = e->d_Sw;
-        S.coin = e->d_coin; S.sig = e->d_sig; S.stake = e->d_stake; S.tot2 = 2 * e->tot; S.scal = e->d_scal;
-        S.ctot = e->d_rbtot; S.gchain = e->d_gchain; S.carry = e->d_cs_carry; S.ring = RB_RING;
-        const int threads = std::min(1024, std::max(32, (M + 31) / 32 * 32));
-        const size_t smem = (size_t)M * 8 + 32 * 8 + (size_t)3 * M * 4 + 32 * 4;
+        const StreamParams S = stream_params(e, first, n);
+        const int threads = stream_threads(e->M);
+        const size_t smem = stream_smem(e->M);
         {
             Span sp(e, 0);
             if (e->wide) k_stream_divide<true><<<1, threads, smem, e->stream>>>(S);
             else k_stream_divide<false><<<1, threads, smem, e->stream>>>(S);
             CK(cudaGetLastError());
         }
-        e->n_rowed = first + n;
-        CK(cudaEventRecord(e->scan_ev, e->stream));         // (it wrote can_see rows and the carry heads on the compute stream)
-        e->scan_ev_set = true;
         e->stats.kernel_launches += 1;
-        e->stats.events_divided += n;
-        e->n_divided += n;
-        return SW_OK;
+        return stream_divided(e, n);         // (it wrote can_see rows and the carry heads on the compute stream)
     }
     if (first + n > e->n_rowed) {
         // rows are behind (small appends, or after sw_rewind): scan everything appended so far, here -- after the
@@ -1062,19 +1190,11 @@ int sw_divide_rounds(sw_engine *e, int first, int n) {
     return SW_OK;
 }
 
-// Node.divide_rounds for B independent node-views at once (M <= 64, same member count, same device): everything of a
-// view runs on the view's own stream, except the round kernels, which advance side by side in ONE cooperative launch.
-int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, const int *n) {
-    sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
-    if (!e || !first || !n) return fail(e, SW_E_ARG, "bad argument");
-    for (int v = 0; v < B; v++) {
-        sw_engine *x = engines[v];
-        if (!x || x->wide || x->M != e->M || x->device != e->device || x->unit != e->unit)
-            return fail(e, SW_E_UNSUPPORTED, "sw_batch_divide_rounds: the views must be M <= 64 engines of one shape on one device");
-        if (n[v] <= 0 || first[v] != x->n_divided || first[v] + n[v] > x->n_events)
-            return fail(e, SW_E_ARG, "sw_batch_divide_rounds: view %d: bad range [%d,%d)", v, first[v], first[v] + n[v]);
-    }
-    CK(cudaSetDevice(e->device));
+// The chunk path of sw_batch_divide_rounds (M <= 64, one stake shape): every step of a view runs on the view's own
+// stream, except the round kernels, which advance side by side in ONE cooperative launch on the stream of `e`, the
+// first engine of the batch (its parameter buffers; it is charged the timings and launches).
+static int chunk_views(sw_engine *e, sw_engine *const *engines, int B, const int *first, const int *n) {
+    const bool unit = engines[0]->unit;
     const int per_launch = e->n_sm;                         // (one CTA per view at least: its warps loop over its chains)
     if (B > e->views_cap) {
         if (e->d_views) cudaFree(e->d_views);
@@ -1124,13 +1244,13 @@ int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, c
                 cudaLaunchAttribute at[1];
                 rc_launch_config(cfg, at, nv, e->stream);
                 const RcParams *qv = e->d_rcviews + v0;
-                if (e->unit) CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster_views<true>, qv));
+                if (unit) CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster_views<true>, qv));
                 else CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster_views<false>, qv));
                 e->stats.kernel_launches += 1;
                 e->stats.rounds_cluster_launches += 1;
             }
-            void *fn = e->NC == 1 ? (e->unit ? (void *)k_rounds_batch_views<1, true> : (void *)k_rounds_batch_views<1, false>)
-                                  : (e->unit ? (void *)k_rounds_batch_views<2, true> : (void *)k_rounds_batch_views<2, false>);
+            void *fn = e->NC == 1 ? (unit ? (void *)k_rounds_batch_views<1, true> : (void *)k_rounds_batch_views<1, false>)
+                                  : (unit ? (void *)k_rounds_batch_views<2, true> : (void *)k_rounds_batch_views<2, false>);
             CK(cudaLaunchCooperativeKernel(fn, dim3(nv * G), dim3(RB_THREADS), args, 0, e->stream));
             e->stats.kernel_launches += 1;
             cudaEventRecord(b, e->stream);
@@ -1146,6 +1266,63 @@ int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, c
             x->n_divided += n[v];
         }
     }
+    return SW_OK;
+}
+
+// Node.divide_rounds for B independent node-views at once: every view takes the path its single call would take.  The
+// views whose call takes the one-launch path join ONE k_stream_divide_views launch (any M, any stakes); the others go
+// through chunk_views.
+int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, const int *n) {
+    sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
+    if (!e || !first || !n) return fail(e, SW_E_ARG, "bad argument");
+    int rc = check_views(engines, B, "sw_batch_divide_rounds", true);
+    if (rc < 0) return rc;
+    std::vector<sw_engine *> sv, cv;                  // the views on the streaming path, and on the chunk path
+    std::vector<int> sn, cfirst, cn;
+    for (int v = 0; v < B; v++) {
+        sw_engine *x = engines[v];
+        if (n[v] <= 0 || first[v] != x->n_divided || first[v] + n[v] > x->n_events)
+            return fail(e, SW_E_ARG, "sw_batch_divide_rounds: view %d: bad range [%d,%d)", v, first[v], first[v] + n[v]);
+        if (n[v] <= sw_engine::STREAM_N && x->n_rowed == first[v]) { sv.push_back(x); sn.push_back(n[v]); }
+        else { cv.push_back(x); cfirst.push_back(first[v]); cn.push_back(n[v]); }
+    }
+    for (sw_engine *x : cv)
+        if (x->wide || x->unit != cv[0]->unit)
+            return fail(e, SW_E_UNSUPPORTED, "sw_batch_divide_rounds: views whose calls bring more than %d events must be M <= 64 engines of one stake shape", sw_engine::STREAM_N);
+    CK(cudaSetDevice(e->device));
+    const int S = (int)sv.size();
+    if (S > 0) {
+        std::vector<StreamParams> Sv(S);
+        for (int i = 0; i < S; i++) {
+            sw_engine *x = sv[i];
+            if (wait_appends(x, x->n_divided + sn[i]) < 0) { e->err = x->err; return SW_E_CUDA; }
+            Sv[i] = stream_params(x, x->n_divided, sn[i]);
+        }
+        if (views_enter(e, sv.data(), S) < 0) return SW_E_CUDA;
+        if (S > e->stviews_cap) {
+            if (e->d_stviews) { CK(cudaStreamSynchronize(e->stream)); CK(cudaFree(e->d_stviews)); e->d_stviews = nullptr; }
+            e->stviews_cap = 0;
+            CK(cudaMalloc((void **)&e->d_stviews, sizeof(StreamParams) * S));
+            e->stviews_cap = S;
+        }
+        CK(cudaMemcpyAsync(e->d_stviews, Sv.data(), sizeof(StreamParams) * S, cudaMemcpyHostToDevice, e->stream));
+        e->stats.h2d_bytes += sizeof(StreamParams) * S;
+        {
+            Span sp(e, 0);
+            if (e->wide) k_stream_divide_views<true><<<S, stream_threads(e->M), stream_smem(e->M), e->stream>>>(e->d_stviews);
+            else k_stream_divide_views<false><<<S, stream_threads(e->M), stream_smem(e->M), e->stream>>>(e->d_stviews);
+            CK(cudaGetLastError());
+        }
+        e->stats.kernel_launches += 1;
+        // each view's later work runs after the batch: no copy, no host synchronisation
+        if (!e->view_ev) CK(cudaEventCreateWithFlags(&e->view_ev, cudaEventDisableTiming));
+        CK(cudaEventRecord(e->view_ev, e->stream));
+        for (int i = 0; i < S; i++) {
+            if (sv[i] != e) CK(cudaStreamWaitEvent(sv[i]->stream, e->view_ev, 0));
+            if (stream_divided(sv[i], sn[i]) < 0) { e->err = sv[i]->err; return SW_E_CUDA; }
+        }
+    }
+    if (!cv.empty()) return chunk_views(e, cv.data(), (int)cv.size(), cfirst.data(), cn.data());
     return SW_OK;
 }
 
@@ -1239,7 +1416,7 @@ int sw_find_order(sw_engine *e, const int32_t *new_c, int n) {
 int sw_batch_decide_fame(sw_engine *const *engines, int B, int32_t *new_c_out, int cap, int32_t *count_out) {
     sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
     if (!e || cap < 0 || (cap > 0 && !new_c_out) || !count_out) return fail(e, SW_E_ARG, "bad argument");
-    int rc = check_views(engines, B, "sw_batch_decide_fame");
+    int rc = check_views(engines, B, "sw_batch_decide_fame", true);
     if (rc < 0) return rc;
     for (int v = 0; v < B; v++)
         if (engines[v]->n_divided == 0)
@@ -1304,7 +1481,7 @@ int sw_batch_decide_fame(sw_engine *const *engines, int B, int32_t *new_c_out, i
 int sw_batch_find_order(sw_engine *const *engines, int B, const int32_t *new_c, const int *offsets, int32_t *count_out) {
     sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
     if (!e || !offsets || !count_out) return fail(e, SW_E_ARG, "bad argument");
-    int rc = check_views(engines, B, "sw_batch_find_order");
+    int rc = check_views(engines, B, "sw_batch_find_order", true);
     if (rc < 0) return rc;
     if (offsets[0] < 0) return fail(e, SW_E_ARG, "sw_batch_find_order: offsets[0] = %d", offsets[0]);
     for (int v = 0; v < B; v++)

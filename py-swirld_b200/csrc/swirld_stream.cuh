@@ -46,7 +46,7 @@ __device__ __forceinline__ i64 st_block_sum(i64 v, i64 *red) {
 }
 
 template <bool WIDE>
-__global__ void __launch_bounds__(1024) k_stream_divide(StreamParams P) {
+__device__ __forceinline__ void stream_divide(const StreamParams &P) {
     extern __shared__ int st_smem[];
     const int M = P.M, c = threadIdx.x, lane = c & 31;
     i64 *stake_s = reinterpret_cast<i64 *>(st_smem);       // [M]
@@ -147,6 +147,21 @@ __global__ void __launch_bounds__(1024) k_stream_divide(StreamParams P) {
     if (c == 0 && P.n > 0) P.scal[SC_MAX_ROUND] = max_round;
 }
 
+template <bool WIDE>
+__global__ void __launch_bounds__(1024) k_stream_divide(StreamParams P) { stream_divide<WIDE>(P); }
+
+// sw_batch_divide_rounds: one CTA per node-view (blockIdx.x), every view's call of a handful of events in one launch.
+// The views share M (so the thread count and the dynamic shared memory); stakes and coin periods are per view.
+template <bool WIDE>
+__global__ void __launch_bounds__(1024) k_stream_divide_views(const StreamParams *Pv) {
+    __shared__ StreamParams P;
+    static_assert(sizeof(StreamParams) % 8 == 0, "staged in 8-byte words");
+    for (int i = threadIdx.x; i < (int)(sizeof(StreamParams) / 8); i += blockDim.x)     // (a struct copy goes through the stack)
+        reinterpret_cast<u64 *>(&P)[i] = reinterpret_cast<const u64 *>(Pv + blockIdx.x)[i];
+    __syncthreads();
+    stream_divide<WIDE>(P);
+}
+
 // the event columns of a small append arrive as ONE packed block: scatter it to the SoA columns
 struct UnpackParams {
     int base, n;
@@ -157,7 +172,7 @@ struct UnpackParams {
 };
 __host__ __device__ inline size_t unpack_off_t(int n) { return (size_t)20 * n + ((8 - (20 * (size_t)n) % 8) % 8); }
 __host__ __device__ inline size_t unpack_bytes(int n) { return unpack_off_t(n) + (size_t)8 * n + (size_t)64 * n + n; }
-__global__ void k_unpack(UnpackParams P) {
+__device__ __forceinline__ void unpack(const UnpackParams &P) {
     const int n = P.n;
     const int32_t *ints = reinterpret_cast<const int32_t *>(P.stage);
     const double *tt = reinterpret_cast<const double *>(P.stage + unpack_off_t(n));
@@ -168,4 +183,13 @@ __global__ void k_unpack(UnpackParams P) {
         P.t[P.base + i] = tt[i]; P.stale[P.base + i] = stl[i];
     }
     for (int i = threadIdx.x; i < 64 * n; i += blockDim.x) P.sig[(size_t)P.base * 64 + i] = sg[i];
+}
+__global__ void k_unpack(UnpackParams P) { unpack(P); }
+
+// sw_batch_append: one CTA per node-view (blockIdx.x); every view's `stage` points into one packed block
+__global__ void k_unpack_views(const UnpackParams *Uv) {
+    __shared__ UnpackParams P;
+    if (threadIdx.x == 0) P = Uv[blockIdx.x];
+    __syncthreads();
+    unpack(P);
 }

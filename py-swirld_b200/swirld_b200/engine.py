@@ -26,7 +26,7 @@ SYMBOLS = [
     "sw_get_witness_table", "sw_get_consensus", "sw_get_transactions", "sw_get_idx", "sw_get_height",
     "sw_sync", "sw_stats", "sw_flush_l2", "sw_version", "sw_debug_counters", "sw_peer_handle", "sw_peer_connect",
     "sw_save", "sw_load", "sw_members", "sw_ingest", "sw_lookup", "sw_batch_divide_rounds",
-    "sw_batch_decide_fame", "sw_batch_find_order",
+    "sw_batch_decide_fame", "sw_batch_find_order", "sw_batch_append",
 ]
 
 
@@ -91,6 +91,7 @@ def load_library(path: str = LIB_PATH):
     L.sw_batch_divide_rounds.argtypes = [vp, i32, vp, vp]
     L.sw_batch_decide_fame.argtypes = [vp, i32, vp, i32, vp]
     L.sw_batch_find_order.argtypes = [vp, i32, vp, vp, vp]
+    L.sw_batch_append.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp]
     L.sw_save.argtypes = [vp, C.c_char_p]
     L.sw_load.argtypes = [C.c_char_p, i32, i32, P(vp)]
     _lib = L
@@ -320,7 +321,9 @@ class Engine:
 
 
 def batch_divide_rounds(engines, firsts, counts):
-    """sw_batch_divide_rounds: divide_rounds of several independent node-views (M <= 64) in one call."""
+    """sw_batch_divide_rounds: divide_rounds of several independent node-views (one member count, one kernel family,
+    one device) in one call.  Calls of at most 16 events run in one launch for all views at any M, whatever their
+    stakes; larger calls need M <= 64 and one stake shape among them, else the whole call is refused."""
     B = len(engines)
     arr = (C.c_void_p * B)(*[e._h for e in engines])
     f = np.ascontiguousarray(firsts, np.int32)
@@ -364,6 +367,30 @@ def batch_decide_fame(engines):
     if rc < 0 and not (cnt < 0).any():
         engines[0]._chk(rc)                # refused as a whole: nothing ran, count_out was not written
     return _per_view("batch_decide_fame", engines, [out[v, :max(0, int(n))].tolist() for v, n in enumerate(cnt)], cnt)
+
+
+def batch_append(engines, columns):
+    """sw_batch_append: Engine.append of several node-views (one device) in one call; columns[v] = (p0, p1, creator,
+    t, sig) of view v.  Returns the events each view appended.  Argument errors raise at once; a view whose events
+    append would refuse appends nothing, and those failures raise as an ExceptionGroup after every view has appended
+    (see _per_view)."""
+    B = len(engines)
+    assert len(columns) == B
+    if B == 0:
+        return []
+    cols = [[np.asarray(c) for c in view] for view in columns]
+    ns = [len(c[0]) for c in cols]
+    for c, n in zip(cols, ns):
+        assert len(c[1]) == n and len(c[2]) == n and len(c[3]) == n and c[4].size == 64 * n
+    cat = [np.ascontiguousarray(np.concatenate([c[k].reshape(-1) for c in cols]), dt)
+           for k, dt in enumerate((np.int32, np.int32, np.int32, np.float64, np.uint8))]
+    offs = np.zeros(B + 1, np.int32)
+    offs[1:] = np.cumsum(ns)
+    rcs = np.zeros(B, np.int32)
+    rc = engines[0]._lib.sw_batch_append(_handles(engines), B, _ptr(offs), *[_ptr(a) for a in cat], _ptr(rcs))
+    if rc < 0 and not (rcs < 0).any():
+        engines[0]._chk(rc)                # refused as a whole: nothing ran, rc_out was not written
+    return _per_view("batch_append", engines, list(ns), rcs)
 
 
 def batch_find_order(engines, new_cs):
