@@ -122,18 +122,15 @@ struct sw_engine {
     int seg_cap = 0;
     void *d_flush = nullptr;
     size_t flush_bytes = 0;
-    // small appends (the reference's cadence: one sync per call): one packed copy instead of eight
+    // small appends (the reference's cadence: one sync per call): one packed copy instead of eight, from a ring of pinned
+    // slots -- one view's columns (sw_append), or a batch's parameters and columns (sw_batch_append, on its first
+    // engine).  h_vbuf cannot hold them: the batched fame and order calls of the same turn rewrite it on the host before
+    // the asynchronous copy from it would have run.
     static constexpr int STAGE_SLOTS = 8, STAGE_EVENTS = 64;
     uint8_t *h_stage = nullptr, *d_stage = nullptr;
+    size_t stage_bytes = 0;       // per slot
     cudaEvent_t stage_ev[STAGE_SLOTS] = {nullptr};
     int stage_next = 0;
-    // sw_batch_append (owned by the first engine of a batch): the packed small views of one call, [parameters][columns],
-    // in a ring of its own.  h_vbuf cannot hold them: the batched fame and order calls of the same turn rewrite it on
-    // the host before the asynchronous copy from it would have run.
-    uint8_t *h_bstage = nullptr, *d_bstage = nullptr;
-    size_t bstage_slot = 0;       // bytes per slot
-    cudaEvent_t bstage_ev[STAGE_SLOTS] = {nullptr};
-    int bstage_next = 0;
     static constexpr int STREAM_N = 16;              // divide_rounds calls of at most this many events take the one-launch path
     StreamParams *d_stviews = nullptr;               // sw_batch_divide_rounds: the parameters of the views on that path
     int stviews_cap = 0;
@@ -592,18 +589,48 @@ int divide_rounds_wide(sw_engine *e, int first, int n) {
 
 size_t w_fame_smem(int NJ, int M) { return (size_t)(32 * NJ + 64) * sizeof(int) + (size_t)(32 + M) * sizeof(i64); }
 
-template <int NJ>
-int fame_rounds_wide(sw_engine *e, const FameParams &P) {
+template <int NJ, class Src>
+int fame_rounds_wide(sw_engine *e, Src P, int B) {
     const int parts = (e->M + FW_THREADS - 1) / FW_THREADS;
-    k_w_fame_rounds<NJ><<<(2 * e->n_sm / parts + 1) * parts, FW_THREADS, w_fame_smem(NJ, e->M), e->stream>>>(P);
+    k_w_fame_rounds<NJ><<<dim3((2 * e->n_sm / parts + 1) * parts, B), FW_THREADS, w_fame_smem(NJ, e->M), e->stream>>>(P);
     return 0;
 }
 
-// B views: `x` CTA groups of `parts` CTAs per view
-template <int NJ>
-int fame_rounds_wide_views(sw_engine *e, const FameParams *Pv, int B, int x) {
-    const int parts = (e->M + FW_THREADS - 1) / FW_THREADS;
-    k_w_fame_rounds_views<NJ><<<dim3(x * parts, B), FW_THREADS, w_fame_smem(NJ, e->M), e->stream>>>(Pv);
+// The fame kernels of B views: P is one view's parameters (B = 1) or the device array of B views' (swirld_kernels.cuh,
+// params).  Every view gets the grid its single call launches (the kernels are latency-bound; spare CTAs exit at once).
+template <class Src>
+void fame_kernels(sw_engine *e, Src P, int B) {
+    if (e->wide) {
+        k_fame_begin<<<dim3(1, B), 32, 0, e->stream>>>(P);
+        SW_NJ(fame_rounds_wide, e, P, B);
+        k_fame_finish<<<dim3(1, B), 1024, 0, e->stream>>>(P);
+        e->stats.kernel_launches += 3;
+    } else {
+        k_fame_rounds<<<dim3(2 * e->n_sm, B), 256, 0, e->stream>>>(P);
+        e->stats.kernel_launches += 1;
+    }
+}
+
+// decide_fame copies the scalars and (speculatively) the first new consensus rounds together: one copy, one
+// synchronisation (a 64-member chunk of 64 K events brings about 90 new rounds: room for 64 only would add a copy and a
+// synchronisation to every such call)
+constexpr int FAME_SPEC = 1024;
+int fame_spec(const sw_engine *e) { return std::min(e->Rcap, FAME_SPEC); }
+
+// What decide_fame does once that copy is in h_scal: `r` = the error the device found, or the count of new rounds,
+// which go to `out` (a second copy when more came than the first one held).  Returns < 0 only when a copy fails.
+int fame_result(sw_engine *e, int32_t *out, int cap, int &r) {
+    r = device_error(e);
+    if (r < 0) return 0;
+    const int cnt = e->h_scal[SC_NEWC];
+    if (cnt > cap) { r = fail(e, SW_E_ARG, "decide_fame: %d new consensus rounds do not fit cap=%d", cnt, cap); return 0; }
+    if (cnt > fame_spec(e)) {
+        CK(cudaMemcpyAsync(e->h_newc, e->d_newc, sizeof(int32_t) * cnt, cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaStreamSynchronize(e->stream));
+        e->stats.d2h_bytes += sizeof(int32_t) * cnt;
+    }
+    if (cnt > 0) memcpy(out, e->h_newc, sizeof(int32_t) * cnt);
+    r = cnt;
     return 0;
 }
 
@@ -642,6 +669,45 @@ OrderParams order_params(const sw_engine *e, int n, const int32_t *rounds) {
     return P;
 }
 
+// sorted(new_c) (swirld.py:283) of n rounds, in place; false when one is not in the round table (`bad`: the first)
+bool sort_rounds(const sw_engine *e, int32_t *rs, int n, int &bad) {
+    std::sort(rs, rs + n);
+    for (int i = 0; i < n; i++)
+        if (rs[i] < 0 || rs[i] >= e->Rcap) { bad = rs[i]; return false; }
+    return true;
+}
+
+// The five order kernels of A views (P: as fame_kernels), every view's grid sized from `maxn` rounds.  The number of
+// newly ordered events stays on the device: the time and sort kernels read it there, the host learns it from the
+// copy at the end of the call.
+template <class Src>
+void order_kernels(sw_engine *e, Src P, int A, int maxn) {
+    const int M = e->M;
+    const int list_ctas = std::max(1, std::min(4 * e->n_sm, (int)(((size_t)maxn * e->MS + 255) / 256)));
+    if (e->wide) {
+        k_w_order_rounds<<<dim3(maxn, A), 1024, (size_t)3 * M * sizeof(int), e->stream>>>(P);
+        k_w_order_cuts<<<dim3(1, A), 1024, (size_t)2 * M * sizeof(int), e->stream>>>(P);
+        k_w_order_list<<<dim3(list_ctas, A), 256, 0, e->stream>>>(P);
+        k_w_order_times<<<dim3(8 * e->n_sm, A), OW_WARPS * 32, (size_t)OW_WARPS * M * sizeof(u64), e->stream>>>(P);
+    } else {
+        k_order_rounds<<<dim3(maxn, A), 1024, 0, e->stream>>>(P);
+        k_order_cuts<<<dim3(1, A), 64, 0, e->stream>>>(P);
+        k_order_list<<<dim3(list_ctas, A), 256, 0, e->stream>>>(P);
+        k_order_times<<<dim3(4 * e->n_sm, A), 256, 0, e->stream>>>(P);
+    }
+    k_order_sort<<<dim3(maxn, A), 1024, 0, e->stream>>>(P);
+    e->stats.kernel_launches += 5;
+}
+
+// what find_order does once its copy of the scalars is in h_scal: the error the device found, else the events it ordered
+int order_result(sw_engine *e) {
+    const int rc = device_error(e);
+    if (rc < 0) return rc;
+    const int nbatch = e->h_scal[SC_BATCH];
+    e->n_tx += nbatch;
+    return nbatch;
+}
+
 // ---- several node-views per call (sw_batch_*)
 // The checks shared by the batched calls: they refuse the whole batch before anything runs (the message goes to the first
 // engine).  `same_shape`: the views must also share M and the kernel family (all but sw_batch_append).
@@ -676,6 +742,26 @@ int views_buffer(sw_engine *e, size_t bytes) {
 }
 
 size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// The next slot of at least `bytes` in the staging ring, once the copy that used it STAGE_SLOTS calls ago is done (a
+// larger ring replaces the ring after the copies and kernels that read it).  Returns the slot's index (< 0: an error);
+// the caller records stage_ev[slot] on the copy stream after its copy.
+int stage_slot(sw_engine *e, size_t bytes) {
+    if (bytes > e->stage_bytes) {
+        CK(cudaStreamSynchronize(e->copy_stream));
+        if (e->h_stage) { CK(cudaFreeHost(e->h_stage)); e->h_stage = nullptr; }
+        if (e->d_stage) { CK(cudaFree(e->d_stage)); e->d_stage = nullptr; }
+        const size_t slot = align256(std::max(bytes, 2 * e->stage_bytes));
+        e->stage_bytes = 0;
+        CK(cudaMallocHost((void **)&e->h_stage, slot * sw_engine::STAGE_SLOTS));
+        CK(cudaMalloc((void **)&e->d_stage, slot * sw_engine::STAGE_SLOTS));
+        e->stage_bytes = slot;
+    }
+    const int si = e->stage_next;
+    e->stage_next = (si + 1) % sw_engine::STAGE_SLOTS;
+    CK(cudaEventSynchronize(e->stage_ev[si]));
+    return si;
+}
 
 // the batch runs on the stream of `e`, the first engine: after everything each view has queued on its own
 int views_enter(sw_engine *e, sw_engine *const *views, int B) {
@@ -800,10 +886,8 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
         CK(dalloc(&e->d_lastord, MP)); CK(dalloc(&e->d_tx, cap)); CK(dalloc(&e->d_idx, cap));
         CK(dalloc(&e->d_batch_ev, cap)); CK(dalloc(&e->d_batch_seg, cap)); CK(dalloc(&e->d_perm, 2 * cap));
         CK(dalloc(&e->d_ts, cap)); CK(dalloc(&e->d_key, cap * 8));
-        const size_t slot = (unpack_bytes(sw_engine::STAGE_EVENTS) + 255) & ~(size_t)255;
-        CK(cudaMallocHost((void **)&e->h_stage, slot * sw_engine::STAGE_SLOTS));
-        CK(cudaMalloc((void **)&e->d_stage, slot * sw_engine::STAGE_SLOTS));
         for (auto &ev : e->stage_ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        if (stage_slot(e, unpack_bytes(sw_engine::STAGE_EVENTS)) < 0) return SW_E_CUDA;   // (the ring, sized for sw_append)
         CK(cudaFuncSetAttribute(k_stream_divide<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
         CK(cudaFuncSetAttribute(k_stream_divide_views<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
         CK(cudaMallocHost((void **)&e->h_scal, sizeof(int32_t) * ((size_t)SC_COUNT + e->Rcap)));
@@ -941,13 +1025,37 @@ StreamParams stream_params(const sw_engine *e, int first, int n) {
 int stream_threads(int M) { return std::min(1024, std::max(32, (M + 31) / 32 * 32)); }
 size_t stream_smem(int M) { return (size_t)M * 8 + 32 * 8 + (size_t)3 * M * 4 + 32 * 4; }
 
+// the reference's own cadence (one sync per call): a call of at most STREAM_N events whose rows are current is divided
+// in ONE launch (swirld_stream.cuh)
+bool stream_path(const sw_engine *e, int first, int n) { return n <= sw_engine::STREAM_N && e->n_rowed == first; }
+
+// the last can_see rows were written on the compute stream: a scan on the copy stream waits for them
+int rows_written(sw_engine *e) {
+    CK(cudaEventRecord(e->scan_ev, e->stream));
+    e->scan_ev_set = true;
+    return 0;
+}
+
+// Before a chunk [first, first+n) on the compute stream: rows behind (small appends, or after sw_rewind) are scanned
+// there, for everything appended so far and after the copies of EVERY appended batch (the scan reads the columns of
+// all of them); else the stream waits for the copies of the batches the chunk touches.
+int rows_ready(sw_engine *e, int first, int n) {
+    if (first + n <= e->n_rowed) return wait_appends(e, first + n);
+    if (wait_appends(e, -1) < 0) return SW_E_CUDA;
+    const int rc = cansee_scan(e, e->stream, e->n_events);
+    return rc < 0 ? rc : rows_written(e);
+}
+
+void divided(sw_engine *e, int n) {
+    e->stats.events_divided += n;
+    e->n_divided += n;
+}
+
 // what a call on the streaming path leaves behind: its rows are complete (written on the compute stream)
 int stream_divided(sw_engine *e, int n) {
     e->n_rowed = e->n_divided + n;
-    CK(cudaEventRecord(e->scan_ev, e->stream));
-    e->scan_ev_set = true;
-    e->stats.events_divided += n;
-    e->n_divided += n;
+    if (rows_written(e) < 0) return SW_E_CUDA;
+    divided(e, n);
     return 0;
 }
 
@@ -978,9 +1086,6 @@ void sw_destroy(sw_engine *e) {
     if (e->d_views) cudaFree(e->d_views);
     if (e->d_rcviews) cudaFree(e->d_rcviews);
     if (e->d_stviews) cudaFree(e->d_stviews);
-    for (auto ev : e->bstage_ev) if (ev) cudaEventDestroy(ev);
-    if (e->h_bstage) cudaFreeHost(e->h_bstage);
-    if (e->d_bstage) cudaFree(e->d_bstage);
     if (e->d_vbuf) cudaFree(e->d_vbuf);
     if (e->h_vbuf) cudaFreeHost(e->h_vbuf);
     for (auto ev : e->stage_ev) if (ev) cudaEventDestroy(ev);
@@ -1062,11 +1167,9 @@ int sw_append(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const i
     cudaStream_t cs = e->copy_stream;
     if (n <= sw_engine::STAGE_EVENTS) {
         // a handful of events: pack the eight columns into one pinned block, one copy, one scatter kernel
-        const size_t slot = (unpack_bytes(sw_engine::STAGE_EVENTS) + 255) & ~(size_t)255;
-        const int si = e->stage_next;
-        e->stage_next = (si + 1) % sw_engine::STAGE_SLOTS;
-        CK(cudaEventSynchronize(e->stage_ev[si]));                       // (the copy that used this slot eight appends ago)
-        uint8_t *hs = e->h_stage + slot * si, *ds = e->d_stage + slot * si;
+        const int si = stage_slot(e, unpack_bytes(n));
+        if (si < 0) return si;
+        uint8_t *hs = e->h_stage + e->stage_bytes * si, *ds = e->d_stage + e->stage_bytes * si;
         const UnpackParams U = append_pack(e, n, p0, p1, creator, t, sig, hs, ds);
         CK(cudaMemcpyAsync(ds, hs, unpack_bytes(n), cudaMemcpyHostToDevice, cs));
         CK(cudaEventRecord(e->stage_ev[si], cs));
@@ -1113,21 +1216,9 @@ int sw_batch_append(sw_engine *const *engines, int B, const int *offsets, const 
     bytes += align256(sizeof(UnpackParams) * packed.size());
     // 2. the packed views: one slot of the first engine's ring, one copy, one scatter kernel
     cudaStream_t cs = e->copy_stream;
-    if (bytes > e->bstage_slot) {
-        CK(cudaStreamSynchronize(cs));                                   // (the copies and kernels that read the old ring)
-        if (e->h_bstage) { CK(cudaFreeHost(e->h_bstage)); e->h_bstage = nullptr; }
-        if (e->d_bstage) { CK(cudaFree(e->d_bstage)); e->d_bstage = nullptr; }
-        const size_t slot = align256(std::max(bytes, 2 * e->bstage_slot));
-        e->bstage_slot = 0;
-        CK(cudaMallocHost((void **)&e->h_bstage, slot * sw_engine::STAGE_SLOTS));
-        CK(cudaMalloc((void **)&e->d_bstage, slot * sw_engine::STAGE_SLOTS));
-        e->bstage_slot = slot;
-        for (auto &ev : e->bstage_ev) if (!ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    }
-    const int si = e->bstage_next;
-    e->bstage_next = (si + 1) % sw_engine::STAGE_SLOTS;
-    CK(cudaEventSynchronize(e->bstage_ev[si]));                          // (the copy that used this slot eight calls ago)
-    uint8_t *hs = e->h_bstage + e->bstage_slot * si, *ds = e->d_bstage + e->bstage_slot * si;
+    const int si = stage_slot(e, bytes);
+    if (si < 0) return si;
+    uint8_t *hs = e->h_stage + e->stage_bytes * si, *ds = e->d_stage + e->stage_bytes * si;
     UnpackParams *U = reinterpret_cast<UnpackParams *>(hs);
     size_t off = align256(sizeof(UnpackParams) * packed.size());
     for (size_t i = 0; i < packed.size(); i++) {
@@ -1137,7 +1228,7 @@ int sw_batch_append(sw_engine *const *engines, int B, const int *offsets, const 
         off += (unpack_bytes(n) + 15) & ~(size_t)15;
     }
     CK(cudaMemcpyAsync(ds, hs, off, cudaMemcpyHostToDevice, cs));
-    CK(cudaEventRecord(e->bstage_ev[si], cs));
+    CK(cudaEventRecord(e->stage_ev[si], cs));
     k_unpack_views<<<(int)packed.size(), 256, 0, cs>>>(reinterpret_cast<const UnpackParams *>(ds));
     CK(cudaGetLastError());
     e->stats.kernel_launches += 1;
@@ -1153,8 +1244,7 @@ int sw_divide_rounds(sw_engine *e, int first, int n) {
     if (first != e->n_divided) return fail(e, SW_E_ARG, "divide_rounds: first=%d but %d events are divided (events must arrive in order)", first, e->n_divided);
     if (first + n > e->n_events) return fail(e, SW_E_KEY, "divide_rounds: events [%d,%d) not appended", first, first + n);
     CK(cudaSetDevice(e->device));
-    if (n <= sw_engine::STREAM_N && e->n_rowed == first) {
-        // the reference's own cadence (one sync per call): the whole of divide_rounds in ONE launch (swirld_stream.cuh)
+    if (stream_path(e, first, n)) {
         if (wait_appends(e, first + n) < 0) return SW_E_CUDA;
         const StreamParams S = stream_params(e, first, n);
         const int threads = stream_threads(e->M);
@@ -1168,25 +1258,16 @@ int sw_divide_rounds(sw_engine *e, int first, int n) {
         e->stats.kernel_launches += 1;
         return stream_divided(e, n);         // (it wrote can_see rows and the carry heads on the compute stream)
     }
-    if (first + n > e->n_rowed) {
-        // rows are behind (small appends, or after sw_rewind): scan everything appended so far, here -- after the
-        // copies of EVERY appended batch (the scan reads the columns of all of them)
-        if (wait_appends(e, -1) < 0) return SW_E_CUDA;
-        int rc = cansee_scan(e, e->stream, e->n_events);
-        if (rc < 0) return rc;
-        CK(cudaEventRecord(e->scan_ev, e->stream));
-        e->scan_ev_set = true;
-    } else if (wait_appends(e, first + n) < 0) return SW_E_CUDA;
+    int rc = rows_ready(e, first, n);
+    if (rc < 0) return rc;
     {
         Span sp(e, 0);
-        int rc;
         if (e->wide) rc = SW_NJ(divide_rounds_wide, e, first, n);
         else rc = e->NC == 1 ? (e->unit ? divide_round_batch<1, true>(e, first, n, sp.s.a) : divide_round_batch<1, false>(e, first, n, sp.s.a))
                              : (e->unit ? divide_round_batch<2, true>(e, first, n, sp.s.a) : divide_round_batch<2, false>(e, first, n, sp.s.a));
         if (rc < 0) return rc;
     }
-    e->stats.events_divided += n;
-    e->n_divided += n;
+    divided(e, n);
     return SW_OK;
 }
 
@@ -1214,12 +1295,7 @@ static int chunk_views(sw_engine *e, sw_engine *const *engines, int B, const int
         const int nv = std::min(per_launch, B - v0), G = e->n_sm / nv;
         for (int v = v0; v < v0 + nv; v++) {
             sw_engine *x = engines[v];
-            if (first[v] + n[v] > x->n_rowed) {
-                if (wait_appends(x, -1) < 0) return SW_E_CUDA;
-                if (cansee_scan(x, x->stream, x->n_events) < 0) return SW_E_CUDA;
-                CK(cudaEventRecord(x->scan_ev, x->stream));
-                x->scan_ev_set = true;
-            } else if (wait_appends(x, first[v] + n[v]) < 0) return SW_E_CUDA;
+            if (rows_ready(x, first[v], n[v]) < 0) return SW_E_CUDA;
             // a view's window stays a round deep (16 pending events per chain) however few warps it has: they loop
             if (round_batch_prep(x, first[v], n[v], G, use_rc, Rv[v], 16) < 0) { e->err = x->err; return SW_E_CUDA; }
             if (use_rc) {
@@ -1262,8 +1338,7 @@ static int chunk_views(sw_engine *e, sw_engine *const *engines, int B, const int
             sw_engine *x = engines[v];
             int rc = x->NC == 1 ? round_batch_finish<1>(x, Rv[v]) : round_batch_finish<2>(x, Rv[v]);
             if (rc < 0) return rc;
-            x->stats.events_divided += n[v];
-            x->n_divided += n[v];
+            divided(x, n[v]);
         }
     }
     return SW_OK;
@@ -1283,7 +1358,7 @@ int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, c
         sw_engine *x = engines[v];
         if (n[v] <= 0 || first[v] != x->n_divided || first[v] + n[v] > x->n_events)
             return fail(e, SW_E_ARG, "sw_batch_divide_rounds: view %d: bad range [%d,%d)", v, first[v], first[v] + n[v]);
-        if (n[v] <= sw_engine::STREAM_N && x->n_rowed == first[v]) { sv.push_back(x); sn.push_back(n[v]); }
+        if (stream_path(x, first[v], n[v])) { sv.push_back(x); sn.push_back(n[v]); }
         else { cv.push_back(x); cfirst.push_back(first[v]); cn.push_back(n[v]); }
     }
     for (sw_engine *x : cv)
@@ -1330,39 +1405,19 @@ int sw_decide_fame(sw_engine *e, int32_t *new_c_out, int cap) {
     if (!e || cap < 0 || (cap > 0 && !new_c_out)) return fail(e, SW_E_ARG, "bad argument");
     CK(cudaSetDevice(e->device));
     if (e->n_divided == 0) return fail(e, SW_E_ARG, "decide_fame: no witnesses yet (max() of an empty dict, swirld.py:225)");
-    const FameParams P = fame_params(e);
     {
         Span sp(e, 1);
-        if (e->wide) {
-            k_fame_begin<<<1, 32, 0, e->stream>>>(P);
-            SW_NJ(fame_rounds_wide, e, P);
-            k_fame_finish<<<1, 1024, 0, e->stream>>>(P);
-            e->stats.kernel_launches += 3;
-        } else {
-            k_fame_rounds<<<2 * e->n_sm, 256, 0, e->stream>>>(P);
-            e->stats.kernel_launches += 1;
-        }
+        fame_kernels(e, fame_params(e), 1);
         CK(cudaGetLastError());
     }
-    // one copy, one synchronisation: the scalars and (speculatively) the first new consensus rounds together
-    // (a 64-member chunk of 64 K events brings about 90 new rounds: room for 64 only would add a copy and a
-    // synchronisation to every such call)
-    const int spec = std::min(e->Rcap, 1024);
+    const int spec = fame_spec(e);
     CK(cudaMemcpyAsync(e->h_scal, e->d_scal, sizeof(int32_t) * (SC_COUNT + spec), cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     if (e->spans.size() >= 256) fold_spans(e);         // (the timings are read in sw_sync / sw_stats; not on every call)
     e->stats.d2h_bytes += sizeof(int32_t) * (SC_COUNT + spec);
-    int rc = device_error(e);
-    if (rc < 0) return rc;
-    const int cnt = e->h_scal[SC_NEWC];
-    if (cnt > cap) return fail(e, SW_E_ARG, "decide_fame: %d new consensus rounds do not fit cap=%d", cnt, cap);
-    if (cnt > spec) {
-        CK(cudaMemcpyAsync(e->h_newc, e->d_newc, sizeof(int32_t) * cnt, cudaMemcpyDeviceToHost, e->stream));
-        CK(cudaStreamSynchronize(e->stream));
-        e->stats.d2h_bytes += sizeof(int32_t) * cnt;
-    }
-    if (cnt > 0) memcpy(new_c_out, e->h_newc, sizeof(int32_t) * cnt);
-    return cnt;
+    int r;
+    const int rc = fame_result(e, new_c_out, cap, r);
+    return rc < 0 ? rc : r;
 }
 
 int sw_find_order(sw_engine *e, const int32_t *new_c, int n) {
@@ -1370,45 +1425,22 @@ int sw_find_order(sw_engine *e, const int32_t *new_c, int n) {
     if (n == 0) return 0;
     CK(cudaSetDevice(e->device));
     std::vector<int32_t> rs(new_c, new_c + n);
-    std::sort(rs.begin(), rs.end());                                  // sorted(new_c), swirld.py:283
-    for (int r : rs) if (r < 0 || r >= e->Rcap) return fail(e, SW_E_KEY, "find_order: unknown round %d", r);
+    int bad;
+    if (!sort_rounds(e, rs.data(), n, bad)) return fail(e, SW_E_KEY, "find_order: unknown round %d", bad);
     if (order_scratch(e, n) < 0) return SW_E_CUDA;
     CK(cudaMemcpyAsync(e->d_rounds_in, rs.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, e->stream));
-    const OrderParams P = order_params(e, n, e->d_rounds_in);
-    const int M = e->M;
     cudaEvent_t a = get_event(e), b = get_event(e);
     cudaEventRecord(a, e->stream);
-    if (e->wide) {
-        k_w_order_rounds<<<n, 1024, (size_t)3 * M * sizeof(int), e->stream>>>(P);
-        k_w_order_cuts<<<1, 1024, (size_t)2 * M * sizeof(int), e->stream>>>(P);
-        k_w_order_list<<<std::max(1, std::min(4 * e->n_sm, (int)(((size_t)n * M + 255) / 256))), 256, 0, e->stream>>>(P);
-    } else {
-        k_order_rounds<<<n, 1024, 0, e->stream>>>(P);
-        k_order_cuts<<<1, 64, 0, e->stream>>>(P);
-        k_order_list<<<std::max(1, std::min(4 * e->n_sm, (n * 64 + 255) / 256)), 256, 0, e->stream>>>(P);
-    }
-    CK(cudaGetLastError());
-    // the number of newly ordered events stays on the device: the time / sort kernels read it there, the host learns it
-    // from the one copy at the end of the call
-    if (e->wide) {
-        const size_t tsm = (size_t)OW_WARPS * M * sizeof(u64);
-        k_w_order_times<<<8 * e->n_sm, OW_WARPS * 32, tsm, e->stream>>>(P);
-    } else k_order_times<<<4 * e->n_sm, 256, 0, e->stream>>>(P);
-    k_order_sort<<<n, 1024, 0, e->stream>>>(P);
+    order_kernels(e, order_params(e, n, e->d_rounds_in), 1, n);
     CK(cudaGetLastError());
     cudaEventRecord(b, e->stream);
     e->spans.push_back(TimedSpan{a, b, 2});
     CK(cudaMemcpyAsync(e->h_scal, e->d_scal, sizeof(int32_t) * SC_COUNT, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));      // (rs, the host vector of the rounds, was consumed by the copy above)
     fold_spans(e);
-    e->stats.kernel_launches += 5;
     e->stats.h2d_bytes += sizeof(int32_t) * n;
     e->stats.d2h_bytes += sizeof(int32_t) * SC_COUNT;
-    int rc = device_error(e);
-    if (rc < 0) return rc;
-    const int nbatch = e->h_scal[SC_BATCH];
-    e->n_tx += nbatch;
-    return nbatch;
+    return order_result(e);
 }
 
 // Node.decide_fame for B node-views in one call: the fame kernels of every view side by side in one grid (blockIdx.y =
@@ -1422,7 +1454,7 @@ int sw_batch_decide_fame(sw_engine *const *engines, int B, int32_t *new_c_out, i
         if (engines[v]->n_divided == 0)
             return fail(e, SW_E_ARG, "sw_batch_decide_fame: view %d: no witnesses yet (max() of an empty dict, swirld.py:225)", v);
     CK(cudaSetDevice(e->device));
-    const int S = SC_COUNT + 1024;                     // per view: the scalars and the new rounds sw_decide_fame copies
+    const int S = SC_COUNT + FAME_SPEC;                // per view: the scalars and the new rounds sw_decide_fame copies
     const size_t pbytes = align256(sizeof(FameParams) * B), sbytes = sizeof(int32_t) * (size_t)S * B;
     if (views_buffer(e, pbytes + sbytes) < 0) return SW_E_CUDA;
     FameParams *hP = reinterpret_cast<FameParams *>(e->h_vbuf);
@@ -1433,43 +1465,20 @@ int sw_batch_decide_fame(sw_engine *const *engines, int B, int32_t *new_c_out, i
     CK(cudaMemcpyAsync(e->d_vbuf, e->h_vbuf, sizeof(FameParams) * B, cudaMemcpyHostToDevice, e->stream));
     e->stats.h2d_bytes += sizeof(FameParams) * B;
     {
-        // every view gets the CTAs its single call launches (the kernels are latency-bound; spare CTAs exit at once)
         Span sp(e, 1);
-        if (e->wide) {
-            const int parts = (e->M + FW_THREADS - 1) / FW_THREADS;
-            k_fame_begin_views<<<dim3(1, B), 32, 0, e->stream>>>(Pv);
-            SW_NJ(fame_rounds_wide_views, e, Pv, B, 2 * e->n_sm / parts + 1);
-            k_fame_finish_views<<<dim3(1, B), 1024, 0, e->stream>>>(Pv);
-        } else {
-            k_fame_rounds_views<<<dim3(2 * e->n_sm, B), 256, 0, e->stream>>>(Pv);
-        }
+        fame_kernels(e, Pv, B);
         k_views_gather<<<B, 256, 0, e->stream>>>(Pv, d_st, S);
         CK(cudaGetLastError());
-        e->stats.kernel_launches += e->wide ? 4 : 2;
+        e->stats.kernel_launches += 1;
     }
     if (views_leave(e, engines, B, h_st, d_st, sbytes) < 0) return SW_E_CUDA;
     if (e->spans.size() >= 256) fold_spans(e);
-    // per view what sw_decide_fame does after its copy: the host mirror of the scalars, the error the device found, and a
-    // second copy when more new rounds came than the first one held
     int first_err = SW_OK;
     for (int v = 0; v < B; v++) {
         sw_engine *x = engines[v];
-        const int spec = std::min(x->Rcap, 1024);
-        memcpy(x->h_scal, h_st + (size_t)S * v, sizeof(int32_t) * (SC_COUNT + spec));
-        int r = device_error(x);
-        if (r == 0) {
-            const int cnt = x->h_scal[SC_NEWC];
-            if (cnt > cap) r = fail(x, SW_E_ARG, "decide_fame: %d new consensus rounds do not fit cap=%d", cnt, cap);
-            else {
-                if (cnt > spec) {
-                    CK(cudaMemcpyAsync(x->h_newc, x->d_newc, sizeof(int32_t) * cnt, cudaMemcpyDeviceToHost, x->stream));
-                    CK(cudaStreamSynchronize(x->stream));
-                    x->stats.d2h_bytes += sizeof(int32_t) * cnt;
-                }
-                if (cnt > 0) memcpy(new_c_out + (size_t)cap * v, x->h_newc, sizeof(int32_t) * cnt);
-                r = cnt;
-            }
-        }
+        memcpy(x->h_scal, h_st + (size_t)S * v, sizeof(int32_t) * (SC_COUNT + fame_spec(x)));
+        int r;
+        if (fame_result(x, new_c_out + (size_t)cap * v, cap, r) < 0) { e->err = x->err; return SW_E_CUDA; }
         count_out[v] = r;
         if (r < 0 && first_err == SW_OK) first_err = r;
     }
@@ -1496,10 +1505,9 @@ int sw_batch_find_order(sw_engine *const *engines, int B, const int32_t *new_c, 
     int maxn = 0;
     for (int v = 0; v < B; v++) {
         const int n = offsets[v + 1] - offsets[v];
-        auto b = rs.begin() + (offsets[v] - offsets[0]);
-        std::sort(b, b + n);                                           // sorted(new_c), swirld.py:283
-        for (auto it = b; it != b + n; ++it)
-            if (*it < 0 || *it >= engines[v]->Rcap) return fail(e, SW_E_KEY, "sw_batch_find_order: view %d: unknown round %d", v, *it);
+        int bad;
+        if (!sort_rounds(engines[v], rs.data() + (offsets[v] - offsets[0]), n, bad))
+            return fail(e, SW_E_KEY, "sw_batch_find_order: view %d: unknown round %d", v, bad);
         if (n > 0) { act.push_back(engines[v]); act_v.push_back(v); maxn = std::max(maxn, n); }
     }
     for (int v = 0; v < B; v++) count_out[v] = 0;
@@ -1524,36 +1532,21 @@ int sw_batch_find_order(sw_engine *const *engines, int B, const int32_t *new_c, 
     if (views_enter(e, act.data(), A) < 0) return SW_E_CUDA;
     CK(cudaMemcpyAsync(e->d_vbuf, e->h_vbuf, inbytes, cudaMemcpyHostToDevice, e->stream));
     e->stats.h2d_bytes += inbytes;
-    const int M = e->M, MS = e->MS;
-    // every view gets the CTAs its single call launches, sized from the view with the most rounds
-    const int list_ctas = std::max(1, std::min(4 * e->n_sm, (int)(((size_t)maxn * MS + 255) / 256)));
     cudaEvent_t a = get_event(e), b = get_event(e);
     cudaEventRecord(a, e->stream);
-    if (e->wide) {
-        k_w_order_rounds_views<<<dim3(maxn, A), 1024, (size_t)3 * M * sizeof(int), e->stream>>>(Pv);
-        k_w_order_cuts_views<<<dim3(1, A), 1024, (size_t)2 * M * sizeof(int), e->stream>>>(Pv);
-        k_w_order_list_views<<<dim3(list_ctas, A), 256, 0, e->stream>>>(Pv);
-        k_w_order_times_views<<<dim3(8 * e->n_sm, A), OW_WARPS * 32, (size_t)OW_WARPS * M * sizeof(u64), e->stream>>>(Pv);
-    } else {
-        k_order_rounds_views<<<dim3(maxn, A), 1024, 0, e->stream>>>(Pv);
-        k_order_cuts_views<<<dim3(1, A), 64, 0, e->stream>>>(Pv);
-        k_order_list_views<<<dim3(list_ctas, A), 256, 0, e->stream>>>(Pv);
-        k_order_times_views<<<dim3(4 * e->n_sm, A), 256, 0, e->stream>>>(Pv);
-    }
-    k_order_sort_views<<<dim3(maxn, A), 1024, 0, e->stream>>>(Pv);
+    order_kernels(e, Pv, A, maxn);
     k_views_gather<<<A, 32, 0, e->stream>>>(Pv, d_st, SC_COUNT);
     CK(cudaGetLastError());
     cudaEventRecord(b, e->stream);
     e->spans.push_back(TimedSpan{a, b, 2});
-    e->stats.kernel_launches += 6;
+    e->stats.kernel_launches += 1;
     if (views_leave(e, act.data(), A, h_st, d_st, sbytes) < 0) return SW_E_CUDA;
     fold_spans(e);
     int first_err = SW_OK;
     for (int i = 0; i < A; i++) {
         sw_engine *x = act[i];
         memcpy(x->h_scal, h_st + (size_t)SC_COUNT * i, sizeof(int32_t) * SC_COUNT);
-        int r = device_error(x);
-        if (r == 0) { r = x->h_scal[SC_BATCH]; x->n_tx += r; }
+        const int r = order_result(x);
         count_out[act_v[i]] = r;
         if (r < 0 && first_err == SW_OK) first_err = r;
     }
@@ -1792,6 +1785,25 @@ bool get_dev(sw_engine *e, FILE *f, void *d, size_t bytes, std::vector<char> &tm
     }
     return true;
 }
+
+// The file: the header, the stake (sw_load needs it to create the engine), then these sections in this order, each
+// sized from the header's counts.  `idrec`: the id records, 36 bytes each (32-byte id, arrival index).
+struct Section { void *p; size_t bytes; bool dev; };
+std::vector<Section> ckpt_sections(sw_engine *e, const CkptHeader &H, std::vector<uint8_t> &idrec) {
+    const size_t M = H.M, n = H.n_events, nd = H.n_divided, nr = H.n_rowed, NJ = H.NJ, R = H.rounds, RM = R * M;
+    const size_t i4 = sizeof(int32_t);
+    const Section SM = H.wide ? Section{e->d_SMw, sizeof(unsigned) * nd * NJ, true} : Section{e->d_SM, sizeof(u64) * nd, true};
+    const Section S = H.wide ? Section{e->d_Sw, sizeof(unsigned) * RM * NJ, true} : Section{e->d_S, sizeof(u64) * RM, true};
+    return {
+        {e->h_creator.data(), i4 * n, false}, {e->h_head.data(), i4 * M, false}, {e->h_count.data(), i4 * M, false},
+        {e->h_height, i4 * n, false}, {e->h_seq, i4 * n, false}, {e->h_stale, n, false},
+        {e->d_p0, i4 * n, true}, {e->d_p1, i4 * n, true}, {e->d_creator, i4 * n, true}, {e->d_t, sizeof(double) * n, true},
+        {e->d_sig, 64 * n, true}, {e->d_row, i4 * nr * M, true}, {e->d_round, i4 * nd, true}, {e->d_wit, nd, true},
+        SM, {e->d_famous_ev, n, true}, {e->d_idx, i4 * n, true}, {e->d_tx, i4 * (size_t)H.n_tx, true},
+        {e->d_W, i4 * RM, true}, {e->d_Wf, i4 * RM, true}, {e->d_famous, RM, true}, {e->d_coin, RM, true},
+        S, {e->d_consensus, R, true}, {e->d_lastord, i4 * M, true}, {e->d_cs_carry, i4 * M, true}, {e->d_rbtot, i4 * M, true},
+        {e->d_gchain, i4 * M * RB_RING, true}, {e->d_scal, i4 * SC_COUNT, true}, {idrec.data(), idrec.size(), false}};
+}
 }  // namespace
 
 int sw_save(sw_engine *e, const char *path) {
@@ -1811,26 +1823,9 @@ int sw_save(sw_engine *e, const char *path) {
     std::vector<uint8_t> idrec((size_t)36 * e->ids.size());
     { size_t o = 0; for (auto &kv : e->ids) { memcpy(&idrec[o], kv.first.data(), 32); memcpy(&idrec[o + 32], &kv.second, 4); o += 36; } }
     std::vector<char> tmp;
-    const size_t RM = (size_t)R * M;
-    bool ok = fwrite(&H, sizeof H, 1, f) == 1 && put_host(f, e->h_stake.data(), sizeof(i64) * M)
-        && put_host(f, e->h_creator.data(), sizeof(int32_t) * n) && put_host(f, e->h_head.data(), sizeof(int32_t) * M)
-        && put_host(f, e->h_count.data(), sizeof(int32_t) * M) && put_host(f, e->h_height, sizeof(int32_t) * n)
-        && put_host(f, e->h_seq, sizeof(int32_t) * n) && put_host(f, e->h_stale, (size_t)n)
-        && put_dev(e, f, e->d_p0, sizeof(int32_t) * n, tmp) && put_dev(e, f, e->d_p1, sizeof(int32_t) * n, tmp)
-        && put_dev(e, f, e->d_creator, sizeof(int32_t) * n, tmp) && put_dev(e, f, e->d_t, sizeof(double) * n, tmp)
-        && put_dev(e, f, e->d_sig, (size_t)64 * n, tmp)
-        && put_dev(e, f, e->d_row, sizeof(int32_t) * (size_t)nr * M, tmp)
-        && put_dev(e, f, e->d_round, sizeof(int32_t) * nd, tmp) && put_dev(e, f, e->d_wit, (size_t)nd, tmp)
-        && (e->wide ? put_dev(e, f, e->d_SMw, sizeof(unsigned) * (size_t)nd * e->NJ, tmp) : put_dev(e, f, e->d_SM, sizeof(u64) * nd, tmp))
-        && put_dev(e, f, e->d_famous_ev, (size_t)n, tmp) && put_dev(e, f, e->d_idx, sizeof(int32_t) * n, tmp)
-        && put_dev(e, f, e->d_tx, sizeof(int32_t) * e->n_tx, tmp)
-        && put_dev(e, f, e->d_W, sizeof(int32_t) * RM, tmp) && put_dev(e, f, e->d_Wf, sizeof(int32_t) * RM, tmp)
-        && put_dev(e, f, e->d_famous, RM, tmp) && put_dev(e, f, e->d_coin, RM, tmp)
-        && (e->wide ? put_dev(e, f, e->d_Sw, sizeof(unsigned) * RM * e->NJ, tmp) : put_dev(e, f, e->d_S, sizeof(u64) * RM, tmp))
-        && put_dev(e, f, e->d_consensus, (size_t)R, tmp)
-        && put_dev(e, f, e->d_lastord, sizeof(int32_t) * M, tmp) && put_dev(e, f, e->d_cs_carry, sizeof(int32_t) * M, tmp)
-        && put_dev(e, f, e->d_rbtot, sizeof(int32_t) * M, tmp) && put_dev(e, f, e->d_gchain, sizeof(int32_t) * (size_t)M * RB_RING, tmp)
-        && put_dev(e, f, e->d_scal, sizeof(int32_t) * SC_COUNT, tmp) && put_host(f, idrec.data(), idrec.size());
+    bool ok = fwrite(&H, sizeof H, 1, f) == 1 && put_host(f, e->h_stake.data(), sizeof(i64) * M);
+    for (const Section &s : ckpt_sections(e, H, idrec))
+        ok = ok && (s.dev ? put_dev(e, f, s.p, s.bytes, tmp) : put_host(f, s.p, s.bytes));
     ok = (fclose(f) == 0) && ok;
     if (!ok) return fail(e, SW_E_ARG, "sw_save: write to %s failed", path);
     return SW_OK;
@@ -1857,31 +1852,12 @@ int sw_load(const char *path, int device, int capacity_events, sw_engine **out) 
     const int M = H.M, n = H.n_events, nd = H.n_divided, nr = H.n_rowed, R = H.rounds;
     if (R > e->Rcap || (int)e->wide != H.wide || e->NJ != H.NJ) { fclose(f); sw_destroy(e); return fail(nullptr, SW_E_ARG, "sw_load: checkpoint does not fit the engine"); }
     std::vector<char> tmp;
-    const size_t RM = (size_t)R * M;
+    std::vector<uint8_t> idrec((size_t)36 * H.n_ids);
     e->h_creator.resize(n);
-    bool ok = get_host(f, e->h_creator.data(), sizeof(int32_t) * n) && get_host(f, e->h_head.data(), sizeof(int32_t) * M)
-        && get_host(f, e->h_count.data(), sizeof(int32_t) * M) && get_host(f, e->h_height, sizeof(int32_t) * n)
-        && get_host(f, e->h_seq, sizeof(int32_t) * n) && get_host(f, e->h_stale, (size_t)n)
-        && get_dev(e, f, e->d_p0, sizeof(int32_t) * n, tmp) && get_dev(e, f, e->d_p1, sizeof(int32_t) * n, tmp)
-        && get_dev(e, f, e->d_creator, sizeof(int32_t) * n, tmp) && get_dev(e, f, e->d_t, sizeof(double) * n, tmp)
-        && get_dev(e, f, e->d_sig, (size_t)64 * n, tmp)
-        && get_dev(e, f, e->d_row, sizeof(int32_t) * (size_t)nr * M, tmp)
-        && get_dev(e, f, e->d_round, sizeof(int32_t) * nd, tmp) && get_dev(e, f, e->d_wit, (size_t)nd, tmp)
-        && (e->wide ? get_dev(e, f, e->d_SMw, sizeof(unsigned) * (size_t)nd * e->NJ, tmp) : get_dev(e, f, e->d_SM, sizeof(u64) * nd, tmp))
-        && get_dev(e, f, e->d_famous_ev, (size_t)n, tmp) && get_dev(e, f, e->d_idx, sizeof(int32_t) * n, tmp)
-        && get_dev(e, f, e->d_tx, sizeof(int32_t) * H.n_tx, tmp)
-        && get_dev(e, f, e->d_W, sizeof(int32_t) * RM, tmp) && get_dev(e, f, e->d_Wf, sizeof(int32_t) * RM, tmp)
-        && get_dev(e, f, e->d_famous, RM, tmp) && get_dev(e, f, e->d_coin, RM, tmp)
-        && (e->wide ? get_dev(e, f, e->d_Sw, sizeof(unsigned) * RM * e->NJ, tmp) : get_dev(e, f, e->d_S, sizeof(u64) * RM, tmp))
-        && get_dev(e, f, e->d_consensus, (size_t)R, tmp)
-        && get_dev(e, f, e->d_lastord, sizeof(int32_t) * M, tmp) && get_dev(e, f, e->d_cs_carry, sizeof(int32_t) * M, tmp)
-        && get_dev(e, f, e->d_rbtot, sizeof(int32_t) * M, tmp) && get_dev(e, f, e->d_gchain, sizeof(int32_t) * (size_t)M * RB_RING, tmp)
-        && get_dev(e, f, e->d_scal, sizeof(int32_t) * SC_COUNT, tmp);
-    if (ok) {
-        std::vector<uint8_t> idrec((size_t)36 * H.n_ids);
-        ok = get_host(f, idrec.data(), idrec.size());
-        for (size_t o = 0; ok && o < idrec.size(); o += 36) { Id32 k; int32_t v; memcpy(k.data(), &idrec[o], 32); memcpy(&v, &idrec[o + 32], 4); e->ids.emplace(k, v); }
-    }
+    bool ok = true;
+    for (const Section &s : ckpt_sections(e, H, idrec))
+        ok = ok && (s.dev ? get_dev(e, f, s.p, s.bytes, tmp) : get_host(f, s.p, s.bytes));
+    for (size_t o = 0; ok && o < idrec.size(); o += 36) { Id32 k; int32_t v; memcpy(k.data(), &idrec[o], 32); memcpy(&v, &idrec[o + 32], 4); e->ids.emplace(k, v); }
     fclose(f);
     if (!ok) { sw_destroy(e); return fail(nullptr, SW_E_ARG, "sw_load: %s is truncated or does not match its header", path); }
     // the derived columns live on the device too

@@ -18,6 +18,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 
 typedef unsigned long long u64;
 typedef long long i64;
@@ -199,6 +200,23 @@ __device__ __forceinline__ void fame_collect(const FameParams &P, int max_c, int
     if (tid == 0) { P.scal[SC_NEWC] = s_base; P.scal[SC_MAXC] = max_c; }
 }
 
+// The fame and order kernels take their parameters from a Src: a value (one node-view per launch) or the device array
+// of the views of sw_batch_decide_fame / sw_batch_find_order.  Then blockIdx.y is the view, Pv[blockIdx.y] its
+// parameters, staged in shared memory; blockIdx.x and gridDim.x are what they are in a single-view launch, so the
+// grid-stride loops and k_fame_rounds' last-CTA ticket count one view's CTAs.  The order grids are sized from the view
+// with the most rounds: a CTA beyond its view's rounds exits.
+template <typename T>
+__device__ __forceinline__ const T &view_params(const T *Pv) {
+    __shared__ T Ps;
+    if (threadIdx.x == 0) Ps = Pv[blockIdx.y];
+    __syncthreads();
+    return Ps;
+}
+template <typename T>
+__device__ __forceinline__ const T &params(const T &P) { return P; }
+template <typename T>
+__device__ __forceinline__ const T &params(const T *Pv) { return view_params(Pv); }
+
 __device__ __forceinline__ void fame_begin_body(const FameParams &P) {     // one warp
     const int lane = threadIdx.x;
     const int mc = fame_max_c(P, lane);
@@ -207,10 +225,10 @@ __device__ __forceinline__ void fame_begin_body(const FameParams &P) {     // on
     const int max_r = P.scal[SC_MAX_ROUND];
     for (int r = mc + lane; r <= max_r && r < P.Rcap; r += 32) { P.rem[r] = 0; P.done[r] = 0; }
 }
-__global__ void k_fame_begin(FameParams P) { fame_begin_body(P); }
+template <class Src> __global__ void k_fame_begin(Src s) { fame_begin_body(params(s)); }
 
-// M <= 64: each candidate round is one CTA's, which writes its rem / done whole.  (A template so that each kernel gets
-// its own copy of the body's shared variables: k_fame_rounds then compiles as it did without the views kernel.)
+// M <= 64: each candidate round is one CTA's, which writes its rem / done whole.  (A template over VIEWS so that each
+// instance of k_fame_rounds gets its own copy of the body's shared variables and keeps its registers.)
 template <bool VIEWS>
 __device__ __forceinline__ void fame_rounds_body(const FameParams &P) {
     __shared__ u64 sv[2][64];
@@ -306,10 +324,13 @@ __device__ __forceinline__ void fame_rounds_body(const FameParams &P) {
     if (tid == 0) P.scal[SC_TICKET] = 0;
     fame_collect(P, max_c, max_r);
 }
-__global__ void __launch_bounds__(256) k_fame_rounds(FameParams P) { fame_rounds_body<false>(P); }
+template <class Src> __global__ void __launch_bounds__(256) k_fame_rounds(Src s) { fame_rounds_body<std::is_pointer<Src>::value>(params(s)); }
 
-__device__ __forceinline__ void fame_finish_body(const FameParams &P) { fame_collect(P, P.scal[SC_MAXC], P.scal[SC_MAX_ROUND]); }
-__global__ void __launch_bounds__(1024, 1) k_fame_finish(FameParams P) { fame_finish_body(P); }
+template <class Src>
+__global__ void __launch_bounds__(1024, 1) k_fame_finish(Src s) {
+    const FameParams &P = params(s);
+    fame_collect(P, P.scal[SC_MAXC], P.scal[SC_MAX_ROUND]);
+}
 
 // ---------------------------------------------------------------- K4: find_order
 struct OrderParams {
@@ -424,7 +445,12 @@ __device__ __forceinline__ void order_rounds_body(const OrderParams &P) {
         PLAN(3)[si * 64 + tid] = ua >= 0 ? P.seq[ua] : -1;
     }
 }
-__global__ void __launch_bounds__(1024, 1) k_order_rounds(OrderParams P) { order_rounds_body(P); }
+template <class Src>
+__global__ void __launch_bounds__(1024, 1) k_order_rounds(Src s) {
+    const OrderParams &P = params(s);
+    if constexpr (std::is_pointer<Src>::value) if ((int)blockIdx.x >= P.nrounds) return;
+    order_rounds_body(P);
+}
 
 // B: the only sequential part -- round after round, what each chain still has to give: the events
 // (lastord[c], min(reach, thr)].  A famous witness that an earlier round already ordered does not seed
@@ -479,7 +505,7 @@ __device__ __forceinline__ void order_cuts_body(const OrderParams &P) {
     if (c < M) P.lastord[c] = lo;
     if (c == 0) { P.seg_start[P.nrounds] = total; P.scal[SC_BATCH] = total; }
 }
-__global__ void __launch_bounds__(64) k_order_cuts(OrderParams P) { order_cuts_body(P); }
+template <class Src> __global__ void __launch_bounds__(64) k_order_cuts(Src s) { order_cuts_body(params(s)); }
 
 // C: list the ordered events of every (round, chain): from the cut down the self-parent chain
 __device__ __forceinline__ void order_list_body(const OrderParams &P) {
@@ -495,7 +521,7 @@ __device__ __forceinline__ void order_list_body(const OrderParams &P) {
         }
     }
 }
-__global__ void k_order_list(OrderParams P) { order_list_body(P); }
+template <class Src> __global__ void k_order_list(Src s) { order_list_body(params(s)); }
 
 // Consensus timestamp and sort key of each newly ordered event (swirld.py:295-306):
 // one warp per event, lane = famous witness.  For a witness that sees x the reference
@@ -562,7 +588,7 @@ __device__ __forceinline__ void order_times_body(const OrderParams &P) {
     }
     }
 }
-__global__ void __launch_bounds__(256) k_order_times(OrderParams P) { order_times_body(P); }
+template <class Src> __global__ void __launch_bounds__(256) k_order_times(Src s) { order_times_body(params(s)); }
 
 __device__ __forceinline__ bool order_less(const OrderParams &P, int a, int b) {
     // a, b are batch slots (-1 = padding = +infinity); (ts, white ^ sig) ascending
@@ -610,36 +636,18 @@ __device__ __forceinline__ void order_sort_body(const OrderParams &P) {
         P.idx[x] = P.tx_base + s0 + i;
     }
 }
-__global__ void __launch_bounds__(1024) k_order_sort(OrderParams P) { order_sort_body(P); }
-
-// ---------------------------------------------------------------- several node-views per launch
-// sw_batch_decide_fame / sw_batch_find_order run the bodies above for B independent node-views at once (the pattern of
-// k_rounds_batch_views): blockIdx.y is the view, Pv[blockIdx.y] its parameters, staged in shared memory; blockIdx.x and
-// gridDim.x are what they are in a single-view launch, so the grid-stride loops and k_fame_rounds' last-CTA ticket count
-// one view's CTAs.  The order grids are sized from the view with the most rounds: a CTA beyond its view's rounds exits.
-template <typename T>
-__device__ __forceinline__ const T &view_params(const T *Pv) {
-    __shared__ T Ps;
-    if (threadIdx.x == 0) Ps = Pv[blockIdx.y];
-    __syncthreads();
-    return Ps;
+template <class Src>
+__global__ void __launch_bounds__(1024) k_order_sort(Src s) {
+    const OrderParams &P = params(s);
+    if constexpr (std::is_pointer<Src>::value) if ((int)blockIdx.x >= P.nrounds) return;
+    order_sort_body(P);
 }
 
-__global__ void k_fame_begin_views(const FameParams *Pv) { fame_begin_body(view_params(Pv)); }
-__global__ void __launch_bounds__(256) k_fame_rounds_views(const FameParams *Pv) { fame_rounds_body<true>(view_params(Pv)); }
-__global__ void __launch_bounds__(1024, 1) k_fame_finish_views(const FameParams *Pv) { fame_finish_body(view_params(Pv)); }
-
-__global__ void __launch_bounds__(1024, 1) k_order_rounds_views(const OrderParams *Pv) {
-    const OrderParams &P = view_params(Pv);
-    if ((int)blockIdx.x < P.nrounds) order_rounds_body(P);
-}
-__global__ void __launch_bounds__(64) k_order_cuts_views(const OrderParams *Pv) { order_cuts_body(view_params(Pv)); }
-__global__ void k_order_list_views(const OrderParams *Pv) { order_list_body(view_params(Pv)); }
-__global__ void __launch_bounds__(256) k_order_times_views(const OrderParams *Pv) { order_times_body(view_params(Pv)); }
-__global__ void __launch_bounds__(1024) k_order_sort_views(const OrderParams *Pv) {
-    const OrderParams &P = view_params(Pv);
-    if ((int)blockIdx.x < P.nrounds) order_sort_body(P);
-}
+// what the host launches: each kernel for one view by value and for the device array of several views
+#define SW_SRC_INSTANCES(K, T) template __global__ void K<T>(T); template __global__ void K<const T *>(const T *);
+SW_SRC_INSTANCES(k_fame_begin, FameParams) SW_SRC_INSTANCES(k_fame_rounds, FameParams) SW_SRC_INSTANCES(k_fame_finish, FameParams)
+SW_SRC_INSTANCES(k_order_rounds, OrderParams) SW_SRC_INSTANCES(k_order_cuts, OrderParams) SW_SRC_INSTANCES(k_order_list, OrderParams)
+SW_SRC_INSTANCES(k_order_times, OrderParams) SW_SRC_INSTANCES(k_order_sort, OrderParams)
 
 // the first n ints of every view's scalar block (SC_*, and for decide_fame the new rounds behind them) into row v of
 // one staging array: one device-to-host copy brings back what B single calls copy one by one

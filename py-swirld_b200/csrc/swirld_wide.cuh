@@ -686,8 +686,8 @@ __device__ __forceinline__ void w_fame_rounds_body(const FameParams &P) {
         if (tid == 0) { if (left) atomicAdd(&P.rem[r], left); if (dn) P.done[r] = 1; }
     }
 }
-template <int NJ>
-__global__ void __launch_bounds__(FW_THREADS) k_w_fame_rounds(FameParams P) { w_fame_rounds_body<NJ>(P); }
+template <int NJ, class Src>
+__global__ void __launch_bounds__(FW_THREADS) k_w_fame_rounds(Src s) { w_fame_rounds_body<NJ>(params(s)); }
 
 // ------------------------------------------------------------------ find_order (swirld.py:280-311)
 // Same plan as swirld_kernels.cuh (A per round, B sequential cuts, C listing, times, sort) with per-round
@@ -759,7 +759,12 @@ __device__ __forceinline__ void w_order_rounds_body(const OrderParams &P) {
         WPLAN(3)[(size_t)si * M + c] = U >= 0 ? P.seq[U] : -1;
     }
 }
-__global__ void __launch_bounds__(1024, 1) k_w_order_rounds(OrderParams P) { w_order_rounds_body(P); }
+template <class Src>
+__global__ void __launch_bounds__(1024, 1) k_w_order_rounds(Src s) {
+    const OrderParams &P = params(s);
+    if constexpr (std::is_pointer<Src>::value) if ((int)blockIdx.x >= P.nrounds) return;
+    w_order_rounds_body(P);
+}
 
 __device__ __forceinline__ void w_order_cuts_body(const OrderParams &P) {
     extern __shared__ int oc_smem[];
@@ -809,7 +814,7 @@ __device__ __forceinline__ void w_order_cuts_body(const OrderParams &P) {
     if (c < M) P.lastord[c] = lo;
     if (c == 0) { P.seg_start[P.nrounds] = total; P.scal[SC_BATCH] = total; }
 }
-__global__ void __launch_bounds__(1024) k_w_order_cuts(OrderParams P) { w_order_cuts_body(P); }
+template <class Src> __global__ void __launch_bounds__(1024) k_w_order_cuts(Src s) { w_order_cuts_body(params(s)); }
 
 __device__ __forceinline__ void w_order_list_body(const OrderParams &P) {
     const size_t tot = (size_t)P.nrounds * P.M;
@@ -825,7 +830,7 @@ __device__ __forceinline__ void w_order_list_body(const OrderParams &P) {
         }
     }
 }
-__global__ void k_w_order_list(OrderParams P) { w_order_list_body(P); }
+template <class Src> __global__ void k_w_order_list(Src s) { w_order_list_body(params(s)); }
 
 __device__ __forceinline__ u64 dbl_key(double d) {       // order-preserving image of a double
     const u64 b = (u64)__double_as_longlong(d);
@@ -893,15 +898,10 @@ __device__ __forceinline__ void w_order_times_body(const OrderParams &P) {
         }
     }
 }
-__global__ void __launch_bounds__(OW_WARPS * 32) k_w_order_times(OrderParams P) { w_order_times_body(P); }
+template <class Src> __global__ void __launch_bounds__(OW_WARPS * 32) k_w_order_times(Src s) { w_order_times_body(params(s)); }
 
-// several node-views per launch (swirld_kernels.cuh, view_params): blockIdx.y is the view
-template <int NJ>
-__global__ void __launch_bounds__(FW_THREADS) k_w_fame_rounds_views(const FameParams *Pv) { w_fame_rounds_body<NJ>(view_params(Pv)); }
-__global__ void __launch_bounds__(1024, 1) k_w_order_rounds_views(const OrderParams *Pv) {
-    const OrderParams &P = view_params(Pv);
-    if ((int)blockIdx.x < P.nrounds) w_order_rounds_body(P);
-}
-__global__ void __launch_bounds__(1024) k_w_order_cuts_views(const OrderParams *Pv) { w_order_cuts_body(view_params(Pv)); }
-__global__ void k_w_order_list_views(const OrderParams *Pv) { w_order_list_body(view_params(Pv)); }
-__global__ void __launch_bounds__(OW_WARPS * 32) k_w_order_times_views(const OrderParams *Pv) { w_order_times_body(view_params(Pv)); }
+SW_SRC_INSTANCES(k_w_order_rounds, OrderParams) SW_SRC_INSTANCES(k_w_order_cuts, OrderParams)
+SW_SRC_INSTANCES(k_w_order_list, OrderParams) SW_SRC_INSTANCES(k_w_order_times, OrderParams)
+#define SW_W_FAME_INSTANCES(NJ) template __global__ void k_w_fame_rounds<NJ, FameParams>(FameParams); \
+    template __global__ void k_w_fame_rounds<NJ, const FameParams *>(const FameParams *);
+SW_W_FAME_INSTANCES(1) SW_W_FAME_INSTANCES(2) SW_W_FAME_INSTANCES(4) SW_W_FAME_INSTANCES(8) SW_W_FAME_INSTANCES(16) SW_W_FAME_INSTANCES(32)
