@@ -53,7 +53,7 @@ typedef struct sw_stats_t {
     int64_t events_divided;    /* events through divide_rounds */
     double ms_rounds_kernel;   /* subset of ms_divide_rounds spent in the round-number kernel itself
                                   (M <= 64: k_rb_prep + k_rounds_cluster + k_rounds_batch; above: k_rounds_wide) */
-    int64_t rounds_cluster_launches;   /* launches of k_rounds_cluster / k_rounds_cluster_views: 0 when the device cannot
+    int64_t rounds_cluster_launches;   /* launches of k_rounds_cluster (one view or several): 0 when the device cannot
                                           hold the 16-CTA cluster and every chunk ran on the grid-wide k_rounds_batch */
 } sw_stats_t;
 

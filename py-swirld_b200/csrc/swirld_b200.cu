@@ -170,6 +170,11 @@ int fail(sw_engine *e, int code, const char *fmt, ...) {
     (e->NJ == 1 ? F<1>(__VA_ARGS__) : e->NJ == 2 ? F<2>(__VA_ARGS__) : e->NJ == 4 ? F<4>(__VA_ARGS__) \
      : e->NJ == 8 ? F<8>(__VA_ARGS__) : e->NJ == 16 ? F<16>(__VA_ARGS__) : F<32>(__VA_ARGS__))
 
+// call F<NC, UNIT>(args) for the M <= 64 kernels of engine x: its words per member set, and whether all stakes are 1
+#define SW_NCU(x, F, ...)                                                                \
+    ((x)->NC == 1 ? ((x)->unit ? F<1, true>(__VA_ARGS__) : F<1, false>(__VA_ARGS__))    \
+                  : ((x)->unit ? F<2, true>(__VA_ARGS__) : F<2, false>(__VA_ARGS__)))
+
 template <typename T>
 cudaError_t dalloc(T **p, size_t n) { return cudaMalloc((void **)p, std::max<size_t>(n, 1) * sizeof(T)); }
 
@@ -460,23 +465,28 @@ int chunk_prep(sw_engine *e, const RbParams &R, int32_t *rsg) {
     return 0;
 }
 
-// rounds of the chunk by the cooperative round-batch kernel (swirld_rounds.cuh), M <= 64: parameters + the grouping of
-// the chunk, with the seq-space rows for the cluster round kernel (`rows`)
-// (`grid` = CTAs this view's round kernel will run on)
-int round_batch_prep(sw_engine *e, int first, int n, int grid, bool rows, RbParams &R, int min_L = 1) {
+// rounds of the chunk by the cooperative round-batch kernel (swirld_rounds.cuh), M <= 64: parameters R + the grouping
+// of the chunk (`grid` = CTAs this view's round kernel will run on).  `rc`: the chunk goes to the cluster round kernel
+// first, with the parameters Q and the seq-space rows; R then continues from where the cluster stopped.
+int round_batch_prep(sw_engine *e, int first, int n, int grid, int min_L, bool rc, RbParams &R, RcParams &Q) {
     R = chunk_params(e, first, n);
     R.L = std::max(std::min(min_L, RB_LMAX), std::min(RB_LMAX, grid * (RB_THREADS / 32) / e->M));
     R.epoch = ++e->rb_epoch;
     R.Wf = e->d_Wf; R.sc = e->d_sc;
     R.res = e->d_res; R.stake = e->d_stake; R.tot2 = 2 * e->tot; R.scal = e->d_scal;
     R.SM = e->d_SM; R.dbg = e->d_dbg;
-    if (rows && (size_t)n > e->rsg_cap) {
+    if (rc && (size_t)n > e->rsg_cap) {
         if (e->d_rsg) { CK(cudaStreamSynchronize(e->stream)); CK(cudaFree(e->d_rsg)); e->d_rsg = nullptr; e->rsg_cap = 0; }
         const size_t want = std::min<size_t>((size_t)e->cap, std::max<size_t>((size_t)n, 1 << 16));
         CK(dalloc(&e->d_rsg, want * 64));
         e->rsg_cap = want;
     }
-    return chunk_prep<64>(e, R, rows ? e->d_rsg : nullptr);
+    if (chunk_prep<64>(e, R, rc ? e->d_rsg : nullptr) < 0) return SW_E_CUDA;
+    if (rc) {
+        Q = RcParams{R, e->d_rsg, e->d_rccont};
+        R.cont = e->d_rccont;
+    }
+    return 0;
 }
 
 // what follows the round kernel: ring of recent events, witness flags / table / list, seen-masks, strongly-seen sets
@@ -498,41 +508,63 @@ int round_batch_finish(sw_engine *e, const RbParams &R) {
     return 0;
 }
 
+// one thread-block cluster per view (blockIdx.y)
 void rc_launch_config(cudaLaunchConfig_t &cfg, cudaLaunchAttribute *at, int clusters, cudaStream_t stream) {
     cfg = cudaLaunchConfig_t{};
-    cfg.gridDim = dim3(RC_CS * clusters); cfg.blockDim = dim3(RC_THREADS); cfg.dynamicSmemBytes = RC_SMEM_BYTES; cfg.stream = stream;
+    cfg.gridDim = dim3(RC_CS, clusters); cfg.blockDim = dim3(RC_THREADS); cfg.dynamicSmemBytes = RC_SMEM_BYTES; cfg.stream = stream;
     at[0].id = cudaLaunchAttributeClusterDimension;
     at[0].val.clusterDim.x = RC_CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
 }
 
-// `start`: the event that opens the caller's span, recorded just before (the round-kernel span starts there too: an
-// event record costs the stream a few microseconds)
+// sw_create: the cluster round kernel's launch attributes, and how many of its clusters the device holds at once
+template <int NC, bool UNIT>
+cudaError_t rc_setup(int *clusters) {
+    cudaError_t er = cudaSuccess;
+    for (const void *fn : {(const void *)k_rounds_cluster<UNIT, RcParams>, (const void *)k_rounds_cluster<UNIT, const RcParams *>}) {
+        if (er == cudaSuccess) er = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RC_SMEM_BYTES);
+        if (er == cudaSuccess) er = cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    }
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute at[1];
+    rc_launch_config(cfg, at, 1, nullptr);
+    if (er == cudaSuccess) er = cudaOccupancyMaxActiveClusters(clusters, (const void *)k_rounds_cluster<UNIT, const RcParams *>, &cfg);
+    return er;
+}
+
+// The round kernels of nv views' chunks, G CTAs per view: with `rc` the chunk inside one thread-block cluster per view
+// first, then the cooperative kernel, which takes over whatever a cluster hands back (normally nothing).  R and Q are one
+// view's parameters (nv = 1) or the device arrays of nv views'.  The round-kernel span starts at `start`, which the
+// caller recorded; `shared`: it is the start of the caller's own span too (an event record costs the stream a few
+// microseconds).
+template <int NC, bool UNIT, class RSrc, class QSrc>
+int round_kernels(sw_engine *e, RSrc R, QSrc Q, int nv, int G, bool rc, cudaEvent_t start, bool shared) {
+    if (rc) {
+        cudaLaunchConfig_t cfg;
+        cudaLaunchAttribute at[1];
+        rc_launch_config(cfg, at, nv, e->stream);
+        CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster<UNIT, QSrc>, Q));
+        e->stats.kernel_launches += 1;
+        e->stats.rounds_cluster_launches += 1;
+    }
+    void *args[] = {(void *)&R};
+    CK(cudaLaunchCooperativeKernel((void *)k_rounds_batch<NC, UNIT, RSrc>, dim3(G, nv), dim3(RB_THREADS), args, 0, e->stream));
+    e->stats.kernel_launches += 1;
+    cudaEvent_t b = get_event(e);
+    cudaEventRecord(b, e->stream);
+    e->spans.push_back(TimedSpan{start, b, 4, shared});
+    return 0;
+}
+
+// `start`: the event that opens the caller's span, recorded just before
 template <int NC, bool UNIT>
 int divide_round_batch(sw_engine *e, int first, int n, cudaEvent_t start) {
     const int grid = std::max(e->n_sm / 2, e->n_sm - 16);       // 16 SMs stay free for the can_see scan of the next chunk
     const bool rc = e->rc_ok && n >= e->rc_min_n;
     RbParams R;
-    void *args[] = {(void *)&R};
-    {
-        cudaEvent_t b = get_event(e);
-        if (round_batch_prep(e, first, n, grid, rc, R) < 0) return SW_E_CUDA;
-        if (rc) {
-            // the chunk inside one thread-block cluster; k_rounds_batch takes over whatever it hands back (normally nothing)
-            RcParams Q{R, e->d_rsg, e->d_rccont};
-            cudaLaunchConfig_t cfg;
-            cudaLaunchAttribute at[1];
-            rc_launch_config(cfg, at, 1, e->stream);
-            CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster<UNIT>, Q));
-            R.cont = e->d_rccont;
-            e->stats.kernel_launches += 1;
-            e->stats.rounds_cluster_launches += 1;
-        }
-        CK(cudaLaunchCooperativeKernel((void *)k_rounds_batch<NC, UNIT>, dim3(grid), dim3(RB_THREADS), args, 0, e->stream));
-        e->stats.kernel_launches += 1;
-        cudaEventRecord(b, e->stream);
-        e->spans.push_back(TimedSpan{start, b, 4, true});
-    }
+    RcParams Q{};
+    if (round_batch_prep(e, first, n, grid, 1, rc, R, Q) < 0 || round_kernels<NC, UNIT>(e, R, Q, 1, grid, rc, start, true) < 0)
+        return SW_E_CUDA;
     return round_batch_finish<NC>(e, R);
 }
 
@@ -861,18 +893,7 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
             if (const char *v = getenv("SW_RC_MIN_N")) e->rc_min_n = std::max(1, atoi(v));
             if (want) {
                 int ncl = 0;
-                const void *fn = e->unit ? (const void *)k_rounds_cluster<true> : (const void *)k_rounds_cluster<false>;
-                cudaError_t er = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RC_SMEM_BYTES);
-                if (er == cudaSuccess) er = cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-                if (er == cudaSuccess) {
-                    const void *fv = e->unit ? (const void *)k_rounds_cluster_views<true> : (const void *)k_rounds_cluster_views<false>;
-                    er = cudaFuncSetAttribute(fv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RC_SMEM_BYTES);
-                    if (er == cudaSuccess) er = cudaFuncSetAttribute(fv, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-                    cudaLaunchConfig_t cfg;
-                    cudaLaunchAttribute at[1];
-                    rc_launch_config(cfg, at, 1, nullptr);
-                    if (er == cudaSuccess) er = cudaOccupancyMaxActiveClusters(&ncl, fv, &cfg);
-                }
+                const cudaError_t er = SW_NCU(e, rc_setup, &ncl);
                 e->rc_ok = er == cudaSuccess && ncl >= 1;
                 if (er != cudaSuccess) (void)cudaGetLastError();
             }
@@ -888,8 +909,8 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
         CK(dalloc(&e->d_ts, cap)); CK(dalloc(&e->d_key, cap * 8));
         for (auto &ev : e->stage_ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
         if (stage_slot(e, unpack_bytes(sw_engine::STAGE_EVENTS)) < 0) return SW_E_CUDA;   // (the ring, sized for sw_append)
-        CK(cudaFuncSetAttribute(k_stream_divide<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
-        CK(cudaFuncSetAttribute(k_stream_divide_views<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
+        CK(cudaFuncSetAttribute(k_stream_divide<true, StreamParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
+        CK(cudaFuncSetAttribute(k_stream_divide<true, const StreamParams *>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
         CK(cudaMallocHost((void **)&e->h_scal, sizeof(int32_t) * ((size_t)SC_COUNT + e->Rcap)));
         e->h_newc = e->h_scal + SC_COUNT;
         CK(cudaMemcpyAsync(e->d_stake, e->h_stake.data(), sizeof(i64) * M, cudaMemcpyHostToDevice, e->stream));
@@ -972,6 +993,19 @@ UnpackParams append_pack(const sw_engine *e, int n, const int32_t *p0, const int
     return U;
 }
 
+// The first `bytes` of slot `si` of the staging ring go over on the copy stream and one k_unpack scatters them: U is one
+// view's parameters (B = 1) or the device array of B views' at the start of the slot
+template <class Src>
+int unpack_staged(sw_engine *e, int si, size_t bytes, Src U, int B) {
+    cudaStream_t cs = e->copy_stream;
+    CK(cudaMemcpyAsync(e->d_stage + e->stage_bytes * si, e->h_stage + e->stage_bytes * si, bytes, cudaMemcpyHostToDevice, cs));
+    CK(cudaEventRecord(e->stage_ev[si], cs));
+    k_unpack<<<dim3(1, B), 256, 0, cs>>>(U);
+    CK(cudaGetLastError());
+    e->stats.kernel_launches += 1;
+    return 0;
+}
+
 // More events: one copy per column on the engine's copy stream (from pinned memory, asynchronous)
 int append_copy(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const int32_t *creator, const double *t,
                 const uint8_t *sig) {
@@ -1025,6 +1059,19 @@ StreamParams stream_params(const sw_engine *e, int first, int n) {
 int stream_threads(int M) { return std::min(1024, std::max(32, (M + 31) / 32 * 32)); }
 size_t stream_smem(int M) { return (size_t)M * 8 + 32 * 8 + (size_t)3 * M * 4 + 32 * 4; }
 
+// The one launch: S is one view's parameters (B = 1) or the device array of B views' (swirld_kernels.cuh, params)
+template <class Src>
+int stream_kernel(sw_engine *e, Src S, int B) {
+    {
+        Span sp(e, 0);
+        if (e->wide) k_stream_divide<true><<<dim3(1, B), stream_threads(e->M), stream_smem(e->M), e->stream>>>(S);
+        else k_stream_divide<false><<<dim3(1, B), stream_threads(e->M), stream_smem(e->M), e->stream>>>(S);
+        CK(cudaGetLastError());
+    }
+    e->stats.kernel_launches += 1;
+    return 0;
+}
+
 // the reference's own cadence (one sync per call): a call of at most STREAM_N events whose rows are current is divided
 // in ONE launch (swirld_stream.cuh)
 bool stream_path(const sw_engine *e, int first, int n) { return n <= sw_engine::STREAM_N && e->n_rowed == first; }
@@ -1057,6 +1104,54 @@ int stream_divided(sw_engine *e, int n) {
     if (rows_written(e) < 0) return SW_E_CUDA;
     divided(e, n);
     return 0;
+}
+
+// The chunk path of sw_batch_divide_rounds (M <= 64, one stake shape): every step of a view runs on the view's own
+// stream, except the round kernels, which advance side by side in ONE cooperative launch on the stream of `e`, the
+// first engine of the batch (its parameter buffers; it is charged the timings and launches).
+template <int NC, bool UNIT>
+int chunk_views(sw_engine *e, sw_engine *const *engines, int B, const int *first, const int *n) {
+    const int per_launch = e->n_sm;                         // (one CTA per view at least: its warps loop over its chains)
+    if (B > e->views_cap) {
+        if (e->d_views) cudaFree(e->d_views);
+        if (e->d_rcviews) cudaFree(e->d_rcviews);
+        e->d_views = nullptr; e->d_rcviews = nullptr;
+        CK(cudaMalloc((void **)&e->d_views, sizeof(RbParams) * B));
+        CK(cudaMalloc((void **)&e->d_rcviews, sizeof(RcParams) * B));
+        e->views_cap = B;
+    }
+    // one thread-block cluster per view first (swirld_rcluster.cuh); the grid-wide kernel then takes what they hand back
+    bool use_rc = true;
+    for (int v = 0; v < B; v++) use_rc = use_rc && engines[v]->rc_ok && n[v] >= e->rc_min_n;
+    std::vector<RcParams> Qv(B);
+    if (!e->view_ev) CK(cudaEventCreateWithFlags(&e->view_ev, cudaEventDisableTiming));
+    std::vector<RbParams> Rv(B);
+    for (int v0 = 0; v0 < B; v0 += per_launch) {
+        const int nv = std::min(per_launch, B - v0), G = e->n_sm / nv;
+        for (int v = v0; v < v0 + nv; v++) {
+            sw_engine *x = engines[v];
+            if (rows_ready(x, first[v], n[v]) < 0) return SW_E_CUDA;
+            // a view's window stays a round deep (16 pending events per chain) however few warps it has: they loop
+            if (round_batch_prep(x, first[v], n[v], G, 16, use_rc, Rv[v], Qv[v]) < 0) { e->err = x->err; return SW_E_CUDA; }
+            cudaEvent_t ev = get_event(x);
+            CK(cudaEventRecord(ev, x->stream));
+            CK(cudaStreamWaitEvent(e->stream, ev, 0));
+            x->pool.push_back(ev);
+        }
+        CK(cudaMemcpyAsync(e->d_views + v0, Rv.data() + v0, sizeof(RbParams) * nv, cudaMemcpyHostToDevice, e->stream));
+        cudaEvent_t a = get_event(e);
+        cudaEventRecord(a, e->stream);
+        if (use_rc) CK(cudaMemcpyAsync(e->d_rcviews + v0, Qv.data() + v0, sizeof(RcParams) * nv, cudaMemcpyHostToDevice, e->stream));
+        if (round_kernels<NC, UNIT>(e, (const RbParams *)e->d_views + v0, (const RcParams *)e->d_rcviews + v0, nv, G, use_rc, a, false) < 0)
+            return SW_E_CUDA;
+        CK(cudaEventRecord(e->view_ev, e->stream));
+        CK(cudaStreamSynchronize(e->stream));       // (Rv / the event are reused by the next group; the views' finish kernels follow)
+        for (int v = v0; v < v0 + nv; v++) {
+            if (round_batch_finish<NC>(engines[v], Rv[v]) < 0) return SW_E_CUDA;
+            divided(engines[v], n[v]);
+        }
+    }
+    return SW_OK;
 }
 
 }  // namespace
@@ -1164,25 +1259,19 @@ int sw_append(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const i
     if (rc < 0) return rc;
     // The copies go to their own stream: they touch only the new rows, so they overlap the kernels of
     // earlier chunks still running on the compute stream; later compute work waits for them.
-    cudaStream_t cs = e->copy_stream;
     if (n <= sw_engine::STAGE_EVENTS) {
         // a handful of events: pack the eight columns into one pinned block, one copy, one scatter kernel
         const int si = stage_slot(e, unpack_bytes(n));
         if (si < 0) return si;
-        uint8_t *hs = e->h_stage + e->stage_bytes * si, *ds = e->d_stage + e->stage_bytes * si;
-        const UnpackParams U = append_pack(e, n, p0, p1, creator, t, sig, hs, ds);
-        CK(cudaMemcpyAsync(ds, hs, unpack_bytes(n), cudaMemcpyHostToDevice, cs));
-        CK(cudaEventRecord(e->stage_ev[si], cs));
-        k_unpack<<<1, 256, 0, cs>>>(U);
-        CK(cudaGetLastError());
-        e->stats.kernel_launches += 1;
+        const UnpackParams U = append_pack(e, n, p0, p1, creator, t, sig, e->h_stage + e->stage_bytes * si, e->d_stage + e->stage_bytes * si);
+        if (unpack_staged(e, si, unpack_bytes(n), U, 1) < 0) return SW_E_CUDA;
     } else if (append_copy(e, n, p0, p1, creator, t, sig) < 0) return SW_E_CUDA;
-    return append_commit(e, n, cs);
+    return append_commit(e, n, e->copy_stream);
 }
 
 // Node.add_event for B node-views in one call.  Every view is validated as sw_append validates it; the views of at most
-// STAGE_EVENTS events go over packed in ONE block (their parameters first) and are scattered by ONE k_unpack_views, on
-// the first engine's copy stream; larger views make the copies their sw_append makes, on their own copy streams.
+// STAGE_EVENTS events go over packed in ONE block (their parameters first) and are scattered by ONE k_unpack, on the
+// first engine's copy stream; larger views make the copies their sw_append makes, on their own copy streams.
 int sw_batch_append(sw_engine *const *engines, int B, const int *offsets, const int32_t *p0, const int32_t *p1,
                     const int32_t *creator, const double *t, const uint8_t *sig, int32_t *rc_out) {
     sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
@@ -1215,7 +1304,6 @@ int sw_batch_append(sw_engine *const *engines, int B, const int *offsets, const 
     if (packed.empty()) return first_err;
     bytes += align256(sizeof(UnpackParams) * packed.size());
     // 2. the packed views: one slot of the first engine's ring, one copy, one scatter kernel
-    cudaStream_t cs = e->copy_stream;
     const int si = stage_slot(e, bytes);
     if (si < 0) return si;
     uint8_t *hs = e->h_stage + e->stage_bytes * si, *ds = e->d_stage + e->stage_bytes * si;
@@ -1227,14 +1315,10 @@ int sw_batch_append(sw_engine *const *engines, int B, const int *offsets, const 
         U[i] = append_pack(x, n, p0 + o, p1 + o, creator + o, t + o, sig + (size_t)64 * o, hs + off, ds + off);
         off += (unpack_bytes(n) + 15) & ~(size_t)15;
     }
-    CK(cudaMemcpyAsync(ds, hs, off, cudaMemcpyHostToDevice, cs));
-    CK(cudaEventRecord(e->stage_ev[si], cs));
-    k_unpack_views<<<(int)packed.size(), 256, 0, cs>>>(reinterpret_cast<const UnpackParams *>(ds));
-    CK(cudaGetLastError());
-    e->stats.kernel_launches += 1;
+    if (unpack_staged(e, si, off, reinterpret_cast<const UnpackParams *>(ds), (int)packed.size()) < 0) return SW_E_CUDA;
     // each view's pending-append event comes from its own pool (wait_appends returns it there)
     for (int v : packed)
-        if (append_commit(engines[v], offsets[v + 1] - offsets[v], cs) < 0) { e->err = engines[v]->err; return SW_E_CUDA; }
+        if (append_commit(engines[v], offsets[v + 1] - offsets[v], e->copy_stream) < 0) { e->err = engines[v]->err; return SW_E_CUDA; }
     return first_err;
 }
 
@@ -1245,107 +1329,22 @@ int sw_divide_rounds(sw_engine *e, int first, int n) {
     if (first + n > e->n_events) return fail(e, SW_E_KEY, "divide_rounds: events [%d,%d) not appended", first, first + n);
     CK(cudaSetDevice(e->device));
     if (stream_path(e, first, n)) {
-        if (wait_appends(e, first + n) < 0) return SW_E_CUDA;
-        const StreamParams S = stream_params(e, first, n);
-        const int threads = stream_threads(e->M);
-        const size_t smem = stream_smem(e->M);
-        {
-            Span sp(e, 0);
-            if (e->wide) k_stream_divide<true><<<1, threads, smem, e->stream>>>(S);
-            else k_stream_divide<false><<<1, threads, smem, e->stream>>>(S);
-            CK(cudaGetLastError());
-        }
-        e->stats.kernel_launches += 1;
+        if (wait_appends(e, first + n) < 0 || stream_kernel(e, stream_params(e, first, n), 1) < 0) return SW_E_CUDA;
         return stream_divided(e, n);         // (it wrote can_see rows and the carry heads on the compute stream)
     }
     int rc = rows_ready(e, first, n);
     if (rc < 0) return rc;
     {
         Span sp(e, 0);
-        if (e->wide) rc = SW_NJ(divide_rounds_wide, e, first, n);
-        else rc = e->NC == 1 ? (e->unit ? divide_round_batch<1, true>(e, first, n, sp.s.a) : divide_round_batch<1, false>(e, first, n, sp.s.a))
-                             : (e->unit ? divide_round_batch<2, true>(e, first, n, sp.s.a) : divide_round_batch<2, false>(e, first, n, sp.s.a));
+        rc = e->wide ? SW_NJ(divide_rounds_wide, e, first, n) : SW_NCU(e, divide_round_batch, e, first, n, sp.s.a);
         if (rc < 0) return rc;
     }
     divided(e, n);
     return SW_OK;
 }
 
-// The chunk path of sw_batch_divide_rounds (M <= 64, one stake shape): every step of a view runs on the view's own
-// stream, except the round kernels, which advance side by side in ONE cooperative launch on the stream of `e`, the
-// first engine of the batch (its parameter buffers; it is charged the timings and launches).
-static int chunk_views(sw_engine *e, sw_engine *const *engines, int B, const int *first, const int *n) {
-    const bool unit = engines[0]->unit;
-    const int per_launch = e->n_sm;                         // (one CTA per view at least: its warps loop over its chains)
-    if (B > e->views_cap) {
-        if (e->d_views) cudaFree(e->d_views);
-        if (e->d_rcviews) cudaFree(e->d_rcviews);
-        e->d_views = nullptr; e->d_rcviews = nullptr;
-        CK(cudaMalloc((void **)&e->d_views, sizeof(RbParams) * B));
-        CK(cudaMalloc((void **)&e->d_rcviews, sizeof(RcParams) * B));
-        e->views_cap = B;
-    }
-    // one thread-block cluster per view first (swirld_rcluster.cuh); the grid-wide kernel then takes what they hand back
-    bool use_rc = true;
-    for (int v = 0; v < B; v++) use_rc = use_rc && engines[v]->rc_ok && n[v] >= e->rc_min_n;
-    std::vector<RcParams> Qv(B);
-    if (!e->view_ev) CK(cudaEventCreateWithFlags(&e->view_ev, cudaEventDisableTiming));
-    std::vector<RbParams> Rv(B);
-    for (int v0 = 0; v0 < B; v0 += per_launch) {
-        const int nv = std::min(per_launch, B - v0), G = e->n_sm / nv;
-        for (int v = v0; v < v0 + nv; v++) {
-            sw_engine *x = engines[v];
-            if (rows_ready(x, first[v], n[v]) < 0) return SW_E_CUDA;
-            // a view's window stays a round deep (16 pending events per chain) however few warps it has: they loop
-            if (round_batch_prep(x, first[v], n[v], G, use_rc, Rv[v], 16) < 0) { e->err = x->err; return SW_E_CUDA; }
-            if (use_rc) {
-                Qv[v] = RcParams{Rv[v], x->d_rsg, x->d_rccont};
-                Rv[v].cont = x->d_rccont;
-            }
-            cudaEvent_t ev = get_event(x);
-            CK(cudaEventRecord(ev, x->stream));
-            CK(cudaStreamWaitEvent(e->stream, ev, 0));
-            x->pool.push_back(ev);
-        }
-        CK(cudaMemcpyAsync(e->d_views + v0, Rv.data() + v0, sizeof(RbParams) * nv, cudaMemcpyHostToDevice, e->stream));
-        const RbParams *pv = e->d_views + v0;
-        int g = G;
-        void *args[] = {(void *)&pv, (void *)&g};
-        {
-            cudaEvent_t a = get_event(e), b = get_event(e);
-            cudaEventRecord(a, e->stream);
-            if (use_rc) {
-                CK(cudaMemcpyAsync(e->d_rcviews + v0, Qv.data() + v0, sizeof(RcParams) * nv, cudaMemcpyHostToDevice, e->stream));
-                cudaLaunchConfig_t cfg;
-                cudaLaunchAttribute at[1];
-                rc_launch_config(cfg, at, nv, e->stream);
-                const RcParams *qv = e->d_rcviews + v0;
-                if (unit) CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster_views<true>, qv));
-                else CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster_views<false>, qv));
-                e->stats.kernel_launches += 1;
-                e->stats.rounds_cluster_launches += 1;
-            }
-            void *fn = e->NC == 1 ? (unit ? (void *)k_rounds_batch_views<1, true> : (void *)k_rounds_batch_views<1, false>)
-                                  : (unit ? (void *)k_rounds_batch_views<2, true> : (void *)k_rounds_batch_views<2, false>);
-            CK(cudaLaunchCooperativeKernel(fn, dim3(nv * G), dim3(RB_THREADS), args, 0, e->stream));
-            e->stats.kernel_launches += 1;
-            cudaEventRecord(b, e->stream);
-            e->spans.push_back(TimedSpan{a, b, 4});
-        }
-        CK(cudaEventRecord(e->view_ev, e->stream));
-        CK(cudaStreamSynchronize(e->stream));       // (Rv / the event are reused by the next group; the views' finish kernels follow)
-        for (int v = v0; v < v0 + nv; v++) {
-            sw_engine *x = engines[v];
-            int rc = x->NC == 1 ? round_batch_finish<1>(x, Rv[v]) : round_batch_finish<2>(x, Rv[v]);
-            if (rc < 0) return rc;
-            divided(x, n[v]);
-        }
-    }
-    return SW_OK;
-}
-
 // Node.divide_rounds for B independent node-views at once: every view takes the path its single call would take.  The
-// views whose call takes the one-launch path join ONE k_stream_divide_views launch (any M, any stakes); the others go
+// views whose call takes the one-launch path join ONE k_stream_divide launch (any M, any stakes); the others go
 // through chunk_views.
 int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, const int *n) {
     sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
@@ -1382,13 +1381,7 @@ int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, c
         }
         CK(cudaMemcpyAsync(e->d_stviews, Sv.data(), sizeof(StreamParams) * S, cudaMemcpyHostToDevice, e->stream));
         e->stats.h2d_bytes += sizeof(StreamParams) * S;
-        {
-            Span sp(e, 0);
-            if (e->wide) k_stream_divide_views<true><<<S, stream_threads(e->M), stream_smem(e->M), e->stream>>>(e->d_stviews);
-            else k_stream_divide_views<false><<<S, stream_threads(e->M), stream_smem(e->M), e->stream>>>(e->d_stviews);
-            CK(cudaGetLastError());
-        }
-        e->stats.kernel_launches += 1;
+        if (stream_kernel(e, (const StreamParams *)e->d_stviews, S) < 0) return SW_E_CUDA;
         // each view's later work runs after the batch: no copy, no host synchronisation
         if (!e->view_ev) CK(cudaEventCreateWithFlags(&e->view_ev, cudaEventDisableTiming));
         CK(cudaEventRecord(e->view_ev, e->stream));
@@ -1397,7 +1390,7 @@ int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, c
             if (stream_divided(sv[i], sn[i]) < 0) { e->err = sv[i]->err; return SW_E_CUDA; }
         }
     }
-    if (!cv.empty()) return chunk_views(e, cv.data(), (int)cv.size(), cfirst.data(), cn.data());
+    if (!cv.empty()) return SW_NCU(cv[0], chunk_views, e, cv.data(), (int)cv.size(), cfirst.data(), cn.data());
     return SW_OK;
 }
 

@@ -200,15 +200,17 @@ __device__ __forceinline__ void fame_collect(const FameParams &P, int max_c, int
     if (tid == 0) { P.scal[SC_NEWC] = s_base; P.scal[SC_MAXC] = max_c; }
 }
 
-// The fame and order kernels take their parameters from a Src: a value (one node-view per launch) or the device array
-// of the views of sw_batch_decide_fame / sw_batch_find_order.  Then blockIdx.y is the view, Pv[blockIdx.y] its
-// parameters, staged in shared memory; blockIdx.x and gridDim.x are what they are in a single-view launch, so the
-// grid-stride loops and k_fame_rounds' last-CTA ticket count one view's CTAs.  The order grids are sized from the view
-// with the most rounds: a CTA beyond its view's rounds exits.
+// The kernels that the sw_batch_* calls launch for several node-views take their parameters from a Src: a value (one
+// view per launch) or the device array of the views.  Then blockIdx.y is the view, Pv[blockIdx.y] its parameters,
+// staged in shared memory; blockIdx.x and gridDim.x are what they are in a single-view launch, so the grid-stride
+// loops, k_fame_rounds' last-CTA ticket and the round kernel's grid barrier count one view's CTAs.  The order grids are
+// sized from the view with the most rounds: a CTA beyond its view's rounds exits.
 template <typename T>
 __device__ __forceinline__ const T &view_params(const T *Pv) {
     __shared__ T Ps;
-    if (threadIdx.x == 0) Ps = Pv[blockIdx.y];
+    static_assert(sizeof(T) % 8 == 0, "staged in 8-byte words");
+    for (int i = threadIdx.x; i < (int)(sizeof(T) / 8); i += blockDim.x)     // (a struct copy goes through the stack)
+        reinterpret_cast<u64 *>(&Ps)[i] = reinterpret_cast<const u64 *>(Pv + blockIdx.y)[i];
     __syncthreads();
     return Ps;
 }
@@ -645,6 +647,9 @@ __global__ void __launch_bounds__(1024) k_order_sort(Src s) {
 
 // what the host launches: each kernel for one view by value and for the device array of several views
 #define SW_SRC_INSTANCES(K, T) template __global__ void K<T>(T); template __global__ void K<const T *>(const T *);
+// ... and for a kernel with template parameters before its Src
+#define SW_SRC_INSTANCES_OF(K, T, ...) \
+    template __global__ void K<__VA_ARGS__, T>(T); template __global__ void K<__VA_ARGS__, const T *>(const T *);
 SW_SRC_INSTANCES(k_fame_begin, FameParams) SW_SRC_INSTANCES(k_fame_rounds, FameParams) SW_SRC_INSTANCES(k_fame_finish, FameParams)
 SW_SRC_INSTANCES(k_order_rounds, OrderParams) SW_SRC_INSTANCES(k_order_cuts, OrderParams) SW_SRC_INSTANCES(k_order_list, OrderParams)
 SW_SRC_INSTANCES(k_order_times, OrderParams) SW_SRC_INSTANCES(k_order_sort, OrderParams)

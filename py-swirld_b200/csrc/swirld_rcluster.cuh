@@ -583,15 +583,8 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
     rc_cluster_sync();                                          // nobody leaves while its shared memory may still be written
 }
 
-template <bool UNIT>
-__global__ void __launch_bounds__(RC_THREADS, 1) k_rounds_cluster(RcParams Q) { rounds_cluster_body<UNIT>(Q); }
-
-// several independent node-views (swirld_rounds.cuh, k_rounds_batch_views): one cluster per view, as many side by side
-// as the device holds -- the clusters never talk to each other, so this is an ordinary (non-cooperative) launch
-template <bool UNIT>
-__global__ void __launch_bounds__(RC_THREADS, 1) k_rounds_cluster_views(const RcParams *Qv) {
-    __shared__ RcParams Qs;
-    if (threadIdx.x == 0) Qs = Qv[blockIdx.x / RC_CS];
-    __syncthreads();
-    rounds_cluster_body<UNIT>(Qs);
-}
+// several independent node-views (swirld_rounds.cuh, k_rounds_batch): one cluster per view (blockIdx.y), as many side
+// by side as the device holds -- the clusters never talk to each other, so this is an ordinary (non-cooperative) launch
+template <bool UNIT, class Src>
+__global__ void __launch_bounds__(RC_THREADS, 1) k_rounds_cluster(Src s) { rounds_cluster_body<UNIT>(params(s)); }
+SW_SRC_INSTANCES_OF(k_rounds_cluster, RcParams, false) SW_SRC_INSTANCES_OF(k_rounds_cluster, RcParams, true)

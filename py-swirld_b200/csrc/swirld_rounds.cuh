@@ -144,8 +144,7 @@ __device__ __forceinline__ u64 rb_key(int r, unsigned epoch) {
     return (u64)(r + 1) * 0x9E3779B97F4A7C15ull ^ (u64)(epoch + 1) * 0xC2B2AE3D27D4EB4Full;
 }
 
-// (bx, gx): this CTA's index and the CTA count of ITS hashgraph -- the whole grid, or one view's share of it when
-// several independent node-views advance in one launch (k_rounds_batch_views)
+// (bx, gx): this CTA's index and the CTA count of ITS hashgraph -- one view's row of the grid (k_rounds_batch)
 template <int NC, bool UNIT>
 __device__ __forceinline__ void rounds_batch_body(const RbParams &P, const int bx, const int gx) {
     __shared__ int cur[64], pos[64], len[64], off[64];
@@ -542,22 +541,16 @@ __device__ __forceinline__ void rounds_batch_body(const RbParams &P, const int b
     if (lead && tid == 0 && P.n > 0) P.scal[SC_MAX_ROUND] = rtop;
 }
 
-template <int NC, bool UNIT>
-__global__ void __launch_bounds__(RB_THREADS, 1) k_rounds_batch(RbParams P) {
-    rounds_batch_body<NC, UNIT>(P, blockIdx.x, gridDim.x);
-}
-
 // Several independent node-views (SURVEY.md section 8f-3: the simulation's M nodes each recompute consensus on nearly
-// the same graph, swirld.py:331-345) in ONE cooperative launch: view v runs on CTAs [v*G, (v+1)*G) with its own
-// parameters, barrier counter and result buffers.  The path is latency-bound (one grid-wide step per round), so G small
-// CTA groups advancing side by side use the GPU far better than one view on all of it.
-template <int NC, bool UNIT>
-__global__ void __launch_bounds__(RB_THREADS, 1) k_rounds_batch_views(const RbParams *Pv, int G) {
-    __shared__ RbParams Ps;
-    if (threadIdx.x == 0) Ps = Pv[blockIdx.x / G];
-    __syncthreads();
-    rounds_batch_body<NC, UNIT>(Ps, blockIdx.x % G, G);
+// the same graph, swirld.py:331-345) go in ONE cooperative launch: view blockIdx.y runs on its own row of CTAs with its
+// own parameters, barrier counter and result buffers.  The path is latency-bound (one grid-wide step per round), so
+// small CTA groups advancing side by side use the GPU far better than one view on all of it.
+template <int NC, bool UNIT, class Src>
+__global__ void __launch_bounds__(RB_THREADS, 1) k_rounds_batch(Src s) {
+    rounds_batch_body<NC, UNIT>(params(s), blockIdx.x, gridDim.x);
 }
+SW_SRC_INSTANCES_OF(k_rounds_batch, RbParams, 1, false) SW_SRC_INSTANCES_OF(k_rounds_batch, RbParams, 1, true)
+SW_SRC_INSTANCES_OF(k_rounds_batch, RbParams, 2, false) SW_SRC_INSTANCES_OF(k_rounds_batch, RbParams, 2, true)
 
 // ---- SM(h) = {c_ : W[round h][c_] >= 0 and row(h)[c_] >= W[round h][c_]}, one warp per event
 template <int NC>

@@ -147,20 +147,11 @@ __device__ __forceinline__ void stream_divide(const StreamParams &P) {
     if (c == 0 && P.n > 0) P.scal[SC_MAX_ROUND] = max_round;
 }
 
-template <bool WIDE>
-__global__ void __launch_bounds__(1024) k_stream_divide(StreamParams P) { stream_divide<WIDE>(P); }
-
-// sw_batch_divide_rounds: one CTA per node-view (blockIdx.x), every view's call of a handful of events in one launch.
-// The views share M (so the thread count and the dynamic shared memory); stakes and coin periods are per view.
-template <bool WIDE>
-__global__ void __launch_bounds__(1024) k_stream_divide_views(const StreamParams *Pv) {
-    __shared__ StreamParams P;
-    static_assert(sizeof(StreamParams) % 8 == 0, "staged in 8-byte words");
-    for (int i = threadIdx.x; i < (int)(sizeof(StreamParams) / 8); i += blockDim.x)     // (a struct copy goes through the stack)
-        reinterpret_cast<u64 *>(&P)[i] = reinterpret_cast<const u64 *>(Pv + blockIdx.x)[i];
-    __syncthreads();
-    stream_divide<WIDE>(P);
-}
+// One CTA per node-view: sw_batch_divide_rounds puts every view's call of a handful of events in one launch.  The
+// views share M (so the thread count and the dynamic shared memory); stakes and coin periods are per view.
+template <bool WIDE, class Src>
+__global__ void __launch_bounds__(1024) k_stream_divide(Src s) { stream_divide<WIDE>(params(s)); }
+SW_SRC_INSTANCES_OF(k_stream_divide, StreamParams, false) SW_SRC_INSTANCES_OF(k_stream_divide, StreamParams, true)
 
 // the event columns of a small append arrive as ONE packed block: scatter it to the SoA columns
 struct UnpackParams {
@@ -184,12 +175,6 @@ __device__ __forceinline__ void unpack(const UnpackParams &P) {
     }
     for (int i = threadIdx.x; i < 64 * n; i += blockDim.x) P.sig[(size_t)P.base * 64 + i] = sg[i];
 }
-__global__ void k_unpack(UnpackParams P) { unpack(P); }
-
-// sw_batch_append: one CTA per node-view (blockIdx.x); every view's `stage` points into one packed block
-__global__ void k_unpack_views(const UnpackParams *Uv) {
-    __shared__ UnpackParams P;
-    if (threadIdx.x == 0) P = Uv[blockIdx.x];
-    __syncthreads();
-    unpack(P);
-}
+// one CTA per node-view: sw_batch_append's views all point `stage` into one packed block
+template <class Src> __global__ void k_unpack(Src s) { unpack(params(s)); }
+SW_SRC_INSTANCES(k_unpack, UnpackParams)

@@ -902,6 +902,6 @@ template <class Src> __global__ void __launch_bounds__(OW_WARPS * 32) k_w_order_
 
 SW_SRC_INSTANCES(k_w_order_rounds, OrderParams) SW_SRC_INSTANCES(k_w_order_cuts, OrderParams)
 SW_SRC_INSTANCES(k_w_order_list, OrderParams) SW_SRC_INSTANCES(k_w_order_times, OrderParams)
-#define SW_W_FAME_INSTANCES(NJ) template __global__ void k_w_fame_rounds<NJ, FameParams>(FameParams); \
-    template __global__ void k_w_fame_rounds<NJ, const FameParams *>(const FameParams *);
-SW_W_FAME_INSTANCES(1) SW_W_FAME_INSTANCES(2) SW_W_FAME_INSTANCES(4) SW_W_FAME_INSTANCES(8) SW_W_FAME_INSTANCES(16) SW_W_FAME_INSTANCES(32)
+SW_SRC_INSTANCES_OF(k_w_fame_rounds, FameParams, 1) SW_SRC_INSTANCES_OF(k_w_fame_rounds, FameParams, 2)
+SW_SRC_INSTANCES_OF(k_w_fame_rounds, FameParams, 4) SW_SRC_INSTANCES_OF(k_w_fame_rounds, FameParams, 8)
+SW_SRC_INSTANCES_OF(k_w_fame_rounds, FameParams, 16) SW_SRC_INSTANCES_OF(k_w_fame_rounds, FameParams, 32)
