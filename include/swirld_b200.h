@@ -127,6 +127,13 @@ int sw_decide_fame(sw_engine *e, int32_t *new_c_out, int cap);
  * appended to the consensus order by this call (the caller owns the print of
  * swirld.py:310-311). */
 int sw_find_order(sw_engine *e, const int32_t *new_c, int n);
+/* sw_find_order, and also: the events this call appended to the order, in order, with their consensus time (ts[x],
+ * swirld.py:305) and round received (the r of swirld.py:283), into ev_out / ts_out / rr_out[0 .. return value).  cap must
+ * be >= sw_n_divided - sw_n_transactions (SW_E_ARG before anything runs otherwise).  The first 1024 events come back in
+ * the copy sw_find_order makes; a call that orders more copies the rest in one more round trip.  On an error the
+ * device finds (SW_E_INDEX, SW_E_KEY) the output is unspecified. */
+int sw_find_order_out(sw_engine *e, const int32_t *new_c, int n,
+                      int32_t *ev_out, double *ts_out, int32_t *rr_out, int cap);
 
 /* Node.decide_fame() and Node.find_order(new_c) for B independent node-views in one call each (the simulation's nodes
  * each run the reference's whole main loop, swirld.py:325-328).  The views share one member count (any M up to
@@ -148,6 +155,13 @@ int sw_batch_decide_fame(sw_engine *const *engines, int B, int32_t *new_c_out, i
 /* View v's rounds are new_c[offsets[v] .. offsets[v+1]) (an empty range does nothing); count_out[v] = events appended
  * to view v's order. */
 int sw_batch_find_order(sw_engine *const *engines, int B, const int32_t *new_c, const int *offsets, int32_t *count_out);
+/* sw_batch_find_order, and also: view v's output (as sw_find_order_out's) is packed at out_offsets[v] .. out_offsets[v+1]
+ * of ev_out / ts_out / rr_out (B+1 entries, written by the call; a failed view's range is empty); cap must be >= the sum
+ * over the views of sw_n_divided - sw_n_transactions (SW_E_ARG before anything runs otherwise).  The same launches and
+ * one copy back as sw_batch_find_order; views that order more than 1024 events add one more round trip in all. */
+int sw_batch_find_order_out(sw_engine *const *engines, int B, const int32_t *new_c, const int *offsets,
+                            int32_t *count_out, int32_t *ev_out, double *ts_out, int32_t *rr_out,
+                            int *out_offsets, int cap);
 
 /* ---- views of the Node attributes (swirld.py:48-72) ---- */
 int sw_members(const sw_engine *e);           /* n (swirld.py:40) */
@@ -162,6 +176,9 @@ int sw_get_can_see(sw_engine *e, int first, int n, int32_t *out);        /* can_
 int sw_get_witness_table(sw_engine *e, int first_round, int n_rounds, int32_t *out); /* witnesses[r][c], -1 absent */
 int sw_get_consensus(sw_engine *e, int32_t *out, int cap);               /* sorted(consensus) -> count */
 int sw_get_transactions(sw_engine *e, int first, int n, int32_t *out);   /* transactions[first:first+n] */
+/* by order position, parallel to sw_get_transactions: [first, first+n) within [0, sw_n_transactions) */
+int sw_get_consensus_times(sw_engine *e, int first, int n, double *out);    /* ts[x] of transactions[i], swirld.py:305 */
+int sw_get_rounds_received(sw_engine *e, int first, int n, int32_t *out);   /* the r of swirld.py:283 that ordered it */
 int sw_get_idx(sw_engine *e, int first, int n, int32_t *out);            /* idx.get(h, -1) */
 int sw_get_height(sw_engine *e, int first, int n, int32_t *out);         /* height[h] (swirld.py:68) */
 
@@ -191,7 +208,9 @@ int sw_lookup(sw_engine *e, int n, const uint8_t *ids, int32_t *index_out);   /*
 /* ---- checkpoint / resume (the reference keeps its state in memory only and uses pickle on the wire, swirld.py:129,160):
  * the engine's whole state -- event columns, can_see table, rounds, witness / fame tables, order -- as one binary file
  * of SoA sections.  sw_load builds a new engine from it (capacity_events 0 = the saved capacity; never less than the
- * saved event count) that continues exactly where the saved one stopped: the same later calls give the same results. */
+ * saved event count) that continues exactly where the saved one stopped: the same later calls give the same results.
+ * sw_save writes version 2 of the format; sw_load also reads version 1, which has no consensus times or rounds received:
+ * for the positions such a file had already ordered it reports round received -1 and time NaN (all bits set). */
 int sw_save(sw_engine *e, const char *path);
 int sw_load(const char *path, int device, int capacity_events, sw_engine **out);
 

@@ -113,11 +113,11 @@ struct sw_engine {
     i64 *d_stake = nullptr;
     int32_t *d_scal = nullptr;
     // find_order
-    int32_t *d_lastord = nullptr, *d_tx = nullptr, *d_idx = nullptr, *d_batch_ev = nullptr,
+    int32_t *d_lastord = nullptr, *d_tx = nullptr, *d_tx_rr = nullptr, *d_idx = nullptr, *d_batch_ev = nullptr,
             *d_batch_seg = nullptr, *d_seg_start = nullptr, *d_seg_fw = nullptr, *d_seg_nf = nullptr,
             *d_perm = nullptr, *d_rounds_in = nullptr, *d_plan = nullptr;
     uint8_t *d_seg_white = nullptr;
-    double *d_ts = nullptr;
+    double *d_ts = nullptr, *d_tx_ts = nullptr;   // d_tx_ts, d_tx_rr: by order position, parallel to d_tx
     u64 *d_key = nullptr;
     int seg_cap = 0;
     void *d_flush = nullptr;
@@ -649,6 +649,14 @@ void fame_kernels(sw_engine *e, Src P, int B) {
 constexpr int FAME_SPEC = 1024;
 int fame_spec(const sw_engine *e) { return std::min(e->Rcap, FAME_SPEC); }
 
+// find_order's output comes back the same way: the first events a call orders, with their consensus times and rounds
+// received (OrderOut, 4 ints each), wait behind the scalars in the room of the new rounds (decide_fame has copied
+// those back before any find_order runs) and ride on the copy of the scalars.  The window is what the call can order at
+// most, n_divided - n_transactions, up to ORDER_SPEC; a call that orders more copies the rest from the columns.
+constexpr int ORDER_SPEC = 1024;
+int order_spec(const sw_engine *e) { return std::min(e->n_divided - e->n_tx, ORDER_SPEC); }
+size_t scal_room(const sw_engine *e) { return (size_t)std::max(e->Rcap, 4 * ORDER_SPEC); }   // ints behind the scalars
+
 // What decide_fame does once that copy is in h_scal: `r` = the error the device found, or the count of new rounds,
 // which go to `out` (a second copy when more came than the first one held).  Returns < 0 only when a copy fails.
 int fame_result(sw_engine *e, int32_t *out, int cap, int &r) {
@@ -696,7 +704,8 @@ OrderParams order_params(const sw_engine *e, int n, const int32_t *rounds) {
     P.row = e->d_row; P.p0 = e->d_p0; P.creator = e->d_creator; P.seq = e->d_seq; P.t = e->d_t; P.sig = e->d_sig;
     P.stake = e->d_stake; P.tot = e->tot; P.lastord = e->d_lastord; P.batch_ev = e->d_batch_ev; P.batch_seg = e->d_batch_seg;
     P.seg_start = e->d_seg_start; P.seg_fw = e->d_seg_fw; P.seg_nf = e->d_seg_nf; P.seg_white = e->d_seg_white;
-    P.ts = e->d_ts; P.key = e->d_key; P.perm = e->d_perm; P.tx = e->d_tx; P.idx = e->d_idx; P.tx_base = e->n_tx; P.scal = e->d_scal;
+    P.ts = e->d_ts; P.key = e->d_key; P.perm = e->d_perm; P.tx = e->d_tx; P.tx_cap = e->cap;
+    P.idx = e->d_idx; P.tx_base = e->n_tx; P.scal = e->d_scal; P.out_n = 0;
     P.plan = e->d_plan; P.plan_stride = (int)(e->seg_cap * e->MS);
     return P;
 }
@@ -738,6 +747,21 @@ int order_result(sw_engine *e) {
     const int nbatch = e->h_scal[SC_BATCH];
     e->n_tx += nbatch;
     return nbatch;
+}
+
+// The output of a find_order call that ordered the positions [base, base + cnt), of which the first `staged` came back
+// in `st`, into ev/ts/rr[0, cnt): the rest is copied from the columns on stream `s` (the caller synchronises it once).
+int order_output(sw_engine *e, cudaStream_t s, int base, int cnt, const OrderOut *st, int staged,
+                 int32_t *ev, double *ts, int32_t *rr) {
+    const int k = std::min(cnt, staged);
+    for (int i = 0; i < k; i++) { ev[i] = st[i].ev; ts[i] = st[i].ts; rr[i] = st[i].rr; }
+    if (cnt > k) {
+        const size_t n = cnt - k, at = (size_t)base + k;
+        CK(cudaMemcpyAsync(ev + k, e->d_tx + at, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(ts + k, e->d_tx_ts + at, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(rr + k, e->d_tx_rr + at, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s));
+    }
+    return cnt - k;
 }
 
 // ---- several node-views per call (sw_batch_*)
@@ -902,16 +926,18 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
         CK(dalloc(&e->d_W, RM)); CK(dalloc(&e->d_famous, RM));
         CK(dalloc(&e->d_consensus, (size_t)e->Rcap)); CK(dalloc(&e->d_done, (size_t)e->Rcap)); CK(dalloc(&e->d_coin, RM));
         CK(dalloc(&e->d_rem, (size_t)e->Rcap));
-        CK(dalloc(&e->d_stake, (size_t)M)); CK(dalloc(&e->d_scal, (size_t)SC_COUNT + e->Rcap));
+        CK(dalloc(&e->d_stake, (size_t)M)); CK(dalloc(&e->d_scal, (size_t)SC_COUNT + scal_room(e)));
         e->d_newc = e->d_scal + SC_COUNT;                  // (sw_decide_fame copies the scalars and the new rounds at once)
-        CK(dalloc(&e->d_lastord, MP)); CK(dalloc(&e->d_tx, cap)); CK(dalloc(&e->d_idx, cap));
+        CK(dalloc(&e->d_lastord, MP)); CK(dalloc(&e->d_tx, 4 * cap)); CK(dalloc(&e->d_idx, cap));
+        e->d_tx_rr = e->d_tx + cap;                        // (one block: OrderParams finds both from d_tx and cap)
+        e->d_tx_ts = reinterpret_cast<double *>(e->d_tx + 2 * cap);
         CK(dalloc(&e->d_batch_ev, cap)); CK(dalloc(&e->d_batch_seg, cap)); CK(dalloc(&e->d_perm, 2 * cap));
         CK(dalloc(&e->d_ts, cap)); CK(dalloc(&e->d_key, cap * 8));
         for (auto &ev : e->stage_ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
         if (stage_slot(e, unpack_bytes(sw_engine::STAGE_EVENTS)) < 0) return SW_E_CUDA;   // (the ring, sized for sw_append)
         CK(cudaFuncSetAttribute(k_stream_divide<true, StreamParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
         CK(cudaFuncSetAttribute(k_stream_divide<true, const StreamParams *>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
-        CK(cudaMallocHost((void **)&e->h_scal, sizeof(int32_t) * ((size_t)SC_COUNT + e->Rcap)));
+        CK(cudaMallocHost((void **)&e->h_scal, sizeof(int32_t) * ((size_t)SC_COUNT + scal_room(e))));
         e->h_newc = e->h_scal + SC_COUNT;
         CK(cudaMemcpyAsync(e->d_stake, e->h_stake.data(), sizeof(i64) * M, cudaMemcpyHostToDevice, e->stream));
         // kernels that need more than the default 48 KB of dynamic shared memory: the limit is a property of the kernel in
@@ -1158,7 +1184,7 @@ int chunk_views(sw_engine *e, sw_engine *const *engines, int B, const int *first
 
 extern "C" {
 
-int sw_version(void) { return 203; }
+int sw_version(void) { return 204; }
 
 const char *sw_last_error(const sw_engine *e) { return e ? e->err.c_str() : g_create_error.c_str(); }
 
@@ -1414,7 +1440,15 @@ int sw_decide_fame(sw_engine *e, int32_t *new_c_out, int cap) {
 }
 
 int sw_find_order(sw_engine *e, const int32_t *new_c, int n) {
-    if (!e || n < 0 || (n > 0 && !new_c)) return fail(e, SW_E_ARG, "bad argument");
+    return sw_find_order_out(e, new_c, n, nullptr, nullptr, nullptr, 0);
+}
+
+int sw_find_order_out(sw_engine *e, const int32_t *new_c, int n, int32_t *ev_out, double *ts_out, int32_t *rr_out, int cap) {
+    if (!e || n < 0 || (n > 0 && !new_c) || cap < 0 || (cap > 0 && (!ev_out || !ts_out || !rr_out)))
+        return fail(e, SW_E_ARG, "bad argument");
+    const bool want = ev_out != nullptr;               // (sw_find_order: the count only)
+    if (want && cap < e->n_divided - e->n_tx)
+        return fail(e, SW_E_ARG, "find_order: cap=%d < %d events it may order", cap, e->n_divided - e->n_tx);
     if (n == 0) return 0;
     CK(cudaSetDevice(e->device));
     std::vector<int32_t> rs(new_c, new_c + n);
@@ -1424,16 +1458,29 @@ int sw_find_order(sw_engine *e, const int32_t *new_c, int n) {
     CK(cudaMemcpyAsync(e->d_rounds_in, rs.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, e->stream));
     cudaEvent_t a = get_event(e), b = get_event(e);
     cudaEventRecord(a, e->stream);
-    order_kernels(e, order_params(e, n, e->d_rounds_in), 1, n);
+    OrderParams P = order_params(e, n, e->d_rounds_in);
+    P.out_n = want ? order_spec(e) : 0;
+    order_kernels(e, P, 1, n);
     CK(cudaGetLastError());
     cudaEventRecord(b, e->stream);
     e->spans.push_back(TimedSpan{a, b, 2});
-    CK(cudaMemcpyAsync(e->h_scal, e->d_scal, sizeof(int32_t) * SC_COUNT, cudaMemcpyDeviceToHost, e->stream));
+    const size_t bytes = sizeof(int32_t) * (SC_COUNT + 4 * (size_t)P.out_n);
+    CK(cudaMemcpyAsync(e->h_scal, e->d_scal, bytes, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));      // (rs, the host vector of the rounds, was consumed by the copy above)
     fold_spans(e);
     e->stats.h2d_bytes += sizeof(int32_t) * n;
-    e->stats.d2h_bytes += sizeof(int32_t) * SC_COUNT;
-    return order_result(e);
+    e->stats.d2h_bytes += bytes;
+    const int base = e->n_tx;
+    const int r = order_result(e);
+    if (r <= 0 || !want) return r;
+    const int rest = order_output(e, e->stream, base, r, reinterpret_cast<const OrderOut *>(e->h_scal + SC_COUNT), P.out_n,
+                                  ev_out, ts_out, rr_out);
+    if (rest < 0) return rest;
+    if (rest > 0) {
+        CK(cudaStreamSynchronize(e->stream));
+        e->stats.d2h_bytes += (2 * sizeof(int32_t) + sizeof(double)) * (size_t)rest;
+    }
+    return r;
 }
 
 // Node.decide_fame for B node-views in one call: the fame kernels of every view side by side in one grid (blockIdx.y =
@@ -1481,8 +1528,15 @@ int sw_batch_decide_fame(sw_engine *const *engines, int B, int32_t *new_c_out, i
 // Node.find_order for B node-views in one call: the five order kernels of every view with rounds to order side by side
 // (blockIdx.y = view), the views' parameters and rounds in one copy there, their scalars in one copy back.
 int sw_batch_find_order(sw_engine *const *engines, int B, const int32_t *new_c, const int *offsets, int32_t *count_out) {
+    return sw_batch_find_order_out(engines, B, new_c, offsets, count_out, nullptr, nullptr, nullptr, nullptr, 0);
+}
+
+int sw_batch_find_order_out(sw_engine *const *engines, int B, const int32_t *new_c, const int *offsets, int32_t *count_out,
+                            int32_t *ev_out, double *ts_out, int32_t *rr_out, int *out_offsets, int cap) {
     sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
-    if (!e || !offsets || !count_out) return fail(e, SW_E_ARG, "bad argument");
+    const bool want = out_offsets != nullptr;          // (sw_batch_find_order: the counts only)
+    if (!e || !offsets || !count_out || cap < 0 || (want && cap > 0 && (!ev_out || !ts_out || !rr_out)))
+        return fail(e, SW_E_ARG, "bad argument");
     int rc = check_views(engines, B, "sw_batch_find_order", true);
     if (rc < 0) return rc;
     if (offsets[0] < 0) return fail(e, SW_E_ARG, "sw_batch_find_order: offsets[0] = %d", offsets[0]);
@@ -1503,14 +1557,24 @@ int sw_batch_find_order(sw_engine *const *engines, int B, const int32_t *new_c, 
             return fail(e, SW_E_KEY, "sw_batch_find_order: view %d: unknown round %d", v, bad);
         if (n > 0) { act.push_back(engines[v]); act_v.push_back(v); maxn = std::max(maxn, n); }
     }
+    // the output: every view's window is the largest of the active views' (one row length for the gather)
+    int win = 0;
+    if (want) {
+        i64 need = 0;
+        for (int v = 0; v < B; v++) need += engines[v]->n_divided - engines[v]->n_tx;
+        if (need > cap) return fail(e, SW_E_ARG, "sw_batch_find_order: cap=%d < %lld events the views may order", cap, (long long)need);
+        for (sw_engine *x : act) win = std::max(win, order_spec(x));
+    }
     for (int v = 0; v < B; v++) count_out[v] = 0;
+    if (want) for (int v = 0; v <= B; v++) out_offsets[v] = 0;
     const int A = (int)act.size();
     if (A == 0) return SW_OK;
     CK(cudaSetDevice(e->device));
     for (int i = 0; i < A; i++) if (order_scratch(act[i], offsets[act_v[i] + 1] - offsets[act_v[i]]) < 0) { e->err = act[i]->err; return SW_E_CUDA; }
-    // [A parameter blocks][the rounds] go over in one copy; [A x SC_COUNT] scalars come back in one
+    // [A parameter blocks][the rounds] go over in one copy; A rows of the scalars and the output window come back in one
+    const int S = SC_COUNT + 4 * win;
     const size_t pbytes = sizeof(OrderParams) * A, inbytes = pbytes + sizeof(int32_t) * total, soff = align256(inbytes);
-    const size_t sbytes = sizeof(int32_t) * (size_t)SC_COUNT * A;
+    const size_t sbytes = sizeof(int32_t) * (size_t)S * A;
     if (views_buffer(e, soff + sbytes) < 0) return SW_E_CUDA;
     OrderParams *hP = reinterpret_cast<OrderParams *>(e->h_vbuf);
     int32_t *h_rounds = reinterpret_cast<int32_t *>(e->h_vbuf + pbytes);
@@ -1519,6 +1583,7 @@ int sw_batch_find_order(sw_engine *const *engines, int B, const int32_t *new_c, 
     for (int i = 0; i < A; i++) {
         const int v = act_v[i];
         hP[i] = order_params(act[i], offsets[v + 1] - offsets[v], d_rounds + (offsets[v] - offsets[0]));
+        hP[i].out_n = win;
     }
     const OrderParams *Pv = reinterpret_cast<const OrderParams *>(e->d_vbuf);
     int32_t *d_st = reinterpret_cast<int32_t *>(e->d_vbuf + soff), *h_st = reinterpret_cast<int32_t *>(e->h_vbuf + soff);
@@ -1528,7 +1593,7 @@ int sw_batch_find_order(sw_engine *const *engines, int B, const int32_t *new_c, 
     cudaEvent_t a = get_event(e), b = get_event(e);
     cudaEventRecord(a, e->stream);
     order_kernels(e, Pv, A, maxn);
-    k_views_gather<<<A, 32, 0, e->stream>>>(Pv, d_st, SC_COUNT);
+    k_views_gather<<<A, win ? 256 : 32, 0, e->stream>>>(Pv, d_st, S);
     CK(cudaGetLastError());
     cudaEventRecord(b, e->stream);
     e->spans.push_back(TimedSpan{a, b, 2});
@@ -1536,12 +1601,28 @@ int sw_batch_find_order(sw_engine *const *engines, int B, const int32_t *new_c, 
     if (views_leave(e, act.data(), A, h_st, d_st, sbytes) < 0) return SW_E_CUDA;
     fold_spans(e);
     int first_err = SW_OK;
+    size_t rest = 0;
+    int pos = 0, vn = 0;                               // view v's output is packed at pos (out_offsets[v] .. [v+1])
     for (int i = 0; i < A; i++) {
         sw_engine *x = act[i];
-        memcpy(x->h_scal, h_st + (size_t)SC_COUNT * i, sizeof(int32_t) * SC_COUNT);
+        memcpy(x->h_scal, h_st + (size_t)S * i, sizeof(int32_t) * SC_COUNT);
+        const int base = x->n_tx;
         const int r = order_result(x);
         count_out[act_v[i]] = r;
         if (r < 0 && first_err == SW_OK) first_err = r;
+        if (!want) continue;
+        for (; vn <= act_v[i]; vn++) out_offsets[vn] = pos;
+        if (r <= 0) continue;
+        const int k = order_output(x, e->stream, base, r, reinterpret_cast<const OrderOut *>(h_st + (size_t)S * i + SC_COUNT),
+                                   win, ev_out + pos, ts_out + pos, rr_out + pos);
+        if (k < 0) { e->err = x->err; return k; }
+        rest += k;
+        pos += r;
+    }
+    if (want) for (; vn <= B; vn++) out_offsets[vn] = pos;
+    if (rest > 0) {                                    // the views that ordered more than the window: one more synchronisation
+        CK(cudaStreamSynchronize(e->stream));
+        e->stats.d2h_bytes += (2 * sizeof(int32_t) + sizeof(double)) * rest;
     }
     return first_err;
 }
@@ -1594,6 +1675,8 @@ GETTER(sw_get_famous, int8_t, e->d_famous_ev, e->n_events, 1)
 GETTER(sw_get_can_see, int32_t, e->d_row, e->n_divided, e->M)
 GETTER(sw_get_witness_table, int32_t, e->d_W, e->Rcap, e->M)
 GETTER(sw_get_transactions, int32_t, e->d_tx, e->n_tx, 1)
+GETTER(sw_get_consensus_times, double, e->d_tx_ts, e->n_tx, 1)
+GETTER(sw_get_rounds_received, int32_t, e->d_tx_rr, e->n_tx, 1)
 GETTER(sw_get_idx, int32_t, e->d_idx, e->n_events, 1)
 
 int sw_get_height(sw_engine *e, int first, int n, int32_t *out) {
@@ -1780,14 +1863,16 @@ bool get_dev(sw_engine *e, FILE *f, void *d, size_t bytes, std::vector<char> &tm
 }
 
 // The file: the header, the stake (sw_load needs it to create the engine), then these sections in this order, each
-// sized from the header's counts.  `idrec`: the id records, 36 bytes each (32-byte id, arrival index).
+// sized from the header's counts.  `idrec`: the id records, 36 bytes each (32-byte id, arrival index).  Version 2 adds
+// the consensus times and rounds received of the ordered positions behind them.
+constexpr int32_t CKPT_VERSION = 2;
 struct Section { void *p; size_t bytes; bool dev; };
 std::vector<Section> ckpt_sections(sw_engine *e, const CkptHeader &H, std::vector<uint8_t> &idrec) {
     const size_t M = H.M, n = H.n_events, nd = H.n_divided, nr = H.n_rowed, NJ = H.NJ, R = H.rounds, RM = R * M;
-    const size_t i4 = sizeof(int32_t);
+    const size_t i4 = sizeof(int32_t), ntx = H.n_tx;
     const Section SM = H.wide ? Section{e->d_SMw, sizeof(unsigned) * nd * NJ, true} : Section{e->d_SM, sizeof(u64) * nd, true};
     const Section S = H.wide ? Section{e->d_Sw, sizeof(unsigned) * RM * NJ, true} : Section{e->d_S, sizeof(u64) * RM, true};
-    return {
+    std::vector<Section> v = {
         {e->h_creator.data(), i4 * n, false}, {e->h_head.data(), i4 * M, false}, {e->h_count.data(), i4 * M, false},
         {e->h_height, i4 * n, false}, {e->h_seq, i4 * n, false}, {e->h_stale, n, false},
         {e->d_p0, i4 * n, true}, {e->d_p1, i4 * n, true}, {e->d_creator, i4 * n, true}, {e->d_t, sizeof(double) * n, true},
@@ -1796,6 +1881,8 @@ std::vector<Section> ckpt_sections(sw_engine *e, const CkptHeader &H, std::vecto
         {e->d_W, i4 * RM, true}, {e->d_Wf, i4 * RM, true}, {e->d_famous, RM, true}, {e->d_coin, RM, true},
         S, {e->d_consensus, R, true}, {e->d_lastord, i4 * M, true}, {e->d_cs_carry, i4 * M, true}, {e->d_rbtot, i4 * M, true},
         {e->d_gchain, i4 * M * RB_RING, true}, {e->d_scal, i4 * SC_COUNT, true}, {idrec.data(), idrec.size(), false}};
+    if (H.version >= 2) { v.push_back({e->d_tx_ts, sizeof(double) * ntx, true}); v.push_back({e->d_tx_rr, i4 * ntx, true}); }
+    return v;
 }
 }  // namespace
 
@@ -1810,7 +1897,7 @@ int sw_save(sw_engine *e, const char *path) {
     const int R = std::min(e->Rcap, e->h_scal[SC_MAX_ROUND] + 2);
     CkptHeader H{};
     memcpy(H.magic, CKPT_MAGIC, 8);
-    H.version = 1; H.M = M; H.cap = e->cap; H.C = e->C; H.Rcap = e->Rcap; H.wide = e->wide ? 1 : 0; H.NJ = e->NJ;
+    H.version = CKPT_VERSION; H.M = M; H.cap = e->cap; H.C = e->C; H.Rcap = e->Rcap; H.wide = e->wide ? 1 : 0; H.NJ = e->NJ;
     H.n_events = n; H.n_divided = nd; H.n_tx = e->n_tx; H.n_rowed = nr; H.rounds = R; H.rb_epoch = e->rb_epoch;
     H.n_ids = (uint32_t)e->ids.size();
     std::vector<uint8_t> idrec((size_t)36 * e->ids.size());
@@ -1831,7 +1918,7 @@ int sw_load(const char *path, int device, int capacity_events, sw_engine **out) 
     FILE *f = fopen(path, "rb");
     if (!f) return fail(e, SW_E_ARG, "sw_load: cannot open %s", path);
     CkptHeader H{};
-    if (fread(&H, sizeof H, 1, f) != 1 || memcmp(H.magic, CKPT_MAGIC, 8) != 0 || H.version != 1 || H.M < 1 || H.M > SW_MAX_MEMBERS
+    if (fread(&H, sizeof H, 1, f) != 1 || memcmp(H.magic, CKPT_MAGIC, 8) != 0 || H.version < 1 || H.version > CKPT_VERSION || H.M < 1 || H.M > SW_MAX_MEMBERS
         || (H.M > 64 && !H.wide)) {
         fclose(f);
         return fail(e, SW_E_ARG, "sw_load: %s is not a swirld_b200 checkpoint", path);
@@ -1857,6 +1944,11 @@ int sw_load(const char *path, int device, int capacity_events, sw_engine **out) 
     bool ok2 = cudaMemcpy(e->d_seq, e->h_seq, sizeof(int32_t) * n, cudaMemcpyHostToDevice) == cudaSuccess
         && cudaMemcpy(e->d_height, e->h_height, sizeof(int32_t) * n, cudaMemcpyHostToDevice) == cudaSuccess
         && cudaMemcpy(e->d_stale, e->h_stale, (size_t)n, cudaMemcpyHostToDevice) == cudaSuccess;
+    // a version-1 file has no times or rounds received for what it had ordered: NaN (all bits set) and -1
+    if (ok2 && H.version < 2)
+        ok2 = cudaMemsetAsync(e->d_tx_ts, 0xff, sizeof(double) * (size_t)H.n_tx, e->stream) == cudaSuccess
+            && cudaMemsetAsync(e->d_tx_rr, 0xff, sizeof(int32_t) * (size_t)H.n_tx, e->stream) == cudaSuccess
+            && cudaStreamSynchronize(e->stream) == cudaSuccess;
     if (!ok2) { sw_destroy(e); return fail(nullptr, SW_E_CUDA, "sw_load: device copy failed"); }
     e->n_events = n; e->n_divided = nd; e->n_tx = H.n_tx; e->n_rowed = nr; e->rb_epoch = H.rb_epoch;
     e->h_stale_cum.assign((size_t)n + 1, 0);

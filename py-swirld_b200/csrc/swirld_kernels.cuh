@@ -335,8 +335,14 @@ __global__ void __launch_bounds__(1024, 1) k_fame_finish(Src s) {
 }
 
 // ---------------------------------------------------------------- K4: find_order
+// One entry of a find_order call's output as the host copies it back behind the scalars: the event, its round received
+// (the r of swirld.py:283) and its consensus timestamp (ts[x], swirld.py:305)
+struct OrderOut { int32_t ev, rr; double ts; };
+static_assert(sizeof(OrderOut) == 4 * sizeof(int32_t), "OrderOut is 4 ints of the scalar block");
+
 struct OrderParams {
     int M, Rcap, nrounds;
+    int tx_cap;                  // the order columns: tx[tx_cap] int32, then rounds received int32, then times f64
     const int32_t *rounds;       // [nrounds] sorted(new_c)
     const int32_t *W;
     const int8_t *famous;
@@ -356,15 +362,18 @@ struct OrderParams {
     double *ts;                  // [cap] per batch slot
     u64 *key;                    // [cap][8] big-endian words of white ^ sig
     int32_t *perm;               // [cap] scratch
-    int32_t *tx;                 // [cap] transactions
+    int32_t *tx;                 // [cap] transactions (and behind them, see tx_cap, their rounds received and times)
     int32_t *idx;                // [cap]
     int tx_base;
+    int out_n;                   // the first out_n events this call orders go behind the scalars (0: the count only)
     int32_t *scal;
     // plan scratch, 8 planes of [plan_stride] ints indexed by segment*64 + chain (or witness slot):
     // 0 thr, 1 reach over all famous witnesses, 2 seq[thr], 3 seq[reach], 4 creator of witness slot, 5 cut, 6 count, 7 offset
     int32_t *plan;
     int plan_stride;
 };
+// (the batched calls copy it once per view: the new fields sit in what was padding)
+static_assert(sizeof(OrderParams) == 232, "OrderParams keeps its size");
 
 // Plan: for each new consensus round the famous witnesses f_w, the whitening
 // XOR (swirld.py:284-285) and, per member chain c, the range of events this round
@@ -609,11 +618,13 @@ __device__ __forceinline__ bool order_less(const OrderParams &P, int a, int b) {
 
 // One CTA per segment: bitonic sort of the segment's batch slots (padded to a power of
 // two with -1 = +infinity; P.perm holds 2 ints per batch slot so the padding is real),
-// then append to transactions / idx (swirld.py:306-309).
+// then append to transactions / idx (swirld.py:306-309), with each event's consensus timestamp and round received at its
+// position, and the first out_n of them behind the scalars (OrderOut), where the copy of the scalars brings them back.
 __device__ __forceinline__ void order_sort_body(const OrderParams &P) {
     const int si = blockIdx.x;
     const int s0 = P.seg_start[si], cnt = P.seg_start[si + 1] - s0;
     if (cnt <= 0) return;
+    const int r = P.rounds[si];
     int n2 = 1;
     while (n2 < cnt) n2 <<= 1;
     int32_t *perm = P.perm + 2 * (size_t)s0;        // n2 < 2 * cnt
@@ -633,13 +644,17 @@ __device__ __forceinline__ void order_sort_body(const OrderParams &P) {
             __syncthreads();
         }
     for (int i = threadIdx.x; i < cnt; i += blockDim.x) {
-        const int x = P.batch_ev[perm[i]];
-        P.tx[P.tx_base + s0 + i] = x;
-        P.idx[x] = P.tx_base + s0 + i;
+        const int b = perm[i], x = P.batch_ev[b], pos = s0 + i;
+        const double ts = P.ts[b];
+        P.tx[P.tx_base + pos] = x;
+        P.tx[(size_t)P.tx_cap + P.tx_base + pos] = r;
+        reinterpret_cast<double *>(P.tx + 2 * (size_t)P.tx_cap)[P.tx_base + pos] = ts;
+        P.idx[x] = P.tx_base + pos;
+        if (pos < P.out_n) { OrderOut &o = reinterpret_cast<OrderOut *>(P.scal + SC_COUNT)[pos]; o.ev = x; o.rr = r; o.ts = ts; }
     }
 }
 template <class Src>
-__global__ void __launch_bounds__(1024) k_order_sort(Src s) {
+__global__ void __launch_bounds__(1024, 1) k_order_sort(Src s) {
     const OrderParams &P = params(s);
     if constexpr (std::is_pointer<Src>::value) if ((int)blockIdx.x >= P.nrounds) return;
     order_sort_body(P);
@@ -654,12 +669,16 @@ SW_SRC_INSTANCES(k_fame_begin, FameParams) SW_SRC_INSTANCES(k_fame_rounds, FameP
 SW_SRC_INSTANCES(k_order_rounds, OrderParams) SW_SRC_INSTANCES(k_order_cuts, OrderParams) SW_SRC_INSTANCES(k_order_list, OrderParams)
 SW_SRC_INSTANCES(k_order_times, OrderParams) SW_SRC_INSTANCES(k_order_sort, OrderParams)
 
-// the first n ints of every view's scalar block (SC_*, and for decide_fame the new rounds behind them) into row v of
-// one staging array: one device-to-host copy brings back what B single calls copy one by one
+// what a view's scalar block holds behind the scalars: decide_fame's new rounds (Rcap entries), find_order's output
+__device__ __forceinline__ int gather_room(const FameParams &P) { return SC_COUNT + P.Rcap; }
+__device__ __forceinline__ int gather_room(const OrderParams &P) { return SC_COUNT + 4 * P.out_n; }
+
+// the first n ints of every view's scalar block (SC_*, and for decide_fame the new rounds or for find_order the output
+// behind them) into row v of one staging array: one device-to-host copy brings back what B single calls copy one by one
 template <typename T>
 __global__ void k_views_gather(const T *Pv, int32_t *out, int n) {
     const T &P = Pv[blockIdx.x];
-    const int m = min(n, SC_COUNT + P.Rcap);               // (the new rounds' array holds Rcap entries)
+    const int m = min(n, gather_room(P));
     for (int i = threadIdx.x; i < m; i += blockDim.x) out[(size_t)blockIdx.x * n + i] = P.scal[i];
 }
 

@@ -27,6 +27,7 @@ SYMBOLS = [
     "sw_sync", "sw_stats", "sw_flush_l2", "sw_version", "sw_debug_counters", "sw_peer_handle", "sw_peer_connect",
     "sw_save", "sw_load", "sw_members", "sw_ingest", "sw_lookup", "sw_batch_divide_rounds",
     "sw_batch_decide_fame", "sw_batch_find_order", "sw_batch_append",
+    "sw_get_consensus_times", "sw_get_rounds_received", "sw_find_order_out", "sw_batch_find_order_out",
 ]
 
 
@@ -76,7 +77,8 @@ def load_library(path: str = LIB_PATH):
     for f in ("sw_n_events", "sw_n_divided", "sw_max_round", "sw_n_transactions", "sw_sync"):
         getattr(L, f).argtypes = [vp]
     for f in ("sw_get_round", "sw_get_witness_flags", "sw_get_famous", "sw_get_can_see",
-              "sw_get_witness_table", "sw_get_transactions", "sw_get_idx", "sw_get_height"):
+              "sw_get_witness_table", "sw_get_transactions", "sw_get_idx", "sw_get_height",
+              "sw_get_consensus_times", "sw_get_rounds_received"):
         getattr(L, f).argtypes = [vp, i32, i32, vp]
     L.sw_get_consensus.argtypes = [vp, vp, i32]
     L.sw_stats.argtypes = [vp, P(SwStats)]
@@ -91,6 +93,8 @@ def load_library(path: str = LIB_PATH):
     L.sw_batch_divide_rounds.argtypes = [vp, i32, vp, vp]
     L.sw_batch_decide_fame.argtypes = [vp, i32, vp, i32, vp]
     L.sw_batch_find_order.argtypes = [vp, i32, vp, vp, vp]
+    L.sw_find_order_out.argtypes = [vp, vp, i32, vp, vp, vp, i32]
+    L.sw_batch_find_order_out.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, i32]
     L.sw_batch_append.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp]
     L.sw_save.argtypes = [vp, C.c_char_p]
     L.sw_load.argtypes = [C.c_char_p, i32, i32, P(vp)]
@@ -224,6 +228,16 @@ class Engine:
             return 0
         return self._chk(self._lib.sw_find_order(self._h, _ptr(a), a.size))
 
+    def find_order_out(self, new_c):
+        """find_order, returning what it appended to the order: (events, consensus times, rounds received), the
+        parallel arrays transactions() / consensus_times() / rounds_received() gain, from the copy find_order makes
+        anyway."""
+        a = np.ascontiguousarray(sorted(new_c), np.int32)
+        cap = max(0, self.n_divided - self.n_transactions)
+        ev, ts, rr = np.empty(cap, np.int32), np.empty(cap, np.float64), np.empty(cap, np.int32)
+        n = self._chk(self._lib.sw_find_order_out(self._h, _ptr(a), a.size, _ptr(ev), _ptr(ts), _ptr(rr), cap))
+        return ev[:n].copy(), ts[:n].copy(), rr[:n].copy()
+
     # -- views
     @property
     def n_events(self):
@@ -277,6 +291,14 @@ class Engine:
 
     def transactions(self, first=0, n=None):
         return self._get(self._lib.sw_get_transactions, np.int32, first, self.n_transactions - first if n is None else n)
+
+    def consensus_times(self, first=0, n=None):
+        """The consensus timestamp (swirld.py:305) of transactions()[first:first+n]."""
+        return self._get(self._lib.sw_get_consensus_times, np.float64, first, self.n_transactions - first if n is None else n)
+
+    def rounds_received(self, first=0, n=None):
+        """The round received (the round whose find_order step ordered it, swirld.py:283) of transactions()[first:first+n]."""
+        return self._get(self._lib.sw_get_rounds_received, np.int32, first, self.n_transactions - first if n is None else n)
 
     def idx(self, first=0, n=None):
         return self._get(self._lib.sw_get_idx, np.int32, first, self.n_events - first if n is None else n)
@@ -408,6 +430,29 @@ def batch_find_order(engines, new_cs):
     if rc < 0 and not (cnt < 0).any():
         engines[0]._chk(rc)
     return _per_view("batch_find_order", engines, [int(n) for n in cnt], cnt)
+
+
+def batch_find_order_out(engines, new_cs):
+    """sw_batch_find_order_out: batch_find_order, returning each view's (events, consensus times, rounds received), as
+    Engine.find_order_out does, from the one copy the batched call makes; errors as batch_find_order."""
+    B = len(engines)
+    assert len(new_cs) == B
+    if B == 0:
+        return []
+    flat = np.ascontiguousarray(np.concatenate([np.asarray(sorted(nc), np.int32) for nc in new_cs]), np.int32)
+    offs = np.zeros(B + 1, np.int32)
+    offs[1:] = np.cumsum([len(nc) for nc in new_cs])
+    cnt = np.zeros(B, np.int32)
+    cap = sum(max(0, e.n_divided - e.n_transactions) for e in engines)
+    ev, ts, rr = np.empty(cap, np.int32), np.empty(cap, np.float64), np.empty(cap, np.int32)
+    oo = np.zeros(B + 1, np.int32)
+    rc = engines[0]._lib.sw_batch_find_order_out(_handles(engines), B, _ptr(flat), _ptr(offs), _ptr(cnt),
+                                                 _ptr(ev), _ptr(ts), _ptr(rr), _ptr(oo), cap)
+    if rc < 0 and not (cnt < 0).any():
+        engines[0]._chk(rc)
+    none = (ev[:0], ts[:0], rr[:0])
+    out = [(ev[a:b], ts[a:b], rr[a:b]) if b > a else none for a, b in zip(oo[:-1].tolist(), oo[1:].tolist())]
+    return _per_view("batch_find_order_out", engines, out, cnt)
 
 
 def run_engine(tr, K, stake=None, coin_period=6, device=0, find_order=True):

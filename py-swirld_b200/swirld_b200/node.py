@@ -10,7 +10,9 @@ while the consensus state and the three hot-path methods (`divide_rounds`, `deci
 `find_order`: swirld.py:187-311) run on the GPU through the C ABI.  The attributes `viz.py` and the
 drivers read (`round`, `famous`, `idx`, `can_see`, `witnesses`, `tbd`) become lazy mapping views that
 pull from the device only what is asked for; `hg`, `height`, `head`, `transactions`, `consensus`
-stay plain Python objects.  Hashes (bytes) are mapped to arrival indices and public keys to member
+stay plain Python objects.  Beyond the reference's surface, `consensus_time` and `round_received` map
+each ordered event to its consensus timestamp (swirld.py:305) and the round that ordered it
+(swirld.py:283); find_order brings them back with the order itself.  Hashes (bytes) are mapped to arrival indices and public keys to member
 ids at this boundary.
 
 No CPU fallback: constructing a bound node without the CUDA library / a GPU raises.
@@ -51,6 +53,29 @@ class _View(Mapping):
 
     def __len__(self):
         return self._count() if self._count is not None else sum(1 for _ in self)
+
+
+class _OrderView(Mapping):
+    """Read-only dict-like view keyed by event hash over a host list parallel to `transactions` (ordered events only)."""
+
+    def __init__(self, node, values):
+        self._n, self._v = node, values
+
+    def __getitem__(self, h):
+        i = self._n._order_pos.get(h)
+        if i is None or i >= len(self._v):
+            raise KeyError(h)
+        return self._v[i]
+
+    def __contains__(self, h):
+        i = self._n._order_pos.get(h)
+        return i is not None and i < len(self._v)
+
+    def __iter__(self):
+        return iter(self._n.transactions[:len(self._v)])
+
+    def __len__(self):
+        return len(self._v)
 
 
 class _Witnesses(Mapping):
@@ -105,6 +130,8 @@ class GpuConsensus:
         self._ops = []                     # the call schedule, replayed if the engine has to grow
         self.head = None
         self.transactions, self.consensus, self.votes = [], set(), {}
+        self._order_pos = {}               # event hash -> its position in transactions
+        self._tx_ts, self._tx_rr = [], []  # parallel to transactions (empty when the engine cannot report them)
         self._round_cache = np.empty(0, np.int32)
         self._famous_cache = self._idx_cache = None
         self._views = {
@@ -115,6 +142,8 @@ class GpuConsensus:
                          lambda: len(self.transactions)),
             "can_see": _View(self, self._can_see_of, lambda i: i < self._eng.n_divided, lambda: self._eng.n_divided),
             "witnesses": _Witnesses(self),
+            "consensus_time": _OrderView(self, self._tx_ts),
+            "round_received": _OrderView(self, self._tx_rr),
         }
         h, ev = self.new_event(None, ())   # the node's own root (the host class signs and hashes it)
         self.add_event(h, ev)
@@ -126,6 +155,8 @@ class GpuConsensus:
     idx = property(lambda self: self._views["idx"])
     can_see = property(lambda self: self._views["can_see"])
     witnesses = property(lambda self: self._views["witnesses"])
+    consensus_time = property(lambda self: self._views["consensus_time"])
+    round_received = property(lambda self: self._views["round_received"])
 
     @property
     def tbd(self):
@@ -262,11 +293,19 @@ class GpuConsensus:
         """Consensus order of the events received in the new rounds (swirld.py:280-311)."""
         new_c = sorted(new_c)
         if new_c:
-            added = self._eng.find_order(new_c)
+            have = len(self.transactions)
+            if hasattr(self._eng, "find_order_out"):     # the order, times and rounds received in one copy
+                ev, ts, rr = self._eng.find_order_out(new_c)
+                self._tx_ts += ts.tolist()
+                self._tx_rr += rr.tolist()
+            else:
+                added = self._eng.find_order(new_c)
+                ev = self._eng.transactions(have, added) if added else ()
             self._ops.append(("o", tuple(new_c)))
-            if added:
-                have = len(self.transactions)
-                self.transactions += [self._i2h[int(i)] for i in self._eng.transactions(have, added)]
+            if len(ev):
+                new = [self._i2h[int(i)] for i in ev]
+                self._order_pos.update((h, have + j) for j, h in enumerate(new))
+                self.transactions += new
                 self._idx_cache = None
         if self.consensus:
             print(self.consensus)                  # swirld.py:310-311
