@@ -46,13 +46,15 @@ typedef struct sw_stats_t {
     double ms_decide_fame;     /* k_fame_* */
     double ms_find_order;      /* k_order_* */
     double ms_can_see;         /* subset of ms_divide_rounds spent in a stand-alone can_see kernel, 0 if fused */
-    int64_t kernel_launches;   /* kernels of this library launched */
+    int64_t kernel_launches;   /* kernels of this library launched (a divide_rounds call whose rounds ran ahead on the
+                                  round stream counts the launches the same call makes without it) */
     int64_t h2d_bytes;
     int64_t d2h_bytes;
     int64_t events;            /* events appended */
     int64_t events_divided;    /* events through divide_rounds */
     double ms_rounds_kernel;   /* subset of ms_divide_rounds spent in the round-number kernel itself
-                                  (M <= 64: k_rb_prep + k_rounds_cluster + k_rounds_batch; above: k_rounds_wide) */
+                                  (M <= 64: k_rb_prep + k_rounds_cluster + k_rounds_batch; above: k_rounds_wide);
+                                  round kernels run ahead on the round stream (SW_ROUNDS_AHEAD) are not timed */
     int64_t rounds_cluster_launches;   /* launches of k_rounds_cluster (one view or several): 0 when the device cannot
                                           hold the 16-CTA cluster and every chunk ran on the grid-wide k_rounds_batch */
 } sw_stats_t;

@@ -73,6 +73,22 @@ struct sw_engine {
     size_t rsg_cap = 0;           // events d_rsg holds
     bool rc_ok = false;           // a 16-CTA cluster with its shared memory can be resident on this device
     int rc_min_n = 2048;          // shorter chunks go to the grid-wide kernel directly
+    // The rounds run ahead (SW_ROUNDS_AHEAD, M <= 64, calls that go to the cluster kernel): a call whose can_see rows reach
+    // beyond its end starts the round kernels of the next piece of events on `rstream`, which then runs beside the call's
+    // finish and fame kernels and the host's turn-around.  Round numbers are a function of the graph alone, so the piece
+    // writes the final rounds of its events; what the engine shows a caller (Wf, the ring, the counts, the round top,
+    // errors) stays the compute stream's, and the round stream keeps its own copies: `d_Wf2`, `d_gchain2`, `d_rbmeta2`
+    // (chunk meta, counts, barrier, witness count) and `d_rscal` (round top, error slot).  One piece at most is in flight:
+    // [n_divided, n_rounded), ended by `rdone`.
+    bool ahead = false;
+    cudaStream_t rstream = nullptr;
+    cudaEvent_t rdone = nullptr, rwait = nullptr;
+    int32_t *d_Wf2 = nullptr, *d_gchain2 = nullptr, *d_rbmeta2 = nullptr, *d_rscal = nullptr;
+    bool rs_synced = false;       // the round stream's copies hold everything below n_rounded
+    int n_rounded = 0;            // events rounded so far (the round stream's piece ends here)
+    int rs_prev_first = 0, rs_prev_n = 0;   // the round stream's last piece, whose events its ring has not taken yet
+    unsigned rs_epoch = 0;        // launches on the round stream (mask-cache keys of their own: the top bit set)
+    int wslot = 0;                // which of the two witness counts of d_rbmeta the next call uses
     RcParams *d_rcviews = nullptr;
     RbParams *d_views = nullptr;  // sw_batch_divide_rounds: the views' parameters (owned by the first engine of a batch)
     int views_cap = 0;
@@ -260,6 +276,7 @@ int reset_state(sw_engine *e, bool keep_events = false) {
     e->n_divided = e->n_tx = 0;
     e->n_rowed = 0;
     e->rb_epoch = 0;
+    e->n_rounded = 0; e->rs_epoch = 0;
     if (!keep_events) {
         e->n_events = 0;
         std::fill(e->h_head.begin(), e->h_head.end(), -1);
@@ -446,8 +463,9 @@ RbParams chunk_params(const sw_engine *e, int first, int n) {
 // the chunk's events grouped by creator (k_rb_prep) from the per-member counts of the host mirror: [first, first+n)
 // holds seqs [lo[c], hi[c]) of member c.  `rsg` (M <= 64): also the seq-space rows of the cluster round kernel.
 template <int CM>
-int chunk_prep(sw_engine *e, const RbParams &R, int32_t *rsg) {
+int chunk_prep(sw_engine *e, const RbParams &R, int32_t *rsg, cudaStream_t st, int32_t *ring = nullptr, int rfirst = 0, int rn = 0) {
     RbChunk<CM> K;
+    K.ring = ring; K.rfirst = rfirst; K.rn = rn;
     int32_t lo[CM];
     counts_at(e, R.first, lo);
     counts_at(e, R.first + R.n, K.ctot);
@@ -459,9 +477,32 @@ int chunk_prep(sw_engine *e, const RbParams &R, int32_t *rsg) {
         K.coff[c] = o; o += cnt;
     }
     K.coff[CM] = o;
-    k_rb_prep<CM><<<std::max(1, std::min(8 * e->n_sm, (R.n + 7) / 8)), 256, 0, e->stream>>>(R, K, rsg);
+    k_rb_prep<CM><<<std::max(1, std::min(8 * e->n_sm, (R.n + 7) / 8)), 256, 0, st>>>(R, K, rsg);
     CK(cudaGetLastError());
-    e->stats.kernel_launches += 1;
+    return 0;
+}
+
+// what the round kernels read besides the chunk (the engine's Wf and scalars; the round stream swaps in its own)
+RbParams round_params(const sw_engine *e, int first, int n, int grid, int min_L) {
+    RbParams R = chunk_params(e, first, n);
+    R.L = std::max(std::min(min_L, RB_LMAX), std::min(RB_LMAX, grid * (RB_THREADS / 32) / e->M));
+    R.Wf = e->d_Wf; R.sc = e->d_sc;
+    R.res = e->d_res; R.stake = e->d_stake; R.tot2 = 2 * e->tot; R.scal = e->d_scal;
+    R.SM = e->d_SM; R.dbg = e->d_dbg;
+    return R;
+}
+
+// the cluster kernel's seq-space rows for n events (both streams use them: a new buffer waits for both)
+int rsg_reserve(sw_engine *e, int n) {
+    if ((size_t)n <= e->rsg_cap) return 0;
+    if (e->d_rsg) {
+        CK(cudaStreamSynchronize(e->stream));
+        if (e->rstream) CK(cudaStreamSynchronize(e->rstream));
+        CK(cudaFree(e->d_rsg)); e->d_rsg = nullptr; e->rsg_cap = 0;
+    }
+    const size_t want = std::min<size_t>((size_t)e->cap, std::max<size_t>((size_t)n, 1 << 16));
+    CK(dalloc(&e->d_rsg, want * 64));
+    e->rsg_cap = want;
     return 0;
 }
 
@@ -469,19 +510,11 @@ int chunk_prep(sw_engine *e, const RbParams &R, int32_t *rsg) {
 // of the chunk (`grid` = CTAs this view's round kernel will run on).  `rc`: the chunk goes to the cluster round kernel
 // first, with the parameters Q and the seq-space rows; R then continues from where the cluster stopped.
 int round_batch_prep(sw_engine *e, int first, int n, int grid, int min_L, bool rc, RbParams &R, RcParams &Q) {
-    R = chunk_params(e, first, n);
-    R.L = std::max(std::min(min_L, RB_LMAX), std::min(RB_LMAX, grid * (RB_THREADS / 32) / e->M));
+    R = round_params(e, first, n, grid, min_L);
     R.epoch = ++e->rb_epoch;
-    R.Wf = e->d_Wf; R.sc = e->d_sc;
-    R.res = e->d_res; R.stake = e->d_stake; R.tot2 = 2 * e->tot; R.scal = e->d_scal;
-    R.SM = e->d_SM; R.dbg = e->d_dbg;
-    if (rc && (size_t)n > e->rsg_cap) {
-        if (e->d_rsg) { CK(cudaStreamSynchronize(e->stream)); CK(cudaFree(e->d_rsg)); e->d_rsg = nullptr; e->rsg_cap = 0; }
-        const size_t want = std::min<size_t>((size_t)e->cap, std::max<size_t>((size_t)n, 1 << 16));
-        CK(dalloc(&e->d_rsg, want * 64));
-        e->rsg_cap = want;
-    }
-    if (chunk_prep<64>(e, R, rc ? e->d_rsg : nullptr) < 0) return SW_E_CUDA;
+    if (rc && rsg_reserve(e, n) < 0) return SW_E_CUDA;
+    if (chunk_prep<64>(e, R, rc ? e->d_rsg : nullptr, e->stream) < 0) return SW_E_CUDA;
+    e->stats.kernel_launches += 1;
     if (rc) {
         Q = RcParams{R, e->d_rsg, e->d_rccont};
         R.cont = e->d_rccont;
@@ -491,9 +524,9 @@ int round_batch_prep(sw_engine *e, int first, int n, int grid, int min_L, bool r
 
 // what follows the round kernel: ring of recent events, witness flags / table / list, seen-masks, strongly-seen sets
 template <int NC>
-int round_batch_finish(sw_engine *e, const RbParams &R) {
+int round_batch_finish(sw_engine *e, const RbParams &R, const RbFold &F = RbFold{}) {
     const int n = R.n, blocks = std::max(1, std::min(296, (n + 255) / 256));
-    k_rb_finish<<<blocks, 256, 0, e->stream>>>(R);
+    k_rb_finish<<<blocks, 256, 0, e->stream>>>(R, F);
     k_rb_seenmask<NC><<<(n + 7) / 8, 256, 0, e->stream>>>(R);
     CK(cudaGetLastError());
     StrongParams Q{};
@@ -532,28 +565,34 @@ cudaError_t rc_setup(int *clusters) {
     return er;
 }
 
-// The round kernels of nv views' chunks, G CTAs per view: with `rc` the chunk inside one thread-block cluster per view
-// first, then the cooperative kernel, which takes over whatever a cluster hands back (normally nothing).  R and Q are one
-// view's parameters (nv = 1) or the device arrays of nv views'.  The round-kernel span starts at `start`, which the
-// caller recorded; `shared`: it is the start of the caller's own span too (an event record costs the stream a few
-// microseconds).
+// The round kernels of nv views' chunks on stream `st`, G CTAs per view: with `rc` the chunk inside one thread-block
+// cluster per view first, then the cooperative kernel, which takes over whatever a cluster hands back (normally nothing).
+// R and Q are one view's parameters (nv = 1) or the device arrays of nv views'.
 template <int NC, bool UNIT, class RSrc, class QSrc>
-int round_kernels(sw_engine *e, RSrc R, QSrc Q, int nv, int G, bool rc, cudaEvent_t start, bool shared) {
+int round_kernels(sw_engine *e, RSrc R, QSrc Q, int nv, int G, bool rc, cudaStream_t st) {
     if (rc) {
         cudaLaunchConfig_t cfg;
         cudaLaunchAttribute at[1];
-        rc_launch_config(cfg, at, nv, e->stream);
+        rc_launch_config(cfg, at, nv, st);
         CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster<UNIT, QSrc>, Q));
-        e->stats.kernel_launches += 1;
-        e->stats.rounds_cluster_launches += 1;
     }
     void *args[] = {(void *)&R};
-    CK(cudaLaunchCooperativeKernel((void *)k_rounds_batch<NC, UNIT, RSrc>, dim3(G, nv), dim3(RB_THREADS), args, 0, e->stream));
-    e->stats.kernel_launches += 1;
+    CK(cudaLaunchCooperativeKernel((void *)k_rounds_batch<NC, UNIT, RSrc>, dim3(G, nv), dim3(RB_THREADS), args, 0, st));
+    return 0;
+}
+
+// what the round kernels of one call count, wherever they ran
+void count_round_kernels(sw_engine *e, bool rc) {
+    e->stats.kernel_launches += rc ? 2 : 1;
+    e->stats.rounds_cluster_launches += rc ? 1 : 0;
+}
+
+// The round-kernel span from `start`, which the caller recorded; `shared`: it is the start of the caller's own span too (an
+// event record costs the stream a few microseconds)
+void round_span(sw_engine *e, cudaEvent_t start, bool shared) {
     cudaEvent_t b = get_event(e);
     cudaEventRecord(b, e->stream);
     e->spans.push_back(TimedSpan{start, b, 4, shared});
-    return 0;
 }
 
 // `start`: the event that opens the caller's span, recorded just before
@@ -563,9 +602,102 @@ int divide_round_batch(sw_engine *e, int first, int n, cudaEvent_t start) {
     const bool rc = e->rc_ok && n >= e->rc_min_n;
     RbParams R;
     RcParams Q{};
-    if (round_batch_prep(e, first, n, grid, 1, rc, R, Q) < 0 || round_kernels<NC, UNIT>(e, R, Q, 1, grid, rc, start, true) < 0)
+    if (round_batch_prep(e, first, n, grid, 1, rc, R, Q) < 0 || round_kernels<NC, UNIT>(e, R, Q, 1, grid, rc, e->stream) < 0)
         return SW_E_CUDA;
+    count_round_kernels(e, rc);
+    round_span(e, start, true);
     return round_batch_finish<NC>(e, R);
+}
+
+// ---- the rounds run ahead (sw_engine::ahead)
+// Everything but the ahead path writes the engine's own Wf, ring and counts: before it runs, the compute stream waits for
+// the round stream's piece, which is given up (its rounds are computed again), and so are the round stream's copies.
+int rs_drain(sw_engine *e) {
+    if (e->rs_synced) CK(cudaStreamWaitEvent(e->stream, e->rdone, 0));
+    e->rs_synced = false;
+    e->n_rounded = e->n_divided;
+    return 0;
+}
+
+// the round stream goes on after what the compute stream has been given so far
+int rs_follow(sw_engine *e) {
+    CK(cudaEventRecord(e->rwait, e->stream));
+    CK(cudaStreamWaitEvent(e->rstream, e->rwait, 0));
+    return 0;
+}
+
+// the round stream's copies of the engine's Wf, ring and scalars, at the first call of a run of ahead calls
+int rs_sync(sw_engine *e) {
+    if (e->rs_synced) return 0;
+    if (rs_follow(e) < 0) return SW_E_CUDA;
+    CK(cudaMemcpyAsync(e->d_Wf2, e->d_Wf, sizeof(int32_t) * e->Rcap * e->M, cudaMemcpyDeviceToDevice, e->rstream));
+    CK(cudaMemcpyAsync(e->d_gchain2, e->d_gchain, sizeof(int32_t) * e->MP * RB_RING, cudaMemcpyDeviceToDevice, e->rstream));
+    CK(cudaMemcpyAsync(e->d_rscal, e->d_scal, sizeof(int32_t) * SC_COUNT, cudaMemcpyDeviceToDevice, e->rstream));
+    CK(cudaMemsetAsync(rb_meta(e).wcnt, 0, 2 * sizeof(int32_t), e->stream));
+    e->wslot = 0;
+    e->rs_prev_n = 0;
+    e->n_rounded = e->n_divided;
+    e->rs_synced = true;
+    return 0;
+}
+
+// rounds of [first, first+n) on the round stream: k_rb_prep (which also gives the round stream's ring the events of its
+// previous piece), k_rounds_cluster and the hand-over launch of k_rounds_batch, on the round stream's meta, ring, Wf and
+// scalars.  `rdone` marks the end.
+template <int NC, bool UNIT>
+int rs_piece(sw_engine *e, int first, int n) {
+    if (rsg_reserve(e, n) < 0) return SW_E_CUDA;
+    const int grid = std::max(e->n_sm / 2, e->n_sm - 16);
+    RbParams R = round_params(e, first, n, grid, 1);
+    int32_t *m = e->d_rbmeta2;
+    const int MP = e->MP;
+    R.ccnt = m; R.cmin = m + MP; R.coff = m + 2 * MP;
+    R.bar = reinterpret_cast<unsigned *>(m + 3 * MP + 8); R.wcnt = m + 3 * MP + 9; R.ctot = m + 3 * MP + 16;
+    R.gchain = e->d_gchain2; R.Wf = e->d_Wf2; R.scal = e->d_rscal;
+    R.epoch = 0x80000000u | ++e->rs_epoch;
+    if (chunk_prep<64>(e, R, e->d_rsg, e->rstream, e->rs_prev_n > 0 ? e->d_gchain2 : nullptr, e->rs_prev_first, e->rs_prev_n) < 0)
+        return SW_E_CUDA;
+    const RcParams Q{R, e->d_rsg, e->d_rccont};
+    R.cont = e->d_rccont;
+    if (round_kernels<NC, UNIT>(e, R, Q, 1, grid, true, e->rstream) < 0) return SW_E_CUDA;
+    CK(cudaEventRecord(e->rdone, e->rstream));
+    e->rs_prev_first = first; e->rs_prev_n = n;
+    e->n_rounded = first + n;
+    return 0;
+}
+
+bool ahead_path(const sw_engine *e, int n) { return e->ahead && !e->wide && e->rc_ok && n >= e->rc_min_n && e->nranks == 1; }
+
+// sw_divide_rounds on the ahead path.  The call's rounds come from the round stream: a piece for whatever part of
+// [first, first+n) none covers yet, then the compute stream waits for it.  The finish kernels publish the call's part of
+// the round stream's state (RbFold).  When the can_see rows reach beyond the call, the next piece, as long as this call,
+// starts on the round stream behind it.  The call counts the launches and the launch number (rb_epoch) the same call
+// makes without the round stream, so the counters do not depend on where pieces begin.
+template <int NC, bool UNIT>
+int divide_ahead(sw_engine *e, int first, int n) {
+    const int end = first + n;
+    if (rs_sync(e) < 0) return SW_E_CUDA;
+    if (e->n_rounded < end && (rs_follow(e) < 0 || rs_piece<NC, UNIT>(e, e->n_rounded, end - e->n_rounded) < 0))
+        return SW_E_CUDA;
+    CK(cudaStreamWaitEvent(e->stream, e->rdone, 0));
+    const RbMeta m = rb_meta(e);
+    RbParams R = chunk_params(e, first, n);
+    R.SM = e->d_SM; R.wcnt = m.wcnt + e->wslot;
+    RbFold F{};
+    F.on = 1; F.Wf = e->d_Wf; F.scal = e->d_scal; F.wnext = m.wcnt + (e->wslot ^ 1); F.rscal = e->d_rscal;
+    counts_at(e, end, F.ctot);
+    e->wslot ^= 1;
+    e->rb_epoch++;
+    e->stats.kernel_launches += 1;                      // (k_rb_prep)
+    count_round_kernels(e, true);
+    if (round_batch_finish<NC>(e, R, F) < 0) return SW_E_CUDA;
+    const int next = std::min(end + n, e->n_rowed);
+    if (e->n_rounded == end && next - end >= e->rc_min_n) {
+        for (auto &a : e->appends) if (a.base < next) CK(cudaStreamWaitEvent(e->rstream, a.done, 0));
+        if (e->scan_ev_set) CK(cudaStreamWaitEvent(e->rstream, e->scan_ev, 0));
+        if (rs_piece<NC, UNIT>(e, end, next - end) < 0) return SW_E_CUDA;
+    }
+    return 0;
 }
 
 size_t rounds_wide_smem(int M) { return (size_t)(2 * M + 16 * M + 1 + 32 + (RW_THREADS / 32) * M + 1) * sizeof(int); }
@@ -575,7 +707,8 @@ template <int NJ>
 int divide_rounds_wide(sw_engine *e, int first, int n) {
     const int M = e->M;
     const RbParams T = chunk_params(e, first, n);       // the grouping and the finish kernel shared with the M <= 64 path
-    if (chunk_prep<SW_MAX_MEMBERS>(e, T, nullptr) < 0) return SW_E_CUDA;
+    if (chunk_prep<SW_MAX_MEMBERS>(e, T, nullptr, e->stream) < 0) return SW_E_CUDA;
+    e->stats.kernel_launches += 1;
     RwParams R{};
     R.M = M; R.first = first; R.n = n; R.Rcap = e->Rcap;
     const int grid = e->n_sm;
@@ -603,7 +736,7 @@ int divide_rounds_wide(sw_engine *e, int first, int n) {
         cudaEventRecord(b, e->stream);
         e->spans.push_back(TimedSpan{a, b, 4});
     }
-    k_rb_finish<<<std::max(1, std::min(2 * e->n_sm, (n + 255) / 256)), 256, 0, e->stream>>>(T);
+    k_rb_finish<<<std::max(1, std::min(2 * e->n_sm, (n + 255) / 256)), 256, 0, e->stream>>>(T, RbFold{});
     k_w_seenmask<NJ><<<std::max(1, std::min(8 * e->n_sm, (n + 7) / 8)), 256, 0, e->stream>>>(M, first, n, e->Rcap, e->d_row, e->d_round, e->d_W, e->d_SMw);
     CK(cudaGetLastError());
     StrongParams Q{};
@@ -781,6 +914,8 @@ int check_views(sw_engine *const *engines, int B, const char *what, bool same_sh
                         same_shape ? "have one member count and one kernel family" : "be");
         if (x->nranks > 1) return fail(e, SW_E_UNSUPPORTED, "%s: view %d is one rank of a multi-GPU engine", what, v);
     }
+    for (int v = 0; v < B; v++)
+        if (rs_drain(engines[v]) < 0) { e->err = engines[v]->err; return SW_E_CUDA; }
     return 0;
 }
 
@@ -920,6 +1055,15 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
                 const cudaError_t er = SW_NCU(e, rc_setup, &ncl);
                 e->rc_ok = er == cudaSuccess && ncl >= 1;
                 if (er != cudaSuccess) (void)cudaGetLastError();
+            }
+            e->ahead = e->rc_ok;
+            if (const char *v = getenv("SW_ROUNDS_AHEAD")) e->ahead = e->ahead && atoi(v) != 0;
+            if (e->ahead) {
+                CK(cudaStreamCreateWithFlags(&e->rstream, cudaStreamNonBlocking));
+                CK(cudaEventCreateWithFlags(&e->rdone, cudaEventDisableTiming));
+                CK(cudaEventCreateWithFlags(&e->rwait, cudaEventDisableTiming));
+                CK(dalloc(&e->d_Wf2, RM)); CK(dalloc(&e->d_gchain2, MP * RB_RING));
+                CK(dalloc(&e->d_rbmeta2, 4 * MP + 64)); CK(dalloc(&e->d_rscal, (size_t)SC_COUNT));
             }
         }
         CK(dalloc(&e->d_round, cap)); CK(dalloc(&e->d_wit, cap)); CK(dalloc(&e->d_famous_ev, cap));
@@ -1168,8 +1312,10 @@ int chunk_views(sw_engine *e, sw_engine *const *engines, int B, const int *first
         cudaEvent_t a = get_event(e);
         cudaEventRecord(a, e->stream);
         if (use_rc) CK(cudaMemcpyAsync(e->d_rcviews + v0, Qv.data() + v0, sizeof(RcParams) * nv, cudaMemcpyHostToDevice, e->stream));
-        if (round_kernels<NC, UNIT>(e, (const RbParams *)e->d_views + v0, (const RcParams *)e->d_rcviews + v0, nv, G, use_rc, a, false) < 0)
+        if (round_kernels<NC, UNIT>(e, (const RbParams *)e->d_views + v0, (const RcParams *)e->d_rcviews + v0, nv, G, use_rc, e->stream) < 0)
             return SW_E_CUDA;
+        count_round_kernels(e, use_rc);
+        round_span(e, a, false);
         CK(cudaEventRecord(e->view_ev, e->stream));
         CK(cudaStreamSynchronize(e->stream));       // (Rv / the event are reused by the next group; the views' finish kernels follow)
         for (int v = v0; v < v0 + nv; v++) {
@@ -1198,11 +1344,14 @@ void sw_destroy(sw_engine *e) {
     if (!e) return;
     cudaSetDevice(e->device);
     if (e->stream) { wait_appends(e, -1); cudaStreamSynchronize(e->stream); }
+    if (e->rstream) cudaStreamSynchronize(e->rstream);
     if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
     fold_spans(e);
     for (auto ev : e->pool) cudaEventDestroy(ev);
     for (auto ev : e->user_ev) if (ev) cudaEventDestroy(ev);
     if (e->scan_ev) cudaEventDestroy(e->scan_ev);
+    if (e->rdone) cudaEventDestroy(e->rdone);
+    if (e->rwait) cudaEventDestroy(e->rwait);
     if (e->view_ev) cudaEventDestroy(e->view_ev);
     if (e->d_views) cudaFree(e->d_views);
     if (e->d_rcviews) cudaFree(e->d_rcviews);
@@ -1222,13 +1371,15 @@ void sw_destroy(sw_engine *e) {
                     e->d_round, e->d_wit, e->d_famous_ev, e->d_W, e->d_S, e->d_famous, e->d_consensus,
                     e->d_done, e->d_rem, e->d_stake, e->d_scal, e->d_lastord, e->d_tx, e->d_idx,
                     e->d_batch_ev, e->d_batch_seg, e->d_perm, e->d_ts, e->d_key, e->d_seg_start, e->d_seg_fw,
-                    e->d_seg_nf, e->d_seg_white, e->d_rounds_in, e->d_plan, e->d_flush, e->d_rsg, e->d_rccont};
+                    e->d_seg_nf, e->d_seg_white, e->d_rounds_in, e->d_plan, e->d_flush, e->d_rsg, e->d_rccont,
+                    e->d_Wf2, e->d_gchain2, e->d_rbmeta2, e->d_rscal};
     for (void *p : ptrs) if (p) cudaFree(p);
     if (e->h_scal) cudaFreeHost(e->h_scal);
     if (e->h_height) cudaFreeHost(e->h_height);
     if (e->h_seq) cudaFreeHost(e->h_seq);
     if (e->h_stale) cudaFreeHost(e->h_stale);
     if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
+    if (e->rstream) cudaStreamDestroy(e->rstream);
     if (e->stream) cudaStreamDestroy(e->stream);
     delete e;
 }
@@ -1236,7 +1387,7 @@ void sw_destroy(sw_engine *e) {
 int sw_reset(sw_engine *e) {
     if (!e) return SW_E_ARG;
     CK(cudaSetDevice(e->device));
-    if (wait_appends(e, -1) < 0) return SW_E_CUDA;
+    if (wait_appends(e, -1) < 0 || rs_drain(e) < 0) return SW_E_CUDA;
     CK(cudaStreamSynchronize(e->stream));
     fold_spans(e);
     e->h_creator.clear();
@@ -1250,7 +1401,7 @@ int sw_reset(sw_engine *e) {
 int sw_rewind(sw_engine *e) {
     if (!e) return SW_E_ARG;
     CK(cudaSetDevice(e->device));
-    if (wait_appends(e, -1) < 0) return SW_E_CUDA;
+    if (wait_appends(e, -1) < 0 || rs_drain(e) < 0) return SW_E_CUDA;
     CK(cudaStreamSynchronize(e->stream));
     fold_spans(e);
     return reset_state(e, true);
@@ -1354,6 +1505,8 @@ int sw_divide_rounds(sw_engine *e, int first, int n) {
     if (first != e->n_divided) return fail(e, SW_E_ARG, "divide_rounds: first=%d but %d events are divided (events must arrive in order)", first, e->n_divided);
     if (first + n > e->n_events) return fail(e, SW_E_KEY, "divide_rounds: events [%d,%d) not appended", first, first + n);
     CK(cudaSetDevice(e->device));
+    const bool ahead = ahead_path(e, n);
+    if (!ahead && rs_drain(e) < 0) return SW_E_CUDA;
     if (stream_path(e, first, n)) {
         if (wait_appends(e, first + n) < 0 || stream_kernel(e, stream_params(e, first, n), 1) < 0) return SW_E_CUDA;
         return stream_divided(e, n);         // (it wrote can_see rows and the carry heads on the compute stream)
@@ -1362,7 +1515,8 @@ int sw_divide_rounds(sw_engine *e, int first, int n) {
     if (rc < 0) return rc;
     {
         Span sp(e, 0);
-        rc = e->wide ? SW_NJ(divide_rounds_wide, e, first, n) : SW_NCU(e, divide_round_batch, e, first, n, sp.s.a);
+        rc = ahead ? SW_NCU(e, divide_ahead, e, first, n)
+           : e->wide ? SW_NJ(divide_rounds_wide, e, first, n) : SW_NCU(e, divide_round_batch, e, first, n, sp.s.a);
         if (rc < 0) return rc;
     }
     divided(e, n);
@@ -1706,6 +1860,7 @@ int sw_debug_counters(sw_engine *e, int64_t *out16, int clear) {
     if (!e || !out16) return SW_E_ARG;
     CK(cudaSetDevice(e->device));
     CK(cudaStreamSynchronize(e->stream));
+    if (e->rstream) CK(cudaStreamSynchronize(e->rstream));     // (the round stream's kernels count there too)
     CK(cudaMemcpy(out16, e->d_dbg, sizeof(long long) * 16, cudaMemcpyDeviceToHost));
     if (clear) CK(cudaMemset(e->d_dbg, 0, sizeof(long long) * 40));
     return SW_OK;

@@ -76,6 +76,10 @@ struct RbChunk {
     int cmin[CM];               // the smallest seq among them (0x7f7f7f7f: none)
     int ctot[CM];               // events of the member up to the end of the chunk
     int coff[CM + 1];           // exclusive prefix sum of ccnt
+    // the rounds run ahead (M <= 64, swirld_b200.cu): the round stream's own ring takes the events of the piece before this
+    // one, [rfirst, rfirst + rn), which ends where this chunk starts (ring NULL: nothing to do)
+    int32_t *ring;
+    int rfirst, rn;
 };
 
 // the chunk's meta arrays, cev, and (rsg != NULL, M <= 64) the seq-space rows of swirld_rcluster.cuh in cev order: one
@@ -104,19 +108,58 @@ __global__ void __launch_bounds__(256) k_rb_prep(RbParams P, const __grid_consta
             }
         }
     }
+    // (ctot - ccnt: the member's events before this chunk, i.e. up to the end of the piece before it)
+    if (K.ring)
+        for (int j = blockIdx.x * blockDim.x + tid; j < K.rn; j += gridDim.x * blockDim.x) {
+            const int h = K.rfirst + j, c = P.creator[h], sq = P.seq[h];
+            if (K.ctot[c] - K.ccnt[c] - sq <= RB_RING) K.ring[c * RB_RING + (sq & (RB_RING - 1))] = h;
+        }
 }
 
 // ---- after the round kernel, one pass over the chunk: each member's most recent RB_RING events for the next chunk, and
 // the reference's witness flags / witnesses table from the finished rounds (swirld.py:221-222, 196-197)
-__global__ void k_rb_finish(RbParams P) {
+//
+// With the rounds run ahead on their own stream (F.on, M <= 64, swirld_b200.cu), the round kernels wrote their own Wf, round
+// top and error slot, and this pass publishes what the call's events add to the engine's: the member counts at the call's
+// end (F.ctot, also the ring's bound), Wf_r[c] = h for every witness h and r in (round of its self-parent, round h] (the
+// entries the round kernel writes: a witness is its member's first event of each round it skips), the round top as the
+// largest round, the capacity error when a round reaches Rcap, and any other error the round stream met.
+struct RbFold {
+    int on;
+    int32_t *Wf, *scal, *wnext;   // the engine's Wf and scalars; the witness count of the next call, zeroed here
+    const int32_t *rscal;         // the round stream's scalars
+    int ctot[64];
+};
+
+__global__ void k_rb_finish(RbParams P, const __grid_constant__ RbFold F) {
+    if (F.on && blockIdx.x == 0) {
+        for (int c = threadIdx.x; c < P.M; c += blockDim.x) P.ctot[c] = F.ctot[c];
+        if (threadIdx.x == 0) {
+            *F.wnext = 0;
+            const int er = F.rscal[SC_ERR];
+            if (er < 0 && er != -5) atomicMin(&F.scal[SC_ERR], er);
+        }
+    }
+    int rmax = -1;
     for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < P.n; j += gridDim.x * blockDim.x) {
         const int h = P.first + j, c = P.creator[h], sq = P.seq[h], pa = P.p0[h], r = P.round[h];
-        if (P.ctot[c] - sq <= RB_RING) P.gchain[c * RB_RING + (sq & (RB_RING - 1))] = h;
-        const bool wit = pa < 0 || r > P.round[pa];
+        if ((F.on ? F.ctot[c] : P.ctot[c]) - sq <= RB_RING) P.gchain[c * RB_RING + (sq & (RB_RING - 1))] = h;
+        const int rp = pa < 0 ? -1 : P.round[pa];
+        const bool wit = pa < 0 || r > rp;
         P.wit[h] = wit ? 1 : 0;
         if (wit && r >= 0 && r < P.Rcap) {
             P.W[(size_t)r * P.M + c] = h;
             P.wlist[atomicAdd(P.wcnt, 1)] = h;                // k_strong runs over the witnesses only
+        }
+        if (F.on && wit)
+            for (int q = rp + 1; q <= r && q < P.Rcap; q++) F.Wf[(size_t)q * P.M + c] = h;
+        rmax = max(rmax, r);
+    }
+    if (F.on) {
+        for (int o = 16; o > 0; o >>= 1) rmax = max(rmax, __shfl_xor_sync(0xffffffffu, rmax, o));
+        if ((threadIdx.x & 31) == 0 && rmax >= 0) {
+            atomicMax(&F.scal[SC_MAX_ROUND], rmax);
+            if (rmax >= P.Rcap) atomicMin(&F.scal[SC_ERR], -5);                   // (the round table is exhausted)
         }
     }
 }
