@@ -68,9 +68,10 @@ struct sw_engine {
     int32_t *d_Wf = nullptr, *d_cev = nullptr, *d_rbmeta = nullptr, *d_rbtot = nullptr, *d_gchain = nullptr;   // round-batch state
     ulonglong2 *d_sc = nullptr;
     uint8_t *d_res = nullptr;
-    // cluster round kernel (swirld_rcluster.cuh): seq-space rows of the current chunk, hand-over state
-    int32_t *d_rsg = nullptr, *d_rccont = nullptr;
-    size_t rsg_cap = 0;           // events d_rsg holds
+    // cluster round kernel (swirld_rcluster.cuh): seq-space rows of the current chunk (the round stream's pieces use both
+    // buffers in turn, the compute stream the first), hand-over state
+    int32_t *d_rsg[2] = {nullptr, nullptr}, *d_rccont = nullptr;
+    size_t rsg_cap[2] = {0, 0};   // events d_rsg[b] holds
     bool rc_ok = false;           // a 16-CTA cluster with its shared memory can be resident on this device
     int rc_min_n = 2048;          // shorter chunks go to the grid-wide kernel directly
     // The rounds run ahead (SW_ROUNDS_AHEAD, M <= 64, calls that go to the cluster kernel): a call whose can_see rows reach
@@ -78,15 +79,24 @@ struct sw_engine {
     // finish and fame kernels and the host's turn-around.  Round numbers are a function of the graph alone, so the piece
     // writes the final rounds of its events; what the engine shows a caller (Wf, the ring, the counts, the round top,
     // errors) stays the compute stream's, and the round stream keeps its own copies: `d_Wf2`, `d_gchain2`, `d_rbmeta2`
-    // (chunk meta, counts, barrier, witness count) and `d_rscal` (round top, error slot).  One piece at most is in flight:
-    // [n_divided, n_rounded), ended by `rdone`.
+    // (two chunk meta blocks: counts, offsets, barrier, witness count) and `d_rscal` (round top, error slot).  The pieces
+    // cover [n_divided, n_rounded); a piece may span several calls, and two stay queued beyond the last call (`rs_pieces`,
+    // each ended by its own event; `rdone`: the end of the last one -- once a call has waited for it, the event also sits
+    // in `rs_free`, which is harmless: it is recorded again only for a newer piece, which then is the last one).  A
+    // piece's k_rb_prep runs on `pstream`, beside the cluster kernel of the piece before it, into the meta block and
+    // d_rsg buffer that piece does not use (`rs_buf` alternates); it waits for the piece before that one to have finished
+    // with them (`rs_bufdone`), and the piece's cluster kernel waits for it (`rs_prepped`).
     bool ahead = false;
-    cudaStream_t rstream = nullptr;
+    cudaStream_t rstream = nullptr, pstream = nullptr;
     cudaEvent_t rdone = nullptr, rwait = nullptr;
+    cudaEvent_t rs_prepped[2] = {nullptr, nullptr}, rs_bufdone[2] = {nullptr, nullptr};
+    int rs_buf = 0;               // the buffers of the next piece
+    struct RsPiece { int end; cudaEvent_t done; };
+    std::vector<RsPiece> rs_pieces;                  // the pieces that end beyond the last call, in order
+    std::vector<cudaEvent_t> rs_free;                // their events once a call has waited for them
     int32_t *d_Wf2 = nullptr, *d_gchain2 = nullptr, *d_rbmeta2 = nullptr, *d_rscal = nullptr;
     bool rs_synced = false;       // the round stream's copies hold everything below n_rounded
     int n_rounded = 0;            // events rounded so far (the round stream's piece ends here)
-    int rs_prev_first = 0, rs_prev_n = 0;   // the round stream's last piece, whose events its ring has not taken yet
     unsigned rs_epoch = 0;        // launches on the round stream (mask-cache keys of their own: the top bit set)
     int wslot = 0;                // which of the two witness counts of d_rbmeta the next call uses
     RcParams *d_rcviews = nullptr;
@@ -218,6 +228,7 @@ void fold_spans(sw_engine *e) {
             else if (s.cat == 2) e->stats.ms_find_order += ms;
             else if (s.cat == 3) { e->stats.ms_can_see += ms; e->stats.ms_divide_rounds += ms; }
             else if (s.cat == 4) e->stats.ms_rounds_kernel += ms;
+            else if (s.cat == 5) e->stats.ms_can_see += ms;       // (a scan inside a divide_rounds span)
         }
         if (!s.shared_a) e->pool.push_back(s.a);
         e->pool.push_back(s.b);
@@ -287,11 +298,31 @@ int reset_state(sw_engine *e, bool keep_events = false) {
     return 0;
 }
 
+// blocks of the scan of [first, first+n) (n > 24), of *B events each
+int cs_blocks(const sw_engine *e, int first, int n, int *B_out) {
+    // block length: >= 16 (32 above 64 members) events per member and block, so that nearly every member's last event of a
+    // block sees every block-start head (then the finality check passes; the rest goes through the waves)
+    int B = std::max(e->cs_min_B, std::min((e->M <= 64 ? 16 : 32) * e->M, 1 << 15));      // (above 64 members seeing every head takes more events per member)
+    B = (B + 3) & ~3;
+    const int first_al = first & ~3;
+    int nb = (first + n <= first_al + B) ? 1 : 1 + (first + n - (first_al + B) + B - 1) / B;
+    if (nb > 1 && first + n - (first_al + (nb - 1) * B) < 3 * B / 4) nb--;     // a short tail joins the block before it
+    *B_out = B;
+    return nb;
+}
+
+// the launches of the scan of [first, first+n)
+int cs_launches(const sw_engine *e, int first, int n) {
+    int B;
+    return n <= 0 ? 0 : n <= 24 ? 1 : cs_blocks(e, first, n, &B) > 1 ? 9 : 4;
+}
+
 // can_see rows of the appended events [n_rowed, upto): the column-tiled blocked scan of swirld_cansee.cuh.
 // `st`: the compute stream (lazily, from sw_divide_rounds) or the copy stream (eagerly, from sw_append: the
 // scan of a new chunk then runs beside the round kernel of the previous one).  The two never overlap: a scan
 // on one stream first waits for the last scan issued on the other (they share the scratch and the carry heads).
-int cansee_scan(sw_engine *e, cudaStream_t st, int upto) {
+// `cat`: the span category of its time (fold_spans).
+int cansee_scan(sw_engine *e, cudaStream_t st, int upto, int cat = 3) {
     const int first = e->n_rowed, n = upto - e->n_rowed;
     if (n <= 0) return 0;
     const int M = e->M;
@@ -305,20 +336,16 @@ int cansee_scan(sw_engine *e, cudaStream_t st, int upto) {
         cudaEventRecord(a, st);
         k_cs_small<<<1, std::min(1024, (M + 31) / 32 * 32), 0, st>>>(C);
         cudaEventRecord(b, st);
-        e->spans.push_back(TimedSpan{a, b, 3});
+        e->spans.push_back(TimedSpan{a, b, cat});
         CK(cudaGetLastError());
         e->stats.kernel_launches += 1;
         e->n_rowed = upto;
         return 0;
     }
-    // block length: >= 16 (32 above 64 members) events per member and block, so that nearly every member's last event of a
-    // block sees every block-start head (then the finality check passes; the rest goes through the waves)
-    int B = std::max(e->cs_min_B, std::min((M <= 64 ? 16 : 32) * M, 1 << 15));      // (above 64 members seeing every head takes more events per member)
-    B = (B + 3) & ~3;
+    int B;
+    C.nb = cs_blocks(e, first, n, &B);
     C.B = B;
     C.first_al = first & ~3;
-    C.nb = (first + n <= C.first_al + B) ? 1 : 1 + (first + n - (C.first_al + B) + B - 1) / B;
-    if (C.nb > 1 && first + n - (C.first_al + (C.nb - 1) * B) < 3 * B / 4) C.nb--;     // a short tail joins the block before it
     // columns per tile: 32 (one warp = one 128-byte row segment) unless the per-member cache val[M][CT] then limits a
     // SM to so few CTAs that narrower tiles finish in fewer waves (M = 1024: 128 KB per CTA at CT = 32)
     const bool has_stale = e->h_stale_cum[first + n] - e->h_stale_cum[first] > 0;
@@ -387,7 +414,7 @@ int cansee_scan(sw_engine *e, cudaStream_t st, int upto) {
     if (shard) k_cs_carry<<<(M + 255) / 256, 256, 0, st>>>(C);
     if (xbarrier() < 0) return SW_E_CUDA;                  // the whole table is in every rank's memory
     cudaEventRecord(b, st);
-    e->spans.push_back(TimedSpan{a, b, 3});
+    e->spans.push_back(TimedSpan{a, b, cat});
     CK(cudaGetLastError());
     e->stats.kernel_launches += C.nb > 1 ? 9 : 4;
     e->n_rowed = upto;
@@ -463,9 +490,8 @@ RbParams chunk_params(const sw_engine *e, int first, int n) {
 // the chunk's events grouped by creator (k_rb_prep) from the per-member counts of the host mirror: [first, first+n)
 // holds seqs [lo[c], hi[c]) of member c.  `rsg` (M <= 64): also the seq-space rows of the cluster round kernel.
 template <int CM>
-int chunk_prep(sw_engine *e, const RbParams &R, int32_t *rsg, cudaStream_t st, int32_t *ring = nullptr, int rfirst = 0, int rn = 0) {
+int chunk_prep(sw_engine *e, const RbParams &R, int32_t *rsg, cudaStream_t st) {
     RbChunk<CM> K;
-    K.ring = ring; K.rfirst = rfirst; K.rn = rn;
     int32_t lo[CM];
     counts_at(e, R.first, lo);
     counts_at(e, R.first + R.n, K.ctot);
@@ -492,17 +518,18 @@ RbParams round_params(const sw_engine *e, int first, int n, int grid, int min_L)
     return R;
 }
 
-// the cluster kernel's seq-space rows for n events (both streams use them: a new buffer waits for both)
-int rsg_reserve(sw_engine *e, int n) {
-    if ((size_t)n <= e->rsg_cap) return 0;
-    if (e->d_rsg) {
+// buffer b of the cluster kernel's seq-space rows, for n events (every stream uses them: a new buffer waits for all)
+int rsg_reserve(sw_engine *e, int n, int b = 0) {
+    if ((size_t)n <= e->rsg_cap[b]) return 0;
+    if (e->d_rsg[b]) {
         CK(cudaStreamSynchronize(e->stream));
         if (e->rstream) CK(cudaStreamSynchronize(e->rstream));
-        CK(cudaFree(e->d_rsg)); e->d_rsg = nullptr; e->rsg_cap = 0;
+        if (e->pstream) CK(cudaStreamSynchronize(e->pstream));
+        CK(cudaFree(e->d_rsg[b])); e->d_rsg[b] = nullptr; e->rsg_cap[b] = 0;
     }
     const size_t want = std::min<size_t>((size_t)e->cap, std::max<size_t>((size_t)n, 1 << 16));
-    CK(dalloc(&e->d_rsg, want * 64));
-    e->rsg_cap = want;
+    CK(dalloc(&e->d_rsg[b], want * 64));
+    e->rsg_cap[b] = want;
     return 0;
 }
 
@@ -513,10 +540,10 @@ int round_batch_prep(sw_engine *e, int first, int n, int grid, int min_L, bool r
     R = round_params(e, first, n, grid, min_L);
     R.epoch = ++e->rb_epoch;
     if (rc && rsg_reserve(e, n) < 0) return SW_E_CUDA;
-    if (chunk_prep<64>(e, R, rc ? e->d_rsg : nullptr, e->stream) < 0) return SW_E_CUDA;
+    if (chunk_prep<64>(e, R, rc ? e->d_rsg[0] : nullptr, e->stream) < 0) return SW_E_CUDA;
     e->stats.kernel_launches += 1;
     if (rc) {
-        Q = RcParams{R, e->d_rsg, e->d_rccont};
+        Q = RcParams{R, e->d_rsg[0], e->d_rccont};
         R.cont = e->d_rccont;
     }
     return 0;
@@ -612,17 +639,21 @@ int divide_round_batch(sw_engine *e, int first, int n, cudaEvent_t start) {
 // ---- the rounds run ahead (sw_engine::ahead)
 // Everything but the ahead path writes the engine's own Wf, ring and counts: before it runs, the compute stream waits for
 // the round stream's piece, which is given up (its rounds are computed again), and so are the round stream's copies.
+// (The round stream runs its pieces in order: waiting for the end of the last one waits for all of them.)
 int rs_drain(sw_engine *e) {
-    if (e->rs_synced) CK(cudaStreamWaitEvent(e->stream, e->rdone, 0));
+    if (e->rs_synced && e->rdone) CK(cudaStreamWaitEvent(e->stream, e->rdone, 0));
     e->rs_synced = false;
     e->n_rounded = e->n_divided;
+    for (auto &p : e->rs_pieces) e->rs_free.push_back(p.done);
+    e->rs_pieces.clear();
     return 0;
 }
 
-// the round stream goes on after what the compute stream has been given so far
+// the round stream and its prep stream go on after what the compute stream has been given so far
 int rs_follow(sw_engine *e) {
     CK(cudaEventRecord(e->rwait, e->stream));
     CK(cudaStreamWaitEvent(e->rstream, e->rwait, 0));
+    CK(cudaStreamWaitEvent(e->pstream, e->rwait, 0));
     return 0;
 }
 
@@ -635,51 +666,101 @@ int rs_sync(sw_engine *e) {
     CK(cudaMemcpyAsync(e->d_rscal, e->d_scal, sizeof(int32_t) * SC_COUNT, cudaMemcpyDeviceToDevice, e->rstream));
     CK(cudaMemsetAsync(rb_meta(e).wcnt, 0, 2 * sizeof(int32_t), e->stream));
     e->wslot = 0;
-    e->rs_prev_n = 0;
     e->n_rounded = e->n_divided;
     e->rs_synced = true;
     return 0;
 }
 
-// rounds of [first, first+n) on the round stream: k_rb_prep (which also gives the round stream's ring the events of its
-// previous piece), k_rounds_cluster and the hand-over launch of k_rounds_batch, on the round stream's meta, ring, Wf and
-// scalars.  `rdone` marks the end.
+// the size of one of the round stream's two meta blocks in d_rbmeta2
+size_t rs_meta_ints(const sw_engine *e) { return 4 * (size_t)e->MP + 64; }
+
+// Rounds of [first, first+n) on the round stream's meta, ring, Wf and scalars.  The caller has made `pstream` wait for the
+// piece's rows.  k_rb_prep runs there, into the buffers the piece before this one does not use, once the piece before
+// that one has finished with them; then on the round stream k_rounds_cluster and the hand-over launch of k_rounds_batch,
+// after the prep.  An event of its own marks the end (rs_pieces), and `rdone` is it too.  Last, the round stream's ring
+// takes the piece's events (k_rb_ring): the only readers of the ring slots it overwrites are this piece's cluster kernel
+// and hand-over, which are before it on the same stream, and the next piece's kernels, which are after it; the preps
+// never read the ring.  So no reader sees a slot overwritten too early or too late.
 template <int NC, bool UNIT>
 int rs_piece(sw_engine *e, int first, int n) {
-    if (rsg_reserve(e, n) < 0) return SW_E_CUDA;
+    const int b = e->rs_buf;
+    e->rs_buf ^= 1;
+    if (rsg_reserve(e, n, b) < 0) return SW_E_CUDA;
     const int grid = std::max(e->n_sm / 2, e->n_sm - 16);
     RbParams R = round_params(e, first, n, grid, 1);
-    int32_t *m = e->d_rbmeta2;
+    int32_t *m = e->d_rbmeta2 + b * rs_meta_ints(e);
     const int MP = e->MP;
     R.ccnt = m; R.cmin = m + MP; R.coff = m + 2 * MP;
     R.bar = reinterpret_cast<unsigned *>(m + 3 * MP + 8); R.wcnt = m + 3 * MP + 9; R.ctot = m + 3 * MP + 16;
     R.gchain = e->d_gchain2; R.Wf = e->d_Wf2; R.scal = e->d_rscal;
     R.epoch = 0x80000000u | ++e->rs_epoch;
-    if (chunk_prep<64>(e, R, e->d_rsg, e->rstream, e->rs_prev_n > 0 ? e->d_gchain2 : nullptr, e->rs_prev_first, e->rs_prev_n) < 0)
-        return SW_E_CUDA;
-    const RcParams Q{R, e->d_rsg, e->d_rccont};
+    CK(cudaStreamWaitEvent(e->pstream, e->rs_bufdone[b], 0));
+    if (chunk_prep<64>(e, R, e->d_rsg[b], e->pstream) < 0) return SW_E_CUDA;
+    CK(cudaEventRecord(e->rs_prepped[b], e->pstream));
+    CK(cudaStreamWaitEvent(e->rstream, e->rs_prepped[b], 0));
+    const RcParams Q{R, e->d_rsg[b], e->d_rccont};
     R.cont = e->d_rccont;
     if (round_kernels<NC, UNIT>(e, R, Q, 1, grid, true, e->rstream) < 0) return SW_E_CUDA;
-    CK(cudaEventRecord(e->rdone, e->rstream));
-    e->rs_prev_first = first; e->rs_prev_n = n;
+    CK(cudaEventRecord(e->rs_bufdone[b], e->rstream));
+    cudaEvent_t done = nullptr;
+    if (!e->rs_free.empty()) { done = e->rs_free.back(); e->rs_free.pop_back(); }
+    else CK(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
+    e->rs_pieces.push_back({first + n, done});
+    CK(cudaEventRecord(done, e->rstream));
+    e->rdone = done;
+    RbRing G;
+    G.ring = e->d_gchain2; G.creator = e->d_creator; G.seq = e->d_seq; G.rfirst = first; G.rn = n;
+    counts_at(e, first + n, G.ctot);
+    k_rb_ring<<<std::max(1, std::min(2 * e->n_sm, (n + 255) / 256)), 256, 0, e->rstream>>>(G);
+    CK(cudaGetLastError());
     e->n_rounded = first + n;
     return 0;
 }
 
 bool ahead_path(const sw_engine *e, int n) { return e->ahead && !e->wide && e->rc_ok && n >= e->rc_min_n && e->nranks == 1; }
 
+// A piece queued ahead covers up to RS_CALLS call lengths of rows, and half the rows left at most, so that near the end
+// of the rows the pieces shrink back to one call: every call after the last piece would wait for all of that piece's
+// rounds before its finish and fame kernels could run.
+constexpr int RS_CALLS = 8;
+
+int rows_written(sw_engine *e);
+
+int rs_ahead_len(const sw_engine *e, int n) {
+    const int avail = e->n_rowed - e->n_rounded;
+    return std::min(avail, n * std::max(1, std::min(RS_CALLS, avail / n / 2)));
+}
+
 // sw_divide_rounds on the ahead path.  The call's rounds come from the round stream: a piece for whatever part of
-// [first, first+n) none covers yet, then the compute stream waits for it.  The finish kernels publish the call's part of
-// the round stream's state (RbFold).  When the can_see rows reach beyond the call, the next piece, as long as this call,
-// starts on the round stream behind it.  The call counts the launches and the launch number (rb_epoch) the same call
-// makes without the round stream, so the counters do not depend on where pieces begin.
+// [first, first+n) none covers yet, then the compute stream waits for the piece that holds the call's end.  The finish
+// kernels publish the call's part of the round stream's state (RbFold).  While the can_see rows reach beyond the pieces,
+// more start on the round stream behind them, until two end beyond this call, so that the round stream is never idle
+// waiting for a call.  The call counts the launches and the launch number (rb_epoch) the same call makes without the
+// round stream, so the counters do not depend on where pieces begin.  `scan_from` >= 0: the call scanned only its own
+// rows, from there (sw_divide_rounds); the rest are scanned here, beside the call's piece, and charged as one scan.
 template <int NC, bool UNIT>
-int divide_ahead(sw_engine *e, int first, int n) {
+int divide_ahead(sw_engine *e, int first, int n, int scan_from) {
     const int end = first + n;
     if (rs_sync(e) < 0) return SW_E_CUDA;
-    if (e->n_rounded < end && (rs_follow(e) < 0 || rs_piece<NC, UNIT>(e, e->n_rounded, end - e->n_rounded) < 0))
+    const bool cover = e->n_rounded < end;
+    if (cover && (rs_follow(e) < 0 || rs_piece<NC, UNIT>(e, e->n_rounded, end - e->n_rounded) < 0))
         return SW_E_CUDA;
-    CK(cudaStreamWaitEvent(e->stream, e->rdone, 0));
+    if (scan_from >= 0) {
+        // (after the piece's k_rb_prep: its cluster kernel is then the first to claim the SMs the prep frees, and the
+        //  scan takes what the cluster leaves)
+        if (cover) CK(cudaStreamWaitEvent(e->stream, e->rs_prepped[e->rs_buf ^ 1], 0));
+        const i64 kl = e->stats.kernel_launches;
+        if (cansee_scan(e, e->stream, e->n_events, 5) < 0 || rows_written(e) < 0) return SW_E_CUDA;
+        e->stats.kernel_launches = kl + cs_launches(e, scan_from, e->n_events - scan_from) - cs_launches(e, scan_from, end - scan_from);
+    }
+    // (the pieces are contiguous from n_divided and the last ends at n_rounded >= end: one of them holds the call's end)
+    size_t k = 0;
+    while (k + 1 < e->rs_pieces.size() && e->rs_pieces[k].end < end) k++;
+    if (e->rs_pieces.empty() || e->rs_pieces[k].end < end) return fail(e, SW_E_CUDA, "divide_ahead: no piece holds the call's end");
+    CK(cudaStreamWaitEvent(e->stream, e->rs_pieces[k].done, 0));
+    if (e->rs_pieces[k].end == end) k++;
+    for (size_t i = 0; i < k; i++) e->rs_free.push_back(e->rs_pieces[i].done);
+    e->rs_pieces.erase(e->rs_pieces.begin(), e->rs_pieces.begin() + k);
     const RbMeta m = rb_meta(e);
     RbParams R = chunk_params(e, first, n);
     R.SM = e->d_SM; R.wcnt = m.wcnt + e->wslot;
@@ -691,11 +772,12 @@ int divide_ahead(sw_engine *e, int first, int n) {
     e->stats.kernel_launches += 1;                      // (k_rb_prep)
     count_round_kernels(e, true);
     if (round_batch_finish<NC>(e, R, F) < 0) return SW_E_CUDA;
-    const int next = std::min(end + n, e->n_rowed);
-    if (e->n_rounded == end && next - end >= e->rc_min_n) {
-        for (auto &a : e->appends) if (a.base < next) CK(cudaStreamWaitEvent(e->rstream, a.done, 0));
-        if (e->scan_ev_set) CK(cudaStreamWaitEvent(e->rstream, e->scan_ev, 0));
-        if (rs_piece<NC, UNIT>(e, end, next - end) < 0) return SW_E_CUDA;
+    while (e->rs_pieces.size() < 2) {
+        const int len = rs_ahead_len(e, n), next = e->n_rounded + len;
+        if (len < e->rc_min_n) break;
+        for (auto &a : e->appends) if (a.base < next) CK(cudaStreamWaitEvent(e->pstream, a.done, 0));
+        if (e->scan_ev_set) CK(cudaStreamWaitEvent(e->pstream, e->scan_ev, 0));
+        if (rs_piece<NC, UNIT>(e, e->n_rounded, len) < 0) return SW_E_CUDA;
     }
     return 0;
 }
@@ -1060,10 +1142,14 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
             if (const char *v = getenv("SW_ROUNDS_AHEAD")) e->ahead = e->ahead && atoi(v) != 0;
             if (e->ahead) {
                 CK(cudaStreamCreateWithFlags(&e->rstream, cudaStreamNonBlocking));
-                CK(cudaEventCreateWithFlags(&e->rdone, cudaEventDisableTiming));
+                CK(cudaStreamCreateWithFlags(&e->pstream, cudaStreamNonBlocking));
                 CK(cudaEventCreateWithFlags(&e->rwait, cudaEventDisableTiming));
+                for (int b = 0; b < 2; b++) {
+                    CK(cudaEventCreateWithFlags(&e->rs_prepped[b], cudaEventDisableTiming));
+                    CK(cudaEventCreateWithFlags(&e->rs_bufdone[b], cudaEventDisableTiming));
+                }
                 CK(dalloc(&e->d_Wf2, RM)); CK(dalloc(&e->d_gchain2, MP * RB_RING));
-                CK(dalloc(&e->d_rbmeta2, 4 * MP + 64)); CK(dalloc(&e->d_rscal, (size_t)SC_COUNT));
+                CK(dalloc(&e->d_rbmeta2, 2 * rs_meta_ints(e))); CK(dalloc(&e->d_rscal, (size_t)SC_COUNT));
             }
         }
         CK(dalloc(&e->d_round, cap)); CK(dalloc(&e->d_wit, cap)); CK(dalloc(&e->d_famous_ev, cap));
@@ -1256,10 +1342,11 @@ int rows_written(sw_engine *e) {
 // Before a chunk [first, first+n) on the compute stream: rows behind (small appends, or after sw_rewind) are scanned
 // there, for everything appended so far and after the copies of EVERY appended batch (the scan reads the columns of
 // all of them); else the stream waits for the copies of the batches the chunk touches.
-int rows_ready(sw_engine *e, int first, int n) {
+// `upto` < n_events: scan only so far (the ahead path scans the rest beside the call's piece).
+int rows_ready(sw_engine *e, int first, int n, int upto = -1) {
     if (first + n <= e->n_rowed) return wait_appends(e, first + n);
     if (wait_appends(e, -1) < 0) return SW_E_CUDA;
-    const int rc = cansee_scan(e, e->stream, e->n_events);
+    const int rc = cansee_scan(e, e->stream, upto < 0 ? e->n_events : upto);
     return rc < 0 ? rc : rows_written(e);
 }
 
@@ -1345,13 +1432,17 @@ void sw_destroy(sw_engine *e) {
     cudaSetDevice(e->device);
     if (e->stream) { wait_appends(e, -1); cudaStreamSynchronize(e->stream); }
     if (e->rstream) cudaStreamSynchronize(e->rstream);
+    if (e->pstream) cudaStreamSynchronize(e->pstream);
     if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
     fold_spans(e);
     for (auto ev : e->pool) cudaEventDestroy(ev);
     for (auto ev : e->user_ev) if (ev) cudaEventDestroy(ev);
     if (e->scan_ev) cudaEventDestroy(e->scan_ev);
-    if (e->rdone) cudaEventDestroy(e->rdone);
+    for (auto &p : e->rs_pieces) cudaEventDestroy(p.done);
+    for (auto ev : e->rs_free) cudaEventDestroy(ev);
     if (e->rwait) cudaEventDestroy(e->rwait);
+    for (auto ev : e->rs_prepped) if (ev) cudaEventDestroy(ev);
+    for (auto ev : e->rs_bufdone) if (ev) cudaEventDestroy(ev);
     if (e->view_ev) cudaEventDestroy(e->view_ev);
     if (e->d_views) cudaFree(e->d_views);
     if (e->d_rcviews) cudaFree(e->d_rcviews);
@@ -1371,7 +1462,7 @@ void sw_destroy(sw_engine *e) {
                     e->d_round, e->d_wit, e->d_famous_ev, e->d_W, e->d_S, e->d_famous, e->d_consensus,
                     e->d_done, e->d_rem, e->d_stake, e->d_scal, e->d_lastord, e->d_tx, e->d_idx,
                     e->d_batch_ev, e->d_batch_seg, e->d_perm, e->d_ts, e->d_key, e->d_seg_start, e->d_seg_fw,
-                    e->d_seg_nf, e->d_seg_white, e->d_rounds_in, e->d_plan, e->d_flush, e->d_rsg, e->d_rccont,
+                    e->d_seg_nf, e->d_seg_white, e->d_rounds_in, e->d_plan, e->d_flush, e->d_rsg[0], e->d_rsg[1], e->d_rccont,
                     e->d_Wf2, e->d_gchain2, e->d_rbmeta2, e->d_rscal};
     for (void *p : ptrs) if (p) cudaFree(p);
     if (e->h_scal) cudaFreeHost(e->h_scal);
@@ -1380,6 +1471,7 @@ void sw_destroy(sw_engine *e) {
     if (e->h_stale) cudaFreeHost(e->h_stale);
     if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
     if (e->rstream) cudaStreamDestroy(e->rstream);
+    if (e->pstream) cudaStreamDestroy(e->pstream);
     if (e->stream) cudaStreamDestroy(e->stream);
     delete e;
 }
@@ -1511,11 +1603,14 @@ int sw_divide_rounds(sw_engine *e, int first, int n) {
         if (wait_appends(e, first + n) < 0 || stream_kernel(e, stream_params(e, first, n), 1) < 0) return SW_E_CUDA;
         return stream_divided(e, n);         // (it wrote can_see rows and the carry heads on the compute stream)
     }
-    int rc = rows_ready(e, first, n);
+    // rows behind by more than one more call (the first call after sw_rewind in the resident pattern): the ahead path
+    // scans the call's own rows first, so that its piece starts before the rest are scanned
+    const int scan_from = ahead && first + n > e->n_rowed && e->n_events - (first + n) >= n ? e->n_rowed : -1;
+    int rc = rows_ready(e, first, n, scan_from >= 0 ? first + n : -1);
     if (rc < 0) return rc;
     {
         Span sp(e, 0);
-        rc = ahead ? SW_NCU(e, divide_ahead, e, first, n)
+        rc = ahead ? SW_NCU(e, divide_ahead, e, first, n, scan_from)
            : e->wide ? SW_NJ(divide_rounds_wide, e, first, n) : SW_NCU(e, divide_round_batch, e, first, n, sp.s.a);
         if (rc < 0) return rc;
     }

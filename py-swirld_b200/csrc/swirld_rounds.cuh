@@ -76,10 +76,6 @@ struct RbChunk {
     int cmin[CM];               // the smallest seq among them (0x7f7f7f7f: none)
     int ctot[CM];               // events of the member up to the end of the chunk
     int coff[CM + 1];           // exclusive prefix sum of ccnt
-    // the rounds run ahead (M <= 64, swirld_b200.cu): the round stream's own ring takes the events of the piece before this
-    // one, [rfirst, rfirst + rn), which ends where this chunk starts (ring NULL: nothing to do)
-    int32_t *ring;
-    int rfirst, rn;
 };
 
 // the chunk's meta arrays, cev, and (rsg != NULL, M <= 64) the seq-space rows of swirld_rcluster.cuh in cev order: one
@@ -108,12 +104,22 @@ __global__ void __launch_bounds__(256) k_rb_prep(RbParams P, const __grid_consta
             }
         }
     }
-    // (ctot - ccnt: the member's events before this chunk, i.e. up to the end of the piece before it)
-    if (K.ring)
-        for (int j = blockIdx.x * blockDim.x + tid; j < K.rn; j += gridDim.x * blockDim.x) {
-            const int h = K.rfirst + j, c = P.creator[h], sq = P.seq[h];
-            if (K.ctot[c] - K.ccnt[c] - sq <= RB_RING) K.ring[c * RB_RING + (sq & (RB_RING - 1))] = h;
-        }
+}
+
+// The rounds run ahead (M <= 64, swirld_b200.cu): after a piece of the round stream, its own ring takes the piece's events
+// [rfirst, rfirst + rn), each member's last RB_RING of them (ctot: the members' events up to the piece's end).
+struct RbRing {
+    int32_t *ring;
+    const int32_t *creator, *seq;
+    int rfirst, rn;
+    int ctot[64];
+};
+
+__global__ void __launch_bounds__(256) k_rb_ring(const __grid_constant__ RbRing G) {
+    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < G.rn; j += gridDim.x * blockDim.x) {
+        const int h = G.rfirst + j, c = G.creator[h], sq = G.seq[h];
+        if (G.ctot[c] - sq <= RB_RING) G.ring[c * RB_RING + (sq & (RB_RING - 1))] = h;
+    }
 }
 
 // ---- after the round kernel, one pass over the chunk: each member's most recent RB_RING events for the next chunk, and
