@@ -61,7 +61,8 @@ typedef struct sw_stats_t {
 
 /* Node.__init__ state (swirld.py:38-72): M members, integer stake per member
  * (NULL = unit stake as in both reference drivers, swirld.py:334 / viz.py:36),
- * coin period C (swirld.py:17), room for capacity_events events. */
+ * coin period C (swirld.py:17), room for capacity_events events.  SW_E_ARG for a
+ * negative stake or a total above (2^63 - 1) / 3, whose triple overflows int64. */
 int sw_create(int M, int capacity_events, const int64_t *stake, int coin_period,
               int device, sw_engine **out);
 void sw_destroy(sw_engine *e);

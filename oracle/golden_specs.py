@@ -49,6 +49,21 @@ SPECS = {
     "g2_m5_n900_s12_k13": ("adversarial", dict(M=5, N=900, seed=12, p_cross=0.05, p_stale=0.3), 13, None),
     "g1_m16_n3000_s13_k250": ("gossip", dict(M=16, N=3000, seed=13), 250, None),
     "g2_m16_n3000_s13_k250": ("adversarial", dict(M=16, N=3000, seed=13, p_cross=0.05, p_stale=0.3), 250, None),
+    # other value columns (traces.restamped): fractional, negative, constant, overflowing and subnormal times, and
+    # signatures that share their first P bytes, so ties of the order are decided at byte P or later
+    "rs_g1_m4_n1500_s21_k1_wall_p56": ("restamped", dict(base="gossip", times="wall", sigs="prefix56", seed=21, M=4, N=1500), 1, None),
+    "rs_g1_m5_n1500_s22_k13_const_p32": ("restamped", dict(base="gossip", times="const", sigs="prefix32", seed=22, M=5, N=1500), 13, None),
+    "rs_g2_m16_n4000_s23_k250_neg_p16": ("restamped", dict(base="adversarial", times="neg", sigs="prefix16", seed=23, M=16, N=4000,
+                                                           p_cross=0.05, p_stale=0.3), 250, None),
+    "rs_g1_m33_n6000_s25_k640_huge_p8": ("restamped", dict(base="gossip", times="huge", sigs="prefix8", seed=25, M=33, N=6000), 640, None),
+    "rs_g1_m64_n12000_s24_k2048_tiny_p60c": ("restamped", dict(base="gossip", times="tiny", sigs="prefix60_coin", seed=24, M=64,
+                                                               N=12000), 2048, None),
+    "rs_g1_m96_n12000_s28_k3000_wall_p60": ("restamped", dict(base="gossip", times="wall", sigs="prefix60", seed=28, M=96, N=12000), 3000, None),
+    "rs_g1_m80_n8000_s27_k999_shuffle_p16": ("restamped", dict(base="gossip", times="shuffle", sigs="prefix16", seed=27, M=80, N=8000), 999,
+                                             [1 + (i % 3 == 0) for i in range(80)]),
+    # the largest stake total B = (2**63 - 1) // 3 whose triple fits in int64: a member count never exceeds 2/3 of it
+    # (quirk Q3), so every event stays in round 0 and nothing is ordered
+    "g1_m4_n600_s31_k7_bigstake": ("gossip", dict(M=4, N=600, seed=31), 7, [2 ** 61, (2 ** 63 - 1) // 3 - 2 ** 61 - 1, 1, 0]),
 }
 
 # the arrival traces and call schedules of two nodes of one gossip simulation over tests/host_sim.py (4 nodes,

@@ -1084,7 +1084,10 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
         e->h_stake[c] = stake ? stake[c] : 1;
         if (e->h_stake[c] < 0) { delete e; return fail(nullptr, SW_E_ARG, "negative stake"); }
         if (e->h_stake[c] != 1) e->unit = false;
-        e->tot += e->h_stake[c];
+        // the fame and round tests compare 3 * (a sum of stakes) with 2 * tot in int64: refuse totals whose triple overflows
+        if (__builtin_add_overflow(e->tot, e->h_stake[c], &e->tot) || e->tot > INT64_MAX / 3) {
+            delete e; return fail(nullptr, SW_E_ARG, "total stake above (2^63 - 1) / 3");
+        }
     }
     // a round other than the last needs more than 2*tot/3 members with a witness (quirk Q3)
     i64 per = std::min<i64>(M, (2 * e->tot) / 3 + 1);

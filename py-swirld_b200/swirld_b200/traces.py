@@ -221,6 +221,69 @@ def late_joiner(M: int, N: int, join_at: int, seed: int = 1) -> Trace:
     return _finish(M, np.array(p0, np.int32), np.array(p1, np.int32), np.array(cr, np.int32), seed, "late-joiner")
 
 
+TIME_KINDS = ("wall", "shuffle", "neg", "const", "huge", "tiny")
+PREFIXES = (8, 16, 32, 56, 60)
+SIG_KINDS = tuple("prefix%d" % p for p in PREFIXES) + tuple("prefix%d_coin" % p for p in PREFIXES) + ("coin0", "coin1")
+
+
+def _restamp_times(kind, tr, rng):
+    N = tr.N
+    i = np.arange(N, dtype=np.float64)
+    if kind == "wall":           # a wall clock in seconds, each member's off by up to 5 s, with sub-microsecond jitter
+        skew = rng.uniform(-5.0, 5.0, tr.M)
+        return 1.7e9 + i * 1e-3 + skew[tr.creator] + rng.uniform(0.0, 1e-6, N)
+    if kind == "shuffle":
+        return rng.permutation(N) + 1.0
+    if kind == "neg":
+        return rng.uniform(-1e6, 1e6, N)
+    if kind == "const":
+        return np.full(N, 1234.5)
+    if kind == "huge":           # medians of two 1e308 overflow to +inf
+        t = rng.uniform(-1.0, 1.0, N)
+        t[rng.random(N) < 0.5] = 1e308
+        return t
+    if kind == "tiny":           # odd multiples of the least subnormal: .5 * (a + b) rounds half to even
+        return rng.integers(1, 1 << 12, N).astype(np.float64) * 5e-324
+    raise ValueError(kind)
+
+
+def _restamp_sigs(kind, tr, rng):
+    N = tr.N
+    sig = tr.sig.copy()
+    if kind in ("coin0", "coin1"):
+        sig[:, 0] = (sig[:, 0] & 0x7F) | (0x80 if kind == "coin1" else 0)
+        return sig
+    P = int(kind[len("prefix"):].split("_")[0])
+    assert P in PREFIXES, kind
+    sig[:, :P] = rng.integers(0, 256, P, dtype=np.uint8)
+    sig[:, 60:] = rng.permutation(N).astype(">u4").view(np.uint8).reshape(N, 4)
+    if kind.endswith("_coin"):
+        sig[:, 0] = (sig[:, 0] & 0x7F) | (tr.sig[:, 0] & 0x80)
+    return sig
+
+
+def restamped(base: str, times: str, sigs: str, seed: int = 1, **base_kwargs) -> Trace:
+    """The graph of generator ``base`` (called with ``seed`` and ``base_kwargs``) with other value columns: the
+    timestamps and signatures that only find_order and the coin read.
+
+    times: ``wall`` (fractional seconds near 1.7e9, out of arrival order across members), ``shuffle`` (a permutation of
+    1..N, not monotone along chains), ``neg`` (mixed signs), ``const`` (one value: every order is decided by the
+    signature key), ``huge`` (half 1e308, the rest in (-1, 1): medians overflow to +inf), ``tiny`` (subnormals).
+    sigs: ``prefixP`` (bytes [0, P) one constant for the trace, bytes [60, 64) a permutation of the events, so ties are
+    decided at byte P or later), ``prefixP_coin`` (the same with bit 7 of byte 0, the coin, left as it was), ``coin0`` /
+    ``coin1`` (the coin bit forced).
+
+    No time is NaN, +-0.0 or -inf and signatures stay pairwise distinct: on such columns the reference's order depends
+    on how Python iterates a set."""
+    tr = globals()[base](seed=seed, **base_kwargs)
+    rng = np.random.default_rng([seed, 0x7E57])
+    t = _restamp_times(times, tr, rng)
+    sig = _restamp_sigs(sigs, tr, rng)
+    assert not np.isnan(t).any() and not (t == 0).any() and not (t == -np.inf).any()
+    assert np.unique(sig, axis=0).shape[0] == tr.N, "signatures must stay distinct"
+    return Trace(tr.M, tr.p0, tr.p1, tr.creator, t, sig, "%s[t=%s,sig=%s]" % (tr.name, times, sigs))
+
+
 def chunks(n: int, k: int):
     """The call schedule: consecutive [first, first+count) slices of K events,
     one (divide_rounds, decide_fame, find_order) triple per slice

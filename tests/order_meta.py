@@ -22,6 +22,7 @@ class OrderMeta:
         self.t = np.empty(0, np.float64)
         self.cs = np.empty((0, o.M), np.int32)      # can_see rows fetched so far (they never change once divided)
         self.ts, self.rr = [], []                   # parallel to the oracle's transactions
+        self.med = []                               # ... and the two times each median was taken from
 
     def add_columns(self, p0, creator, t):
         self.p0 = np.concatenate([self.p0, np.asarray(p0, np.int32)])
@@ -36,7 +37,7 @@ class OrderMeta:
     def _times(self, r, X, wt, fam):
         F = np.array([w for w in wt[r] if w >= 0 and fam[w] == 1], np.int64)
         if X.size == 0:
-            return np.empty(0, np.float64)
+            return np.empty((2, 0), np.float64)
         C = self.creator[X]
         A = np.repeat(F[:, None], X.size, axis=1)
         sees = self.cs[A, C] >= X
@@ -49,7 +50,7 @@ class OrderMeta:
         s = np.sort(np.where(sees, self.t[cur], np.inf), axis=0)
         n = sees.sum(axis=0)
         cols = np.arange(X.size)
-        return .5 * (s[n // 2, cols] + s[(n + 1) // 2, cols])     # swirld.py:305 (n >= 2 for an ordered event)
+        return s[n // 2, cols], s[(n + 1) // 2, cols]             # swirld.py:305 (n >= 2 for an ordered event)
 
     def find_order(self, new_c, n_divided):
         L, h = orc.lib(), self.o._h
@@ -67,7 +68,10 @@ class OrderMeta:
             tx = np.empty(after, np.int32)
             L.or_get_transactions(h, tx)
             X = tx[before:].astype(np.int64)
-            self.ts += self._times(r, X, res["witness_table"], res["famous"]).tolist()
+            a, b = self._times(r, X, res["witness_table"], res["famous"])
+            with np.errstate(over="ignore"):         # two times near DBL_MAX: the sum is +inf, as in the reference
+                self.ts += (.5 * (a + b)).tolist()
+            self.med += list(zip(a.tolist(), b.tolist()))
             self.rr += [r] * X.size
         end = L.or_n_transactions(h)
         tx = np.empty(end, np.int32)
@@ -76,9 +80,10 @@ class OrderMeta:
         return (tx[start:].copy(), np.array(self.ts[start:end], np.float64), np.array(self.rr[start:end], np.int32))
 
 
-def run_oracle_meta(tr, K, stake=None, coin_period=6):
+def run_oracle_meta(tr, K, stake=None, coin_period=6, extra=False):
     """Feed a trace with the call schedule K (chunk size, or a list of chunk sizes); returns the oracle's transactions
-    and their consensus times and rounds received."""
+    and their consensus times and rounds received.  extra=True adds the two times of each median ("median", [n, 2]),
+    results() and coverage()."""
     from swirld_b200.traces import chunks
     o = orc.Oracle(tr.M, stake, coin_period)
     o.append(tr)
@@ -93,6 +98,8 @@ def run_oracle_meta(tr, K, stake=None, coin_period=6):
         orc.lib().or_get_transactions(o._h, tx)
     out = {"transactions": tx, "consensus_time": np.array(m.ts, np.float64),
            "round_received": np.array(m.rr, np.int32)}
+    if extra:
+        out.update(median=np.array(m.med, np.float64).reshape(-1, 2), results=o.results(), coverage=o.coverage())
     o.close()
     return out
 

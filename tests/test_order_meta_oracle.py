@@ -19,7 +19,7 @@ META = sorted(os.path.basename(p)[len("meta_"):-len(".npz")]
 
 
 def test_meta_fixtures_present():
-    assert len(META) == 11
+    assert len(META) == 19
 
 
 @pytest.mark.parametrize("name", META)

@@ -26,13 +26,14 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 import golden_specs as gs  # noqa: E402
 import ref_harness as rh   # noqa: E402
 
-# K = 1 cadence, stakes (zero included), tied times, the late joiner, two-word masks, wide: specs the reference runs in
-# seconds to a minute
+# K = 1 cadence, stakes (zero included, and the largest total), tied times, the late joiner, two-word masks, wide, other
+# value columns: specs the reference runs in seconds to a minute
 SPECS = ["g1_m4_n2000_s1_k1", "g2_m8_n6000_s2_k1",
          "g1_m5_n1500_s4_k11_stake", "g1_m7_n3000_s4_k11_stake", "g1_m80_n8000_s4_k999_stake",
          "g1_m16_n8000_s1_tied8_k1000", "g4_m9_n6000_join3000_s77_k2500",
          "g1_m33_n6000_s7_k640", "g1_m64_n20000_s1_k2000",
-         "g1_m96_n20000_s3_k3000", "g3_m128_n12000_s1_k2048"]
+         "g1_m96_n20000_s3_k3000", "g3_m128_n12000_s1_k2048"] + \
+    [n for n in gs.SPECS if n.startswith("rs_")] + ["g1_m4_n600_s31_k7_bigstake"]
 
 
 def path(name):
