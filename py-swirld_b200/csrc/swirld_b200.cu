@@ -20,6 +20,7 @@
 #include <array>
 #include <string>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 namespace {
@@ -30,7 +31,69 @@ std::string g_create_error;
 using Id32 = std::array<uint64_t, 4>;
 struct Id32Hash { size_t operator()(const Id32 &k) const { return (size_t)(k[0] ^ (k[1] * 0x9E3779B97F4A7C15ull)); } };
 
-struct TimedSpan { cudaEvent_t a, b; int cat; bool shared_a = false; };   // shared_a: `a` is another span's start too
+// ---- the owners of the engine's CUDA resources: move-only, released on destruction
+// Device memory, or pinned host memory (PINNED): cap() elements of T, at least one (a zero-size request gets one)
+template <class T, bool PINNED = false>
+class Mem {
+    T *p_ = nullptr;
+    size_t n_ = 0;
+  public:
+    Mem() = default;
+    Mem(Mem &&o) noexcept : p_(std::exchange(o.p_, nullptr)), n_(std::exchange(o.n_, 0)) {}
+    Mem &operator=(Mem &&o) noexcept { std::swap(p_, o.p_); std::swap(n_, o.n_); return *this; }
+    ~Mem() { reset(); }
+    T *get() const { return p_; }
+    size_t cap() const { return n_; }
+    void reset() {
+        if (p_) (void)(PINNED ? cudaFreeHost(p_) : cudaFree(p_));
+        p_ = nullptr; n_ = 0;
+    }
+    cudaError_t alloc(size_t n) {
+        reset();
+        void *q = nullptr;
+        const size_t bytes = std::max<size_t>(n, 1) * sizeof(T);
+        const cudaError_t s = PINNED ? cudaMallocHost(&q, bytes) : cudaMalloc(&q, bytes);
+        if (s == cudaSuccess) { p_ = static_cast<T *>(q); n_ = std::max<size_t>(n, 1); }
+        return s;
+    }
+};
+template <class T> using Pinned = Mem<T, true>;
+
+// A stream, an event or a peer's IPC-mapped memory
+template <class H, cudaError_t (*Release)(H)>
+class Handle {
+    H h_ = nullptr;
+  protected:
+    // `h` by reference: it is read only once the call that made `s` has written it
+    cudaError_t take(cudaError_t s, const H &h) { reset(); if (s == cudaSuccess) h_ = h; return s; }
+  public:
+    Handle() = default;
+    Handle(Handle &&o) noexcept : h_(std::exchange(o.h_, nullptr)) {}
+    Handle &operator=(Handle &&o) noexcept { std::swap(h_, o.h_); return *this; }
+    ~Handle() { reset(); }
+    H get() const { return h_; }
+    void reset() { if (h_) (void)Release(h_); h_ = nullptr; }
+};
+struct Stream : Handle<cudaStream_t, cudaStreamDestroy> {
+    cudaError_t create() { cudaStream_t s = nullptr; return take(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking), s); }
+};
+struct Event : Handle<cudaEvent_t, cudaEventDestroy> {
+    cudaError_t create(bool timing = false) {
+        cudaEvent_t ev = nullptr;
+        return take(timing ? cudaEventCreate(&ev) : cudaEventCreateWithFlags(&ev, cudaEventDisableTiming), ev);
+    }
+};
+struct PeerMem : Handle<void *, cudaIpcCloseMemHandle> {
+    cudaError_t open(const void *handle64) {
+        cudaIpcMemHandle_t h;
+        memcpy(&h, handle64, sizeof h);
+        void *p = nullptr;
+        return take(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess), p);
+    }
+};
+
+// `a` is `own_a`, or the start of another span, which owns it
+struct TimedSpan { cudaEvent_t a; Event own_a, b; int cat; };
 
 }  // namespace
 
@@ -43,35 +106,36 @@ struct sw_engine {
     bool unit = true;
     i64 tot = 0;
     std::vector<i64> h_stake;
+    Stream stream;
+    Stream copy_stream;                              // sw_append's copies run beside the kernels of earlier chunks
+    Stream rstream, pstream;                         // the round stream and its prep stream (sw_engine::ahead)
     // host mirrors for validation / views
     std::vector<int32_t> h_creator, h_head, h_count;
-    int32_t *h_height = nullptr, *h_seq = nullptr;   // pinned, cap entries: sources of asynchronous copies
-    uint8_t *h_stale = nullptr;                      // pinned: the other-parent is not its member's latest event
+    Pinned<int32_t> h_height, h_seq;                 // cap entries: sources of asynchronous copies
+    Pinned<uint8_t> h_stale;                         // the other-parent is not its member's latest event
     // h_count as it stood after every SNAP-th event and at the end of every append not yet divided, so that the
     // per-member counts of any chunk cost O(M) plus fewer than SNAP events (chunk_prep)
     static constexpr int SNAP = 4096;
     std::vector<int> snap_at;                        // event counts of the snapshots, ascending
     std::vector<int32_t> snap_cnt;                   // [snapshot][M]
     size_t snap_kept = 0;                            // snapshots [0, snap_kept) are all SNAP-event ones
-    cudaStream_t copy_stream = nullptr;              // sw_append's copies run beside the kernels of earlier chunks
-    struct PendingAppend { int base; cudaEvent_t done; };
+    struct PendingAppend { int base; Event done; };
     std::vector<PendingAppend> appends;              // copies (+ eager can_see scans) the compute stream has not waited for yet
-    cudaEvent_t scan_ev = nullptr;                   // last can_see scan issued on the compute stream
+    Event scan_ev;                                   // last can_see scan issued on the compute stream
     bool scan_ev_set = false;
     int n_events = 0, n_divided = 0, n_tx = 0;
     // device columns
-    int32_t *d_p0 = nullptr, *d_p1 = nullptr, *d_creator = nullptr, *d_seq = nullptr, *d_height = nullptr;
-    uint8_t *d_stale = nullptr;
-    long long *d_dbg = nullptr;
+    Mem<int32_t> d_p0, d_p1, d_creator, d_seq, d_height;
+    Mem<uint8_t> d_stale;
+    Mem<long long> d_dbg;
     unsigned rb_epoch = 0;        // launches of the round kernel (mask-cache key)
     int n_sm = 0;
-    int32_t *d_Wf = nullptr, *d_cev = nullptr, *d_rbmeta = nullptr, *d_rbtot = nullptr, *d_gchain = nullptr;   // round-batch state
-    ulonglong2 *d_sc = nullptr;
-    uint8_t *d_res = nullptr;
-    // cluster round kernel (swirld_rcluster.cuh): seq-space rows of the current chunk (the round stream's pieces use both
-    // buffers in turn, the compute stream the first), hand-over state
-    int32_t *d_rsg[2] = {nullptr, nullptr}, *d_rccont = nullptr;
-    size_t rsg_cap[2] = {0, 0};   // events d_rsg[b] holds
+    Mem<int32_t> d_Wf, d_cev, d_rbmeta, d_rbtot, d_gchain;   // round-batch state (d_rbmeta: rb_meta)
+    Mem<ulonglong2> d_sc;
+    Mem<uint8_t> d_res;
+    // cluster round kernel (swirld_rcluster.cuh): seq-space rows of the current chunk, 64 ints per event (the round
+    // stream's pieces use both buffers in turn, the compute stream the first), hand-over state
+    Mem<int32_t> d_rsg[2], d_rccont;
     bool rc_ok = false;           // a 16-CTA cluster with its shared memory can be resident on this device
     int rc_min_n = 2048;          // shorter chunks go to the grid-wide kernel directly
     // The rounds run ahead (SW_ROUNDS_AHEAD, M <= 64, calls that go to the cluster kernel): a call whose can_see rows reach
@@ -87,88 +151,88 @@ struct sw_engine {
     // d_rsg buffer that piece does not use (`rs_buf` alternates); it waits for the piece before that one to have finished
     // with them (`rs_bufdone`), and the piece's cluster kernel waits for it (`rs_prepped`).
     bool ahead = false;
-    cudaStream_t rstream = nullptr, pstream = nullptr;
-    cudaEvent_t rdone = nullptr, rwait = nullptr;
-    cudaEvent_t rs_prepped[2] = {nullptr, nullptr}, rs_bufdone[2] = {nullptr, nullptr};
+    cudaEvent_t rdone = nullptr;  // (not owned: the event of a piece, in rs_pieces or rs_free)
+    Event rwait;
+    Event rs_prepped[2], rs_bufdone[2];
     int rs_buf = 0;               // the buffers of the next piece
-    struct RsPiece { int end; cudaEvent_t done; };
+    struct RsPiece { int end; Event done; };
     std::vector<RsPiece> rs_pieces;                  // the pieces that end beyond the last call, in order
-    std::vector<cudaEvent_t> rs_free;                // their events once a call has waited for them
-    int32_t *d_Wf2 = nullptr, *d_gchain2 = nullptr, *d_rbmeta2 = nullptr, *d_rscal = nullptr;
+    std::vector<Event> rs_free;                      // their events once a call has waited for them
+    Mem<int32_t> d_Wf2, d_gchain2, d_rbmeta2, d_rscal;
     bool rs_synced = false;       // the round stream's copies hold everything below n_rounded
     int n_rounded = 0;            // events rounded so far (the round stream's piece ends here)
     unsigned rs_epoch = 0;        // launches on the round stream (mask-cache keys of their own: the top bit set)
     int wslot = 0;                // which of the two witness counts of d_rbmeta the next call uses
-    RcParams *d_rcviews = nullptr;
-    RbParams *d_views = nullptr;  // sw_batch_divide_rounds: the views' parameters (owned by the first engine of a batch)
-    int views_cap = 0;
-    cudaEvent_t view_ev = nullptr;
+    Mem<RcParams> d_rcviews;
+    Mem<RbParams> d_views;        // sw_batch_divide_rounds: the views' parameters (owned by the first engine of a batch)
+    Event view_ev;
     // sw_batch_decide_fame / sw_batch_find_order (owned by the first engine of a batch): the views' parameters, rounds
     // and gathered scalars, laid out per call in one device block and its pinned host mirror
-    char *d_vbuf = nullptr, *h_vbuf = nullptr;
-    size_t vbuf_bytes = 0;
+    Mem<char> d_vbuf;
+    Pinned<char> h_vbuf;
     int n_rowed = 0;              // events whose can_see row is complete
     // can_see scan scratch (swirld_cansee.cuh)
-    int4 *d_cs_meta = nullptr;
-    uint8_t *d_cs_wr = nullptr, *d_cs_xb = nullptr, *d_cs_sflag = nullptr;
-    int32_t *d_cs_last = nullptr, *d_cs_Q = nullptr, *d_cs_carry = nullptr, *d_cs_slow = nullptr, *d_cs_slowcnt = nullptr, *d_cs_xlist = nullptr, *d_cs_slowblk = nullptr, *d_cs_blkcnt = nullptr;
+    Mem<int4> d_cs_meta;
+    Mem<uint8_t> d_cs_wr, d_cs_xb, d_cs_sflag;
+    Mem<int32_t> d_cs_last, d_cs_Q, d_cs_carry, d_cs_slow, d_cs_slowcnt, d_cs_xlist, d_cs_slowblk, d_cs_blkcnt;
     std::vector<int32_t> h_stale_cum;    // h_stale_cum[i] = stale other-parents among events [0, i)
     int cs_min_B = 256;           // smallest block length the scan uses (sizes the per-block scratch)
-    double *d_t = nullptr;
-    uint8_t *d_sig = nullptr;
-    int32_t *d_row = nullptr, *d_round = nullptr;
-    u64 *d_SM = nullptr;
-    uint8_t *d_wit = nullptr;
-    int8_t *d_famous_ev = nullptr;
+    Mem<double> d_t;
+    Mem<uint8_t> d_sig;
+    Mem<int32_t> d_row, d_round;
+    Mem<u64> d_SM;
+    Mem<uint8_t> d_wit;
+    Mem<int8_t> d_famous_ev;
     // wide path
-    unsigned *d_scw = nullptr, *d_SMw = nullptr, *d_Sw = nullptr;
-    u64 *d_sctag = nullptr, *d_hitmin = nullptr;
+    Mem<unsigned> d_scw, d_SMw, d_Sw;
+    Mem<u64> d_sctag, d_hitmin;
     // several GPUs (sw_peer_connect): tests of a round step sharded by chain, first hits exchanged over NVLink
     int rank = 0, nranks = 1;
-    void *d_xbuf = nullptr;       // [flags: 64 x u32][hits: 8 x 3 x M x u64], IPC-exported
-    void *x_peer[8] = {nullptr};  // the same buffer of every rank (own: d_xbuf)
-    int32_t *row_peer[8] = {nullptr};   // every rank's can_see table (own: d_row)
-    unsigned **d_xflags2 = nullptr;     // device array of the ranks' barrier flag rows (xbuf + 128 bytes)
+    Mem<char> d_xbuf;             // [flags: 64 x u32][hits: 8 x 3 x M x u64], IPC-exported
+    PeerMem x_map[8], row_map[8]; // the other ranks' d_xbuf and d_row, mapped here
+    void *x_peer[8] = {nullptr};  // (not owned) the same buffer of every rank (own: d_xbuf, others: x_map)
+    int32_t *row_peer[8] = {nullptr};   // (not owned) every rank's can_see table (own: d_row, others: row_map)
+    Mem<unsigned *> d_xflags2;    // device array of the ranks' barrier flag rows (xbuf + 128 bytes)
     unsigned xbar_count = 0;      // cross-GPU barriers issued so far (identical on every rank)
-    unsigned *d_xstep = nullptr;  // steps published so far (device-resident: the step count of a launch is data dependent)
+    Mem<unsigned> d_xstep;        // steps published so far (device-resident: the step count of a launch is data dependent)
     // per round
-    int32_t *d_W = nullptr, *d_rem = nullptr, *d_newc = nullptr;
-    u64 *d_S = nullptr;
-    int8_t *d_famous = nullptr;
-    uint8_t *d_consensus = nullptr, *d_done = nullptr, *d_coin = nullptr;
-    i64 *d_stake = nullptr;
-    int32_t *d_scal = nullptr;
+    Mem<int32_t> d_W, d_rem;
+    int32_t *d_newc = nullptr;    // (not owned) right behind the scalars in d_scal
+    Mem<u64> d_S;
+    Mem<int8_t> d_famous;
+    Mem<uint8_t> d_consensus, d_done, d_coin;
+    Mem<i64> d_stake;
+    Mem<int32_t> d_scal;
     // find_order
-    int32_t *d_lastord = nullptr, *d_tx = nullptr, *d_tx_rr = nullptr, *d_idx = nullptr, *d_batch_ev = nullptr,
-            *d_batch_seg = nullptr, *d_seg_start = nullptr, *d_seg_fw = nullptr, *d_seg_nf = nullptr,
-            *d_perm = nullptr, *d_rounds_in = nullptr, *d_plan = nullptr;
-    uint8_t *d_seg_white = nullptr;
-    double *d_ts = nullptr, *d_tx_ts = nullptr;   // d_tx_ts, d_tx_rr: by order position, parallel to d_tx
-    u64 *d_key = nullptr;
-    int seg_cap = 0;
-    void *d_flush = nullptr;
-    size_t flush_bytes = 0;
+    Mem<int32_t> d_lastord, d_tx, d_idx, d_batch_ev, d_batch_seg, d_perm;
+    int32_t *d_tx_rr = nullptr;   // (not owned) by order position, parallel to d_tx, in the same block
+    double *d_tx_ts = nullptr;    // (not owned) likewise
+    Mem<double> d_ts;
+    Mem<u64> d_key;
+    // find_order's per-round scratch, grown by order_scratch (d_seg_nf.cap() rounds)
+    Mem<int32_t> d_seg_start, d_seg_fw, d_seg_nf, d_rounds_in, d_plan;
+    Mem<uint8_t> d_seg_white;
+    Mem<char> d_flush;
     // small appends (the reference's cadence: one sync per call): one packed copy instead of eight, from a ring of pinned
     // slots -- one view's columns (sw_append), or a batch's parameters and columns (sw_batch_append, on its first
     // engine).  h_vbuf cannot hold them: the batched fame and order calls of the same turn rewrite it on the host before
     // the asynchronous copy from it would have run.
     static constexpr int STAGE_SLOTS = 8, STAGE_EVENTS = 64;
-    uint8_t *h_stage = nullptr, *d_stage = nullptr;
-    size_t stage_bytes = 0;       // per slot
-    cudaEvent_t stage_ev[STAGE_SLOTS] = {nullptr};
+    Pinned<uint8_t> h_stage;
+    Mem<uint8_t> d_stage;         // STAGE_SLOTS slots of stage_bytes() each
+    Event stage_ev[STAGE_SLOTS];
     int stage_next = 0;
     static constexpr int STREAM_N = 16;              // divide_rounds calls of at most this many events take the one-launch path
-    StreamParams *d_stviews = nullptr;               // sw_batch_divide_rounds: the parameters of the views on that path
-    int stviews_cap = 0;
-    int32_t *h_scal = nullptr;    // pinned
-    int32_t *h_newc = nullptr;    // pinned, Rcap: right behind h_scal (one copy brings both back)
-    cudaStream_t stream = nullptr;
-    cudaEvent_t user_ev[16] = {nullptr};
+    Mem<StreamParams> d_stviews;                     // sw_batch_divide_rounds: the parameters of the views on that path
+    Pinned<int32_t> h_scal;
+    int32_t *h_newc = nullptr;    // (not owned) Rcap: right behind the scalars in h_scal (one copy brings both back)
+    Event user_ev[16];
     std::vector<TimedSpan> spans;
-    std::vector<cudaEvent_t> pool;
+    std::vector<Event> pool;      // timing events no span or append holds
     std::unordered_map<Id32, int32_t, Id32Hash> ids;     // sw_ingest: event id -> arrival index
     sw_stats_t stats{};
     std::string err;
+    size_t stage_bytes() const { return d_stage.cap() / STAGE_SLOTS; }
 };
 
 namespace {
@@ -201,28 +265,31 @@ int fail(sw_engine *e, int code, const char *fmt, ...) {
     ((x)->NC == 1 ? ((x)->unit ? F<1, true>(__VA_ARGS__) : F<1, false>(__VA_ARGS__))    \
                   : ((x)->unit ? F<2, true>(__VA_ARGS__) : F<2, false>(__VA_ARGS__)))
 
-template <typename T>
-cudaError_t dalloc(T **p, size_t n) { return cudaMalloc((void **)p, std::max<size_t>(n, 1) * sizeof(T)); }
-
-cudaEvent_t get_event(sw_engine *e) {
-    if (!e->pool.empty()) { cudaEvent_t ev = e->pool.back(); e->pool.pop_back(); return ev; }
-    cudaEvent_t ev;
-    cudaEventCreate(&ev);
+Event get_event(sw_engine *e) {                    // a timing event: one the pool has, or a new one
+    Event ev;
+    if (!e->pool.empty()) { ev = std::move(e->pool.back()); e->pool.pop_back(); }
+    else ev.create(true);
     return ev;
 }
 
+// the span from `a` to `b`, which it owns (fold_spans returns them to the pool)
+void add_span(sw_engine *e, Event a, Event b, int cat) {
+    const cudaEvent_t start = a.get();
+    e->spans.push_back(TimedSpan{start, std::move(a), std::move(b), cat});
+}
+
 struct Span {
-    sw_engine *e; TimedSpan s;
-    Span(sw_engine *e_, int cat) : e(e_) { s.a = get_event(e); s.b = get_event(e); s.cat = cat; cudaEventRecord(s.a, e->stream); }
-    ~Span() { cudaEventRecord(s.b, e->stream); e->spans.push_back(s); }
+    sw_engine *e; Event a, b; int cat;
+    Span(sw_engine *e_, int cat_) : e(e_), a(get_event(e_)), b(get_event(e_)), cat(cat_) { cudaEventRecord(a.get(), e->stream.get()); }
+    ~Span() { cudaEventRecord(b.get(), e->stream.get()); add_span(e, std::move(a), std::move(b), cat); }
 };
 
 void fold_spans(sw_engine *e) {
     std::vector<TimedSpan> pending;
     for (auto &s : e->spans) {
-        if (cudaEventQuery(s.b) == cudaErrorNotReady) { pending.push_back(s); continue; }   // (a scan still running on the copy stream)
+        if (cudaEventQuery(s.b.get()) == cudaErrorNotReady) { pending.push_back(std::move(s)); continue; }   // (a scan still running on the copy stream)
         float ms = 0.f;
-        if (cudaEventElapsedTime(&ms, s.a, s.b) == cudaSuccess) {
+        if (cudaEventElapsedTime(&ms, s.a, s.b.get()) == cudaSuccess) {
             if (s.cat == 0) e->stats.ms_divide_rounds += ms;
             else if (s.cat == 1) e->stats.ms_decide_fame += ms;
             else if (s.cat == 2) e->stats.ms_find_order += ms;
@@ -230,8 +297,8 @@ void fold_spans(sw_engine *e) {
             else if (s.cat == 4) e->stats.ms_rounds_kernel += ms;
             else if (s.cat == 5) e->stats.ms_can_see += ms;       // (a scan inside a divide_rounds span)
         }
-        if (!s.shared_a) e->pool.push_back(s.a);
-        e->pool.push_back(s.b);
+        if (s.own_a.get()) e->pool.push_back(std::move(s.own_a));
+        e->pool.push_back(std::move(s.b));
     }
     e->spans.swap(pending);
 }
@@ -240,16 +307,43 @@ void fold_spans(sw_engine *e) {
 int wait_appends(sw_engine *e, int upto) {
     size_t k = 0;
     for (auto &a : e->appends) {
-        if (upto >= 0 && a.base >= upto) { e->appends[k++] = a; continue; }
-        CK(cudaStreamWaitEvent(e->stream, a.done, 0));
-        e->pool.push_back(a.done);           // (re-recorded only after later work was enqueued behind the wait)
+        if (upto >= 0 && a.base >= upto) { e->appends[k++] = std::move(a); continue; }
+        CK(cudaStreamWaitEvent(e->stream.get(), a.done.get(), 0));
+        e->pool.push_back(std::move(a.done));   // (re-recorded only after later work was enqueued behind the wait)
     }
     e->appends.resize(k);
     return 0;
 }
 
+// every stream of the engine idle
+int sync_streams(sw_engine *e) {
+    for (const Stream *s : {&e->stream, &e->copy_stream, &e->rstream, &e->pstream})
+        if (s->get()) CK(cudaStreamSynchronize(s->get()));
+    return 0;
+}
+
+// A buffer and the elements grow() gives it
+template <class T, bool P> struct Sized { Mem<T, P> &m; size_t n; };
+template <class T, bool P> Sized<T, P> sized(Mem<T, P> &m, size_t n) { return {m, n}; }
+
+// The one way a buffer grows.  Nothing happens while `need` <= `have` (in the caller's unit: events, rounds, views or
+// bytes).  Else every stream of the engine goes idle, since a kernel or copy on any of them may still read the old
+// buffers, and the buffers are freed and allocated again at the sizes the caller asks for; after a failure all of them
+// are empty.  Grows are rare (most callers double), so the synchronisation stays off the steady state.
+template <class... S>
+int grow(sw_engine *e, size_t need, size_t have, S... bufs) {
+    if (need <= have) return 0;
+    if (sync_streams(e) < 0) return SW_E_CUDA;
+    (bufs.m.reset(), ...);
+    cudaError_t s = cudaSuccess;
+    ((s = s == cudaSuccess ? bufs.m.alloc(bufs.n) : s), ...);
+    if (s == cudaSuccess) return 0;
+    (bufs.m.reset(), ...);
+    return fail(e, SW_E_CUDA, "growing a buffer: %s", cudaGetErrorString(s));
+}
+
 int device_error(sw_engine *e) {     // after a sync: did a kernel flag an error?
-    int code = e->h_scal[SC_ERR];
+    int code = e->h_scal.get()[SC_ERR];
     if (code < 0) {
         const char *what = code == SW_E_CAPACITY ? "round table exhausted"
                          : code == SW_E_INDEX ? "list index out of range (swirld.py:305: a single seer)"
@@ -262,27 +356,27 @@ int device_error(sw_engine *e) {     // after a sync: did a kernel flag an error
 
 int reset_state(sw_engine *e, bool keep_events = false) {
     const size_t RM = (size_t)e->Rcap * e->M;
-    k_fill_i32<<<256, 256, 0, e->stream>>>(e->d_W, -1, RM);
-    CK(cudaMemsetAsync(e->d_famous, 0xff, RM, e->stream));
-    CK(cudaMemsetAsync(e->d_consensus, 0, e->Rcap, e->stream));
-    CK(cudaMemsetAsync(e->d_famous_ev, 0xff, e->cap, e->stream));
-    k_fill_i32<<<256, 256, 0, e->stream>>>(e->d_idx, -1, (size_t)e->cap);
-    k_fill_i32<<<4, 256, 0, e->stream>>>(e->d_lastord, -1, (size_t)e->MP);
-    k_fill_i32<<<4, 256, 0, e->stream>>>(e->d_cs_carry, -1, (size_t)e->MP);
-    k_fill_i32<<<256, 256, 0, e->stream>>>(e->d_Wf, -1, RM);
-    CK(cudaMemsetAsync(e->d_rbtot, 0, sizeof(int32_t) * e->MP, e->stream));
-    k_fill_i32<<<64, 256, 0, e->stream>>>(e->d_gchain, -1, (size_t)e->MP * RB_RING);
+    k_fill_i32<<<256, 256, 0, e->stream.get()>>>(e->d_W.get(), -1, RM);
+    CK(cudaMemsetAsync(e->d_famous.get(), 0xff, RM, e->stream.get()));
+    CK(cudaMemsetAsync(e->d_consensus.get(), 0, e->Rcap, e->stream.get()));
+    CK(cudaMemsetAsync(e->d_famous_ev.get(), 0xff, e->cap, e->stream.get()));
+    k_fill_i32<<<256, 256, 0, e->stream.get()>>>(e->d_idx.get(), -1, (size_t)e->cap);
+    k_fill_i32<<<4, 256, 0, e->stream.get()>>>(e->d_lastord.get(), -1, (size_t)e->MP);
+    k_fill_i32<<<4, 256, 0, e->stream.get()>>>(e->d_cs_carry.get(), -1, (size_t)e->MP);
+    k_fill_i32<<<256, 256, 0, e->stream.get()>>>(e->d_Wf.get(), -1, RM);
+    CK(cudaMemsetAsync(e->d_rbtot.get(), 0, sizeof(int32_t) * e->MP, e->stream.get()));
+    k_fill_i32<<<64, 256, 0, e->stream.get()>>>(e->d_gchain.get(), -1, (size_t)e->MP * RB_RING);
     if (e->wide) {
-        CK(cudaMemsetAsync(e->d_Sw, 0, RM * e->NJ * sizeof(unsigned), e->stream));
-        CK(cudaMemsetAsync(e->d_sctag, 0, sizeof(u64) * (size_t)e->cap, e->stream));
+        CK(cudaMemsetAsync(e->d_Sw.get(), 0, RM * e->NJ * sizeof(unsigned), e->stream.get()));
+        CK(cudaMemsetAsync(e->d_sctag.get(), 0, sizeof(u64) * (size_t)e->cap, e->stream.get()));
     } else {
-        CK(cudaMemsetAsync(e->d_S, 0, RM * sizeof(u64), e->stream));
-        CK(cudaMemsetAsync(e->d_sc, 0, sizeof(ulonglong2) * (size_t)e->cap, e->stream));
+        CK(cudaMemsetAsync(e->d_S.get(), 0, RM * sizeof(u64), e->stream.get()));
+        CK(cudaMemsetAsync(e->d_sc.get(), 0, sizeof(ulonglong2) * (size_t)e->cap, e->stream.get()));
     }
     int32_t sc[SC_COUNT] = {0};
     sc[SC_MAX_ROUND] = -1;
-    CK(cudaMemcpyAsync(e->d_scal, sc, sizeof sc, cudaMemcpyHostToDevice, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaMemcpyAsync(e->d_scal.get(), sc, sizeof sc, cudaMemcpyHostToDevice, e->stream.get()));
+    CK(cudaStreamSynchronize(e->stream.get()));
     e->stats.kernel_launches += 5;
     e->n_divided = e->n_tx = 0;
     e->n_rowed = 0;
@@ -294,7 +388,7 @@ int reset_state(sw_engine *e, bool keep_events = false) {
         std::fill(e->h_count.begin(), e->h_count.end(), 0);
         e->snap_at.clear(); e->snap_cnt.clear(); e->snap_kept = 0;
     }
-    memset(e->h_scal, 0, sizeof(int32_t) * SC_COUNT);
+    memset(e->h_scal.get(), 0, sizeof(int32_t) * SC_COUNT);
     return 0;
 }
 
@@ -328,15 +422,15 @@ int cansee_scan(sw_engine *e, cudaStream_t st, int upto, int cat = 3) {
     const int M = e->M;
     CsParams C{};
     C.M = M; C.first = first; C.n = n;
-    C.p0 = e->d_p0; C.p1 = e->d_p1; C.creator = e->d_creator; C.stale = e->d_stale; C.row = e->d_row;
-    C.meta = e->d_cs_meta; C.wr = e->d_cs_wr; C.xb = e->d_cs_xb; C.last = e->d_cs_last; C.Qtab = e->d_cs_Q;
-    C.carry = e->d_cs_carry; C.slow_list = e->d_cs_slow; C.slow_cnt = e->d_cs_slowcnt; C.sflag = e->d_cs_sflag; C.xlist = e->d_cs_xlist; C.slow_blk = e->d_cs_slowblk; C.blk_cnt = e->d_cs_blkcnt;
-    cudaEvent_t a = get_event(e), b = get_event(e);
+    C.p0 = e->d_p0.get(); C.p1 = e->d_p1.get(); C.creator = e->d_creator.get(); C.stale = e->d_stale.get(); C.row = e->d_row.get();
+    C.meta = e->d_cs_meta.get(); C.wr = e->d_cs_wr.get(); C.xb = e->d_cs_xb.get(); C.last = e->d_cs_last.get(); C.Qtab = e->d_cs_Q.get();
+    C.carry = e->d_cs_carry.get(); C.slow_list = e->d_cs_slow.get(); C.slow_cnt = e->d_cs_slowcnt.get(); C.sflag = e->d_cs_sflag.get(); C.xlist = e->d_cs_xlist.get(); C.slow_blk = e->d_cs_slowblk.get(); C.blk_cnt = e->d_cs_blkcnt.get();
+    Event a = get_event(e), b = get_event(e);
     if (n <= 24) {                                     // the reference's own cadence: a handful of events per call
-        cudaEventRecord(a, st);
+        cudaEventRecord(a.get(), st);
         k_cs_small<<<1, std::min(1024, (M + 31) / 32 * 32), 0, st>>>(C);
-        cudaEventRecord(b, st);
-        e->spans.push_back(TimedSpan{a, b, cat});
+        cudaEventRecord(b.get(), st);
+        add_span(e, std::move(a), std::move(b), cat);
         CK(cudaGetLastError());
         e->stats.kernel_launches += 1;
         e->n_rowed = upto;
@@ -374,21 +468,21 @@ int cansee_scan(sw_engine *e, cudaStream_t st, int upto, int cat = 3) {
     const int ntiles = std::max(0, tile_hi - tile_lo);
     auto xbarrier = [&]() -> int {
         if (!shard) return 0;
-        k_xbarrier<<<1, 32, 0, st>>>(e->d_xflags2, e->rank, e->nranks, ++e->xbar_count, e->d_scal);
+        k_xbarrier<<<1, 32, 0, st>>>(e->d_xflags2.get(), e->rank, e->nranks, ++e->xbar_count, e->d_scal.get());
         CK(cudaGetLastError());
         return 0;
     };
     const size_t smem = (size_t)(M + C.SV) * CT * sizeof(int) + CS_TILE * sizeof(int4) + 3 * CS_TILE;
     const int pblocks = std::max(1, std::min(8 * e->n_sm, (n + 255) / 256));
-    k_fill_i32<<<std::max(1, std::min(256, (int)(((size_t)C.nb * M + 255) / 256))), 256, 0, st>>>(e->d_cs_last, -1, (size_t)C.nb * M);
+    k_fill_i32<<<std::max(1, std::min(256, (int)(((size_t)C.nb * M + 255) / 256))), 256, 0, st>>>(e->d_cs_last.get(), -1, (size_t)C.nb * M);
     if (C.nb > 1) {
-        CK(cudaMemsetAsync(e->d_cs_wr + first, 0, (size_t)n, st));
-        CK(cudaMemsetAsync(e->d_cs_xb + (first & ~3), 0, (size_t)(n + (first & 3)), st));
-        CK(cudaMemsetAsync(e->d_cs_sflag + first, 0, (size_t)n, st));
-        CK(cudaMemsetAsync(e->d_cs_slowcnt, 0, sizeof(int32_t) * 4, st));
-        CK(cudaMemsetAsync(e->d_cs_blkcnt, 0, sizeof(int32_t) * (size_t)C.nb, st));
+        CK(cudaMemsetAsync(e->d_cs_wr.get() + first, 0, (size_t)n, st));
+        CK(cudaMemsetAsync(e->d_cs_xb.get() + (first & ~3), 0, (size_t)(n + (first & 3)), st));
+        CK(cudaMemsetAsync(e->d_cs_sflag.get() + first, 0, (size_t)n, st));
+        CK(cudaMemsetAsync(e->d_cs_slowcnt.get(), 0, sizeof(int32_t) * 4, st));
+        CK(cudaMemsetAsync(e->d_cs_blkcnt.get(), 0, sizeof(int32_t) * (size_t)C.nb, st));
     }
-    cudaEventRecord(a, st);
+    cudaEventRecord(a.get(), st);
     k_cs_prep<<<pblocks, 256, 0, st>>>(C);
     if (C.nb > 1) {
         if (ntiles > 0) {
@@ -413,8 +507,8 @@ int cansee_scan(sw_engine *e, cudaStream_t st, int upto, int cat = 3) {
     }
     if (shard) k_cs_carry<<<(M + 255) / 256, 256, 0, st>>>(C);
     if (xbarrier() < 0) return SW_E_CUDA;                  // the whole table is in every rank's memory
-    cudaEventRecord(b, st);
-    e->spans.push_back(TimedSpan{a, b, cat});
+    cudaEventRecord(b.get(), st);
+    add_span(e, std::move(a), std::move(b), cat);
     CK(cudaGetLastError());
     e->stats.kernel_launches += C.nb > 1 ? 9 : 4;
     e->n_rowed = upto;
@@ -459,31 +553,36 @@ void counts_at(const sw_engine *e, int x, int32_t *out) {
     for (int i = from; i < x; i++) out[e->h_creator[i]]++;
 }
 
-// d_rbmeta, one layout for both kernel families (MP = max(M, 64) members)
+// A chunk meta block, one layout for both kernel families (MP = max(M, 64) members): d_rbmeta of the compute stream
+// and the round stream's two blocks in d_rbmeta2, rb_meta_ints(MP) ints each
 struct RbMeta {
     int32_t *ccnt, *cmin, *coff;  // [MP], [MP], [MP + 1]: the chunk's per-member counts, smallest seqs, offsets (k_rb_prep)
     unsigned *bar;                // grid barrier counter of the round kernel
-    int32_t *wcnt;                // witnesses of the chunk (k_rb_finish)
+    int32_t *wcnt;                // [2] witnesses of the chunk (k_rb_finish; the ahead path alternates, sw_engine::wslot)
     unsigned *ticket;             // [3] k_rounds_wide's work counters
+    int32_t *ctot;                // [MP] the round stream's per-member counts at the end of its piece (the compute
+                                  // stream keeps its own in d_rbtot)
 };
 
-RbMeta rb_meta(const sw_engine *e) {
-    int32_t *m = e->d_rbmeta;
-    const int MP = e->MP;
+size_t rb_meta_ints(int MP) { return 4 * (size_t)MP + 64; }
+
+RbMeta rb_meta(int32_t *m, int MP) {
     return RbMeta{m, m + MP, m + 2 * MP, reinterpret_cast<unsigned *>(m + 3 * MP + 8), m + 3 * MP + 9,
-                  reinterpret_cast<unsigned *>(m + 3 * MP + 12)};
+                  reinterpret_cast<unsigned *>(m + 3 * MP + 12), m + 3 * MP + 16};
 }
+
+// the chunk's grouping and the round kernel's barrier and witness count in block m
+void use_meta(RbParams &R, const RbMeta &m) { R.ccnt = m.ccnt; R.cmin = m.cmin; R.coff = m.coff; R.bar = m.bar; R.wcnt = m.wcnt; }
 
 // what both kernel families read of the round-batch parameters: the chunk, its grouping by creator (k_rb_prep) and
 // the pass after the round kernel (k_rb_finish)
 RbParams chunk_params(const sw_engine *e, int first, int n) {
     RbParams R{};
     R.M = e->M; R.first = first; R.n = n; R.Rcap = e->Rcap;
-    R.row = e->d_row; R.p0 = e->d_p0; R.creator = e->d_creator; R.seq = e->d_seq; R.round = e->d_round;
-    R.cev = e->d_cev; R.ctot = e->d_rbtot; R.gchain = e->d_gchain; R.wit = e->d_wit; R.W = e->d_W;
-    const RbMeta m = rb_meta(e);
-    R.ccnt = m.ccnt; R.cmin = m.cmin; R.coff = m.coff; R.bar = m.bar;
-    R.wlist = e->d_cev + e->cap; R.wcnt = m.wcnt;
+    R.row = e->d_row.get(); R.p0 = e->d_p0.get(); R.creator = e->d_creator.get(); R.seq = e->d_seq.get(); R.round = e->d_round.get();
+    R.cev = e->d_cev.get(); R.ctot = e->d_rbtot.get(); R.gchain = e->d_gchain.get(); R.wit = e->d_wit.get(); R.W = e->d_W.get();
+    use_meta(R, rb_meta(e->d_rbmeta.get(), e->MP));
+    R.wlist = e->d_cev.get() + e->cap;
     return R;
 }
 
@@ -512,25 +611,16 @@ int chunk_prep(sw_engine *e, const RbParams &R, int32_t *rsg, cudaStream_t st) {
 RbParams round_params(const sw_engine *e, int first, int n, int grid, int min_L) {
     RbParams R = chunk_params(e, first, n);
     R.L = std::max(std::min(min_L, RB_LMAX), std::min(RB_LMAX, grid * (RB_THREADS / 32) / e->M));
-    R.Wf = e->d_Wf; R.sc = e->d_sc;
-    R.res = e->d_res; R.stake = e->d_stake; R.tot2 = 2 * e->tot; R.scal = e->d_scal;
-    R.SM = e->d_SM; R.dbg = e->d_dbg;
+    R.Wf = e->d_Wf.get(); R.sc = e->d_sc.get();
+    R.res = e->d_res.get(); R.stake = e->d_stake.get(); R.tot2 = 2 * e->tot; R.scal = e->d_scal.get();
+    R.SM = e->d_SM.get(); R.dbg = e->d_dbg.get();
     return R;
 }
 
-// buffer b of the cluster kernel's seq-space rows, for n events (every stream uses them: a new buffer waits for all)
+// buffer b of the cluster kernel's seq-space rows, for n events
 int rsg_reserve(sw_engine *e, int n, int b = 0) {
-    if ((size_t)n <= e->rsg_cap[b]) return 0;
-    if (e->d_rsg[b]) {
-        CK(cudaStreamSynchronize(e->stream));
-        if (e->rstream) CK(cudaStreamSynchronize(e->rstream));
-        if (e->pstream) CK(cudaStreamSynchronize(e->pstream));
-        CK(cudaFree(e->d_rsg[b])); e->d_rsg[b] = nullptr; e->rsg_cap[b] = 0;
-    }
     const size_t want = std::min<size_t>((size_t)e->cap, std::max<size_t>((size_t)n, 1 << 16));
-    CK(dalloc(&e->d_rsg[b], want * 64));
-    e->rsg_cap[b] = want;
-    return 0;
+    return grow(e, n, e->d_rsg[b].cap() / 64, sized(e->d_rsg[b], want * 64));
 }
 
 // rounds of the chunk by the cooperative round-batch kernel (swirld_rounds.cuh), M <= 64: parameters R + the grouping
@@ -540,11 +630,11 @@ int round_batch_prep(sw_engine *e, int first, int n, int grid, int min_L, bool r
     R = round_params(e, first, n, grid, min_L);
     R.epoch = ++e->rb_epoch;
     if (rc && rsg_reserve(e, n) < 0) return SW_E_CUDA;
-    if (chunk_prep<64>(e, R, rc ? e->d_rsg[0] : nullptr, e->stream) < 0) return SW_E_CUDA;
+    if (chunk_prep<64>(e, R, rc ? e->d_rsg[0].get() : nullptr, e->stream.get()) < 0) return SW_E_CUDA;
     e->stats.kernel_launches += 1;
     if (rc) {
-        Q = RcParams{R, e->d_rsg[0], e->d_rccont};
-        R.cont = e->d_rccont;
+        Q = RcParams{R, e->d_rsg[0].get(), e->d_rccont.get()};
+        R.cont = e->d_rccont.get();
     }
     return 0;
 }
@@ -553,16 +643,16 @@ int round_batch_prep(sw_engine *e, int first, int n, int grid, int min_L, bool r
 template <int NC>
 int round_batch_finish(sw_engine *e, const RbParams &R, const RbFold &F = RbFold{}) {
     const int n = R.n, blocks = std::max(1, std::min(296, (n + 255) / 256));
-    k_rb_finish<<<blocks, 256, 0, e->stream>>>(R, F);
-    k_rb_seenmask<NC><<<(n + 7) / 8, 256, 0, e->stream>>>(R);
+    k_rb_finish<<<blocks, 256, 0, e->stream.get()>>>(R, F);
+    k_rb_seenmask<NC><<<(n + 7) / 8, 256, 0, e->stream.get()>>>(R);
     CK(cudaGetLastError());
     StrongParams Q{};
-    Q.M = e->M; Q.first = R.first; Q.n = n; Q.Rcap = e->Rcap; Q.creator = e->d_creator; Q.row = e->d_row;
-    Q.round = e->d_round; Q.wit = e->d_wit; Q.SM = e->d_SM; Q.S = e->d_S; Q.stake = e->d_stake; Q.tot2 = 2 * e->tot;
-    Q.coin = e->d_coin; Q.sig = e->d_sig; Q.unit = e->unit ? 1 : 0;
+    Q.M = e->M; Q.first = R.first; Q.n = n; Q.Rcap = e->Rcap; Q.creator = e->d_creator.get(); Q.row = e->d_row.get();
+    Q.round = e->d_round.get(); Q.wit = e->d_wit.get(); Q.SM = e->d_SM.get(); Q.S = e->d_S.get(); Q.stake = e->d_stake.get(); Q.tot2 = 2 * e->tot;
+    Q.coin = e->d_coin.get(); Q.sig = e->d_sig.get(); Q.unit = e->unit ? 1 : 0;
     Q.list = R.wlist; Q.list_n = R.wcnt;
     const int sblocks = std::max(1, std::min((n + 7) / 8, 4 * e->n_sm));
-    k_strong<NC><<<sblocks, 256, 0, e->stream>>>(Q);
+    k_strong<NC><<<sblocks, 256, 0, e->stream.get()>>>(Q);
     CK(cudaGetLastError());
     e->stats.kernel_launches += 3;
     return 0;
@@ -614,12 +704,12 @@ void count_round_kernels(sw_engine *e, bool rc) {
     e->stats.rounds_cluster_launches += rc ? 1 : 0;
 }
 
-// The round-kernel span from `start`, which the caller recorded; `shared`: it is the start of the caller's own span too (an
-// event record costs the stream a few microseconds)
-void round_span(sw_engine *e, cudaEvent_t start, bool shared) {
-    cudaEvent_t b = get_event(e);
-    cudaEventRecord(b, e->stream);
-    e->spans.push_back(TimedSpan{start, b, 4, shared});
+// The round-kernel span from `start`, which the caller recorded: `own` when the span owns it, else the start of the
+// caller's own span too (an event record costs the stream a few microseconds)
+void round_span(sw_engine *e, cudaEvent_t start, Event own = Event()) {
+    Event b = get_event(e);
+    cudaEventRecord(b.get(), e->stream.get());
+    e->spans.push_back(TimedSpan{start, std::move(own), std::move(b), 4});
 }
 
 // `start`: the event that opens the caller's span, recorded just before
@@ -629,10 +719,10 @@ int divide_round_batch(sw_engine *e, int first, int n, cudaEvent_t start) {
     const bool rc = e->rc_ok && n >= e->rc_min_n;
     RbParams R;
     RcParams Q{};
-    if (round_batch_prep(e, first, n, grid, 1, rc, R, Q) < 0 || round_kernels<NC, UNIT>(e, R, Q, 1, grid, rc, e->stream) < 0)
+    if (round_batch_prep(e, first, n, grid, 1, rc, R, Q) < 0 || round_kernels<NC, UNIT>(e, R, Q, 1, grid, rc, e->stream.get()) < 0)
         return SW_E_CUDA;
     count_round_kernels(e, rc);
-    round_span(e, start, true);
+    round_span(e, start);
     return round_batch_finish<NC>(e, R);
 }
 
@@ -641,19 +731,19 @@ int divide_round_batch(sw_engine *e, int first, int n, cudaEvent_t start) {
 // the round stream's piece, which is given up (its rounds are computed again), and so are the round stream's copies.
 // (The round stream runs its pieces in order: waiting for the end of the last one waits for all of them.)
 int rs_drain(sw_engine *e) {
-    if (e->rs_synced && e->rdone) CK(cudaStreamWaitEvent(e->stream, e->rdone, 0));
+    if (e->rs_synced && e->rdone) CK(cudaStreamWaitEvent(e->stream.get(), e->rdone, 0));
     e->rs_synced = false;
     e->n_rounded = e->n_divided;
-    for (auto &p : e->rs_pieces) e->rs_free.push_back(p.done);
+    for (auto &p : e->rs_pieces) e->rs_free.push_back(std::move(p.done));
     e->rs_pieces.clear();
     return 0;
 }
 
 // the round stream and its prep stream go on after what the compute stream has been given so far
 int rs_follow(sw_engine *e) {
-    CK(cudaEventRecord(e->rwait, e->stream));
-    CK(cudaStreamWaitEvent(e->rstream, e->rwait, 0));
-    CK(cudaStreamWaitEvent(e->pstream, e->rwait, 0));
+    CK(cudaEventRecord(e->rwait.get(), e->stream.get()));
+    CK(cudaStreamWaitEvent(e->rstream.get(), e->rwait.get(), 0));
+    CK(cudaStreamWaitEvent(e->pstream.get(), e->rwait.get(), 0));
     return 0;
 }
 
@@ -661,18 +751,15 @@ int rs_follow(sw_engine *e) {
 int rs_sync(sw_engine *e) {
     if (e->rs_synced) return 0;
     if (rs_follow(e) < 0) return SW_E_CUDA;
-    CK(cudaMemcpyAsync(e->d_Wf2, e->d_Wf, sizeof(int32_t) * e->Rcap * e->M, cudaMemcpyDeviceToDevice, e->rstream));
-    CK(cudaMemcpyAsync(e->d_gchain2, e->d_gchain, sizeof(int32_t) * e->MP * RB_RING, cudaMemcpyDeviceToDevice, e->rstream));
-    CK(cudaMemcpyAsync(e->d_rscal, e->d_scal, sizeof(int32_t) * SC_COUNT, cudaMemcpyDeviceToDevice, e->rstream));
-    CK(cudaMemsetAsync(rb_meta(e).wcnt, 0, 2 * sizeof(int32_t), e->stream));
+    CK(cudaMemcpyAsync(e->d_Wf2.get(), e->d_Wf.get(), sizeof(int32_t) * e->Rcap * e->M, cudaMemcpyDeviceToDevice, e->rstream.get()));
+    CK(cudaMemcpyAsync(e->d_gchain2.get(), e->d_gchain.get(), sizeof(int32_t) * e->MP * RB_RING, cudaMemcpyDeviceToDevice, e->rstream.get()));
+    CK(cudaMemcpyAsync(e->d_rscal.get(), e->d_scal.get(), sizeof(int32_t) * SC_COUNT, cudaMemcpyDeviceToDevice, e->rstream.get()));
+    CK(cudaMemsetAsync(rb_meta(e->d_rbmeta.get(), e->MP).wcnt, 0, 2 * sizeof(int32_t), e->stream.get()));
     e->wslot = 0;
     e->n_rounded = e->n_divided;
     e->rs_synced = true;
     return 0;
 }
-
-// the size of one of the round stream's two meta blocks in d_rbmeta2
-size_t rs_meta_ints(const sw_engine *e) { return 4 * (size_t)e->MP + 64; }
 
 // Rounds of [first, first+n) on the round stream's meta, ring, Wf and scalars.  The caller has made `pstream` wait for the
 // piece's rows.  k_rb_prep runs there, into the buffers the piece before this one does not use, once the piece before
@@ -688,30 +775,28 @@ int rs_piece(sw_engine *e, int first, int n) {
     if (rsg_reserve(e, n, b) < 0) return SW_E_CUDA;
     const int grid = std::max(e->n_sm / 2, e->n_sm - 16);
     RbParams R = round_params(e, first, n, grid, 1);
-    int32_t *m = e->d_rbmeta2 + b * rs_meta_ints(e);
-    const int MP = e->MP;
-    R.ccnt = m; R.cmin = m + MP; R.coff = m + 2 * MP;
-    R.bar = reinterpret_cast<unsigned *>(m + 3 * MP + 8); R.wcnt = m + 3 * MP + 9; R.ctot = m + 3 * MP + 16;
-    R.gchain = e->d_gchain2; R.Wf = e->d_Wf2; R.scal = e->d_rscal;
+    const RbMeta m = rb_meta(e->d_rbmeta2.get() + b * rb_meta_ints(e->MP), e->MP);
+    use_meta(R, m);
+    R.ctot = m.ctot; R.gchain = e->d_gchain2.get(); R.Wf = e->d_Wf2.get(); R.scal = e->d_rscal.get();
     R.epoch = 0x80000000u | ++e->rs_epoch;
-    CK(cudaStreamWaitEvent(e->pstream, e->rs_bufdone[b], 0));
-    if (chunk_prep<64>(e, R, e->d_rsg[b], e->pstream) < 0) return SW_E_CUDA;
-    CK(cudaEventRecord(e->rs_prepped[b], e->pstream));
-    CK(cudaStreamWaitEvent(e->rstream, e->rs_prepped[b], 0));
-    const RcParams Q{R, e->d_rsg[b], e->d_rccont};
-    R.cont = e->d_rccont;
-    if (round_kernels<NC, UNIT>(e, R, Q, 1, grid, true, e->rstream) < 0) return SW_E_CUDA;
-    CK(cudaEventRecord(e->rs_bufdone[b], e->rstream));
-    cudaEvent_t done = nullptr;
-    if (!e->rs_free.empty()) { done = e->rs_free.back(); e->rs_free.pop_back(); }
-    else CK(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
-    e->rs_pieces.push_back({first + n, done});
-    CK(cudaEventRecord(done, e->rstream));
-    e->rdone = done;
+    CK(cudaStreamWaitEvent(e->pstream.get(), e->rs_bufdone[b].get(), 0));
+    if (chunk_prep<64>(e, R, e->d_rsg[b].get(), e->pstream.get()) < 0) return SW_E_CUDA;
+    CK(cudaEventRecord(e->rs_prepped[b].get(), e->pstream.get()));
+    CK(cudaStreamWaitEvent(e->rstream.get(), e->rs_prepped[b].get(), 0));
+    const RcParams Q{R, e->d_rsg[b].get(), e->d_rccont.get()};
+    R.cont = e->d_rccont.get();
+    if (round_kernels<NC, UNIT>(e, R, Q, 1, grid, true, e->rstream.get()) < 0) return SW_E_CUDA;
+    CK(cudaEventRecord(e->rs_bufdone[b].get(), e->rstream.get()));
+    Event done;
+    if (!e->rs_free.empty()) { done = std::move(e->rs_free.back()); e->rs_free.pop_back(); }
+    else CK(done.create());
+    e->rs_pieces.push_back({first + n, std::move(done)});
+    e->rdone = e->rs_pieces.back().done.get();
+    CK(cudaEventRecord(e->rdone, e->rstream.get()));
     RbRing G;
-    G.ring = e->d_gchain2; G.creator = e->d_creator; G.seq = e->d_seq; G.rfirst = first; G.rn = n;
+    G.ring = e->d_gchain2.get(); G.creator = e->d_creator.get(); G.seq = e->d_seq.get(); G.rfirst = first; G.rn = n;
     counts_at(e, first + n, G.ctot);
-    k_rb_ring<<<std::max(1, std::min(2 * e->n_sm, (n + 255) / 256)), 256, 0, e->rstream>>>(G);
+    k_rb_ring<<<std::max(1, std::min(2 * e->n_sm, (n + 255) / 256)), 256, 0, e->rstream.get()>>>(G);
     CK(cudaGetLastError());
     e->n_rounded = first + n;
     return 0;
@@ -748,24 +833,24 @@ int divide_ahead(sw_engine *e, int first, int n, int scan_from) {
     if (scan_from >= 0) {
         // (after the piece's k_rb_prep: its cluster kernel is then the first to claim the SMs the prep frees, and the
         //  scan takes what the cluster leaves)
-        if (cover) CK(cudaStreamWaitEvent(e->stream, e->rs_prepped[e->rs_buf ^ 1], 0));
+        if (cover) CK(cudaStreamWaitEvent(e->stream.get(), e->rs_prepped[e->rs_buf ^ 1].get(), 0));
         const i64 kl = e->stats.kernel_launches;
-        if (cansee_scan(e, e->stream, e->n_events, 5) < 0 || rows_written(e) < 0) return SW_E_CUDA;
+        if (cansee_scan(e, e->stream.get(), e->n_events, 5) < 0 || rows_written(e) < 0) return SW_E_CUDA;
         e->stats.kernel_launches = kl + cs_launches(e, scan_from, e->n_events - scan_from) - cs_launches(e, scan_from, end - scan_from);
     }
     // (the pieces are contiguous from n_divided and the last ends at n_rounded >= end: one of them holds the call's end)
     size_t k = 0;
     while (k + 1 < e->rs_pieces.size() && e->rs_pieces[k].end < end) k++;
     if (e->rs_pieces.empty() || e->rs_pieces[k].end < end) return fail(e, SW_E_CUDA, "divide_ahead: no piece holds the call's end");
-    CK(cudaStreamWaitEvent(e->stream, e->rs_pieces[k].done, 0));
+    CK(cudaStreamWaitEvent(e->stream.get(), e->rs_pieces[k].done.get(), 0));
     if (e->rs_pieces[k].end == end) k++;
-    for (size_t i = 0; i < k; i++) e->rs_free.push_back(e->rs_pieces[i].done);
+    for (size_t i = 0; i < k; i++) e->rs_free.push_back(std::move(e->rs_pieces[i].done));
     e->rs_pieces.erase(e->rs_pieces.begin(), e->rs_pieces.begin() + k);
-    const RbMeta m = rb_meta(e);
+    const RbMeta m = rb_meta(e->d_rbmeta.get(), e->MP);
     RbParams R = chunk_params(e, first, n);
-    R.SM = e->d_SM; R.wcnt = m.wcnt + e->wslot;
+    R.SM = e->d_SM.get(); R.wcnt = m.wcnt + e->wslot;
     RbFold F{};
-    F.on = 1; F.Wf = e->d_Wf; F.scal = e->d_scal; F.wnext = m.wcnt + (e->wslot ^ 1); F.rscal = e->d_rscal;
+    F.on = 1; F.Wf = e->d_Wf.get(); F.scal = e->d_scal.get(); F.wnext = m.wcnt + (e->wslot ^ 1); F.rscal = e->d_rscal.get();
     counts_at(e, end, F.ctot);
     e->wslot ^= 1;
     e->rb_epoch++;
@@ -775,8 +860,8 @@ int divide_ahead(sw_engine *e, int first, int n, int scan_from) {
     while (e->rs_pieces.size() < 2) {
         const int len = rs_ahead_len(e, n), next = e->n_rounded + len;
         if (len < e->rc_min_n) break;
-        for (auto &a : e->appends) if (a.base < next) CK(cudaStreamWaitEvent(e->pstream, a.done, 0));
-        if (e->scan_ev_set) CK(cudaStreamWaitEvent(e->pstream, e->scan_ev, 0));
+        for (auto &a : e->appends) if (a.base < next) CK(cudaStreamWaitEvent(e->pstream.get(), a.done.get(), 0));
+        if (e->scan_ev_set) CK(cudaStreamWaitEvent(e->pstream.get(), e->scan_ev.get(), 0));
         if (rs_piece<NC, UNIT>(e, e->n_rounded, len) < 0) return SW_E_CUDA;
     }
     return 0;
@@ -789,7 +874,7 @@ template <int NJ>
 int divide_rounds_wide(sw_engine *e, int first, int n) {
     const int M = e->M;
     const RbParams T = chunk_params(e, first, n);       // the grouping and the finish kernel shared with the M <= 64 path
-    if (chunk_prep<SW_MAX_MEMBERS>(e, T, nullptr, e->stream) < 0) return SW_E_CUDA;
+    if (chunk_prep<SW_MAX_MEMBERS>(e, T, nullptr, e->stream.get()) < 0) return SW_E_CUDA;
     e->stats.kernel_launches += 1;
     RwParams R{};
     R.M = M; R.first = first; R.n = n; R.Rcap = e->Rcap;
@@ -798,12 +883,12 @@ int divide_rounds_wide(sw_engine *e, int first, int n) {
     // events per member below a step's frontier: about three tests per warp and step, never more than half a window
     R.L = std::max(1, std::min(RW_LMAX / 2, 3 * nw * e->nranks / std::max(1, M)));
     R.epoch = ++e->rb_epoch;
-    R.row = e->d_row; R.p0 = e->d_p0; R.creator = e->d_creator; R.seq = e->d_seq; R.round = e->d_round;
-    R.Wf = e->d_Wf; R.scw = e->d_scw; R.sctag = e->d_sctag; R.cev = T.cev;
-    R.cmin = T.cmin; R.coff = T.coff; R.bar = T.bar; R.ticket = rb_meta(e).ticket;
-    R.ctot = T.ctot; R.gchain = T.gchain; R.hitmin = e->d_hitmin;
-    R.stake = e->d_stake; R.tot2 = 2 * e->tot; R.unit = e->unit ? 1 : 0; R.scal = e->d_scal; R.dbg = e->d_dbg;
-    R.rank = e->rank; R.nranks = e->nranks; R.xstep = e->d_xstep;
+    R.row = e->d_row.get(); R.p0 = e->d_p0.get(); R.creator = e->d_creator.get(); R.seq = e->d_seq.get(); R.round = e->d_round.get();
+    R.Wf = e->d_Wf.get(); R.scw = e->d_scw.get(); R.sctag = e->d_sctag.get(); R.cev = T.cev;
+    R.cmin = T.cmin; R.coff = T.coff; R.bar = T.bar; R.ticket = rb_meta(e->d_rbmeta.get(), e->MP).ticket;
+    R.ctot = T.ctot; R.gchain = T.gchain; R.hitmin = e->d_hitmin.get();
+    R.stake = e->d_stake.get(); R.tot2 = 2 * e->tot; R.unit = e->unit ? 1 : 0; R.scal = e->d_scal.get(); R.dbg = e->d_dbg.get();
+    R.rank = e->rank; R.nranks = e->nranks; R.xstep = e->d_xstep.get();
     for (int p = 0; p < e->nranks && p < 8; p++) {
         R.xflag[p] = reinterpret_cast<unsigned *>(e->x_peer[p]);
         R.xhit[p] = reinterpret_cast<u64 *>(reinterpret_cast<char *>(e->x_peer[p]) + 256);
@@ -812,23 +897,23 @@ int divide_rounds_wide(sw_engine *e, int first, int n) {
     CK(cudaFuncSetAttribute(k_rounds_wide<NJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     void *args[] = {(void *)&R};
     {
-        cudaEvent_t a = get_event(e), b = get_event(e);
-        cudaEventRecord(a, e->stream);
-        CK(cudaLaunchCooperativeKernel((void *)k_rounds_wide<NJ>, dim3(grid), dim3(RW_THREADS), args, smem, e->stream));
-        cudaEventRecord(b, e->stream);
-        e->spans.push_back(TimedSpan{a, b, 4});
+        Event a = get_event(e), b = get_event(e);
+        cudaEventRecord(a.get(), e->stream.get());
+        CK(cudaLaunchCooperativeKernel((void *)k_rounds_wide<NJ>, dim3(grid), dim3(RW_THREADS), args, smem, e->stream.get()));
+        cudaEventRecord(b.get(), e->stream.get());
+        add_span(e, std::move(a), std::move(b), 4);
     }
-    k_rb_finish<<<std::max(1, std::min(2 * e->n_sm, (n + 255) / 256)), 256, 0, e->stream>>>(T, RbFold{});
-    k_w_seenmask<NJ><<<std::max(1, std::min(8 * e->n_sm, (n + 7) / 8)), 256, 0, e->stream>>>(M, first, n, e->Rcap, e->d_row, e->d_round, e->d_W, e->d_SMw);
+    k_rb_finish<<<std::max(1, std::min(2 * e->n_sm, (n + 255) / 256)), 256, 0, e->stream.get()>>>(T, RbFold{});
+    k_w_seenmask<NJ><<<std::max(1, std::min(8 * e->n_sm, (n + 7) / 8)), 256, 0, e->stream.get()>>>(M, first, n, e->Rcap, e->d_row.get(), e->d_round.get(), e->d_W.get(), e->d_SMw.get());
     CK(cudaGetLastError());
     StrongParams Q{};
-    Q.M = M; Q.first = first; Q.n = n; Q.Rcap = e->Rcap; Q.creator = e->d_creator; Q.row = e->d_row;
-    Q.round = e->d_round; Q.wit = e->d_wit; Q.stake = e->d_stake; Q.tot2 = 2 * e->tot;
-    Q.coin = e->d_coin; Q.sig = e->d_sig; Q.unit = e->unit ? 1 : 0; Q.list = T.wlist; Q.list_n = T.wcnt;
-    Q.SMw = e->d_SMw; Q.Sw = e->d_Sw;
+    Q.M = M; Q.first = first; Q.n = n; Q.Rcap = e->Rcap; Q.creator = e->d_creator.get(); Q.row = e->d_row.get();
+    Q.round = e->d_round.get(); Q.wit = e->d_wit.get(); Q.stake = e->d_stake.get(); Q.tot2 = 2 * e->tot;
+    Q.coin = e->d_coin.get(); Q.sig = e->d_sig.get(); Q.unit = e->unit ? 1 : 0; Q.list = T.wlist; Q.list_n = T.wcnt;
+    Q.SMw = e->d_SMw.get(); Q.Sw = e->d_Sw.get();
     const size_t ssm = (size_t)(2 * M + 8 * M) * sizeof(int);
     CK(cudaFuncSetAttribute(k_w_strong<NJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssm));
-    k_w_strong<NJ><<<std::max(1, std::min(4 * e->n_sm, (n + 7) / 8)), 256, ssm, e->stream>>>(Q);
+    k_w_strong<NJ><<<std::max(1, std::min(4 * e->n_sm, (n + 7) / 8)), 256, ssm, e->stream.get()>>>(Q);
     CK(cudaGetLastError());
     e->stats.kernel_launches += 4;
     return 0;
@@ -839,7 +924,7 @@ size_t w_fame_smem(int NJ, int M) { return (size_t)(32 * NJ + 64) * sizeof(int) 
 template <int NJ, class Src>
 int fame_rounds_wide(sw_engine *e, Src P, int B) {
     const int parts = (e->M + FW_THREADS - 1) / FW_THREADS;
-    k_w_fame_rounds<NJ><<<dim3((2 * e->n_sm / parts + 1) * parts, B), FW_THREADS, w_fame_smem(NJ, e->M), e->stream>>>(P);
+    k_w_fame_rounds<NJ><<<dim3((2 * e->n_sm / parts + 1) * parts, B), FW_THREADS, w_fame_smem(NJ, e->M), e->stream.get()>>>(P);
     return 0;
 }
 
@@ -848,12 +933,12 @@ int fame_rounds_wide(sw_engine *e, Src P, int B) {
 template <class Src>
 void fame_kernels(sw_engine *e, Src P, int B) {
     if (e->wide) {
-        k_fame_begin<<<dim3(1, B), 32, 0, e->stream>>>(P);
+        k_fame_begin<<<dim3(1, B), 32, 0, e->stream.get()>>>(P);
         SW_NJ(fame_rounds_wide, e, P, B);
-        k_fame_finish<<<dim3(1, B), 1024, 0, e->stream>>>(P);
+        k_fame_finish<<<dim3(1, B), 1024, 0, e->stream.get()>>>(P);
         e->stats.kernel_launches += 3;
     } else {
-        k_fame_rounds<<<dim3(2 * e->n_sm, B), 256, 0, e->stream>>>(P);
+        k_fame_rounds<<<dim3(2 * e->n_sm, B), 256, 0, e->stream.get()>>>(P);
         e->stats.kernel_launches += 1;
     }
 }
@@ -877,11 +962,11 @@ size_t scal_room(const sw_engine *e) { return (size_t)std::max(e->Rcap, 4 * ORDE
 int fame_result(sw_engine *e, int32_t *out, int cap, int &r) {
     r = device_error(e);
     if (r < 0) return 0;
-    const int cnt = e->h_scal[SC_NEWC];
+    const int cnt = e->h_scal.get()[SC_NEWC];
     if (cnt > cap) { r = fail(e, SW_E_ARG, "decide_fame: %d new consensus rounds do not fit cap=%d", cnt, cap); return 0; }
     if (cnt > fame_spec(e)) {
-        CK(cudaMemcpyAsync(e->h_newc, e->d_newc, sizeof(int32_t) * cnt, cudaMemcpyDeviceToHost, e->stream));
-        CK(cudaStreamSynchronize(e->stream));
+        CK(cudaMemcpyAsync(e->h_newc, e->d_newc, sizeof(int32_t) * cnt, cudaMemcpyDeviceToHost, e->stream.get()));
+        CK(cudaStreamSynchronize(e->stream.get()));
         e->stats.d2h_bytes += sizeof(int32_t) * cnt;
     }
     if (cnt > 0) memcpy(out, e->h_newc, sizeof(int32_t) * cnt);
@@ -891,37 +976,31 @@ int fame_result(sw_engine *e, int32_t *out, int cap, int &r) {
 
 FameParams fame_params(const sw_engine *e) {
     FameParams P{};
-    P.M = e->M; P.Rcap = e->Rcap; P.C = e->C; P.W = e->d_W; P.S = e->d_S; P.famous = e->d_famous;
-    P.famous_ev = e->d_famous_ev; P.consensus = e->d_consensus; P.done = e->d_done; P.rem = e->d_rem;
-    P.coin = e->d_coin; P.stake = e->d_stake; P.tot2 = 2 * e->tot; P.unit = e->unit ? 1 : 0; P.newc = e->d_newc; P.scal = e->d_scal;
-    P.Sw = e->d_Sw;
+    P.M = e->M; P.Rcap = e->Rcap; P.C = e->C; P.W = e->d_W.get(); P.S = e->d_S.get(); P.famous = e->d_famous.get();
+    P.famous_ev = e->d_famous_ev.get(); P.consensus = e->d_consensus.get(); P.done = e->d_done.get(); P.rem = e->d_rem.get();
+    P.coin = e->d_coin.get(); P.stake = e->d_stake.get(); P.tot2 = 2 * e->tot; P.unit = e->unit ? 1 : 0; P.newc = e->d_newc; P.scal = e->d_scal.get();
+    P.Sw = e->d_Sw.get();
     return P;
 }
 
 // find_order's per-round scratch, grown on demand to n rounds
+size_t seg_cap(const sw_engine *e) { return e->d_seg_nf.cap(); }
 int order_scratch(sw_engine *e, int n) {
-    if (n <= e->seg_cap) return 0;
-    const size_t MS = e->MS;
-    int nc = std::max(n, std::max(64, 2 * e->seg_cap));
-    for (void *p : {(void *)e->d_seg_start, (void *)e->d_seg_fw, (void *)e->d_seg_nf, (void *)e->d_seg_white, (void *)e->d_rounds_in, (void *)e->d_plan})
-        if (p) cudaFree(p);
-    CK(dalloc(&e->d_seg_start, (size_t)nc + 1)); CK(dalloc(&e->d_seg_fw, (size_t)nc * MS));
-    CK(dalloc(&e->d_seg_nf, (size_t)nc)); CK(dalloc(&e->d_seg_white, (size_t)nc * 64));
-    CK(dalloc(&e->d_rounds_in, (size_t)nc)); CK(dalloc(&e->d_plan, (size_t)nc * MS * 8));
-    e->seg_cap = nc;
-    return 0;
+    const size_t nc = std::max<size_t>(n, std::max<size_t>(64, 2 * seg_cap(e))), MS = e->MS;
+    return grow(e, n, seg_cap(e), sized(e->d_seg_start, nc + 1), sized(e->d_seg_fw, nc * MS), sized(e->d_seg_nf, nc),
+                sized(e->d_seg_white, nc * 64), sized(e->d_rounds_in, nc), sized(e->d_plan, nc * MS * 8));
 }
 
 // find_order over the n sorted rounds at `rounds` (device memory)
 OrderParams order_params(const sw_engine *e, int n, const int32_t *rounds) {
     OrderParams P{};
-    P.M = e->M; P.Rcap = e->Rcap; P.nrounds = n; P.rounds = rounds; P.W = e->d_W; P.famous = e->d_famous;
-    P.row = e->d_row; P.p0 = e->d_p0; P.creator = e->d_creator; P.seq = e->d_seq; P.t = e->d_t; P.sig = e->d_sig;
-    P.stake = e->d_stake; P.tot = e->tot; P.lastord = e->d_lastord; P.batch_ev = e->d_batch_ev; P.batch_seg = e->d_batch_seg;
-    P.seg_start = e->d_seg_start; P.seg_fw = e->d_seg_fw; P.seg_nf = e->d_seg_nf; P.seg_white = e->d_seg_white;
-    P.ts = e->d_ts; P.key = e->d_key; P.perm = e->d_perm; P.tx = e->d_tx; P.tx_cap = e->cap;
-    P.idx = e->d_idx; P.tx_base = e->n_tx; P.scal = e->d_scal; P.out_n = 0;
-    P.plan = e->d_plan; P.plan_stride = (int)(e->seg_cap * e->MS);
+    P.M = e->M; P.Rcap = e->Rcap; P.nrounds = n; P.rounds = rounds; P.W = e->d_W.get(); P.famous = e->d_famous.get();
+    P.row = e->d_row.get(); P.p0 = e->d_p0.get(); P.creator = e->d_creator.get(); P.seq = e->d_seq.get(); P.t = e->d_t.get(); P.sig = e->d_sig.get();
+    P.stake = e->d_stake.get(); P.tot = e->tot; P.lastord = e->d_lastord.get(); P.batch_ev = e->d_batch_ev.get(); P.batch_seg = e->d_batch_seg.get();
+    P.seg_start = e->d_seg_start.get(); P.seg_fw = e->d_seg_fw.get(); P.seg_nf = e->d_seg_nf.get(); P.seg_white = e->d_seg_white.get();
+    P.ts = e->d_ts.get(); P.key = e->d_key.get(); P.perm = e->d_perm.get(); P.tx = e->d_tx.get(); P.tx_cap = e->cap;
+    P.idx = e->d_idx.get(); P.tx_base = e->n_tx; P.scal = e->d_scal.get(); P.out_n = 0;
+    P.plan = e->d_plan.get(); P.plan_stride = (int)(seg_cap(e) * e->MS);
     return P;
 }
 
@@ -941,17 +1020,17 @@ void order_kernels(sw_engine *e, Src P, int A, int maxn) {
     const int M = e->M;
     const int list_ctas = std::max(1, std::min(4 * e->n_sm, (int)(((size_t)maxn * e->MS + 255) / 256)));
     if (e->wide) {
-        k_w_order_rounds<<<dim3(maxn, A), 1024, (size_t)3 * M * sizeof(int), e->stream>>>(P);
-        k_w_order_cuts<<<dim3(1, A), 1024, (size_t)2 * M * sizeof(int), e->stream>>>(P);
-        k_w_order_list<<<dim3(list_ctas, A), 256, 0, e->stream>>>(P);
-        k_w_order_times<<<dim3(8 * e->n_sm, A), OW_WARPS * 32, (size_t)OW_WARPS * M * sizeof(u64), e->stream>>>(P);
+        k_w_order_rounds<<<dim3(maxn, A), 1024, (size_t)3 * M * sizeof(int), e->stream.get()>>>(P);
+        k_w_order_cuts<<<dim3(1, A), 1024, (size_t)2 * M * sizeof(int), e->stream.get()>>>(P);
+        k_w_order_list<<<dim3(list_ctas, A), 256, 0, e->stream.get()>>>(P);
+        k_w_order_times<<<dim3(8 * e->n_sm, A), OW_WARPS * 32, (size_t)OW_WARPS * M * sizeof(u64), e->stream.get()>>>(P);
     } else {
-        k_order_rounds<<<dim3(maxn, A), 1024, 0, e->stream>>>(P);
-        k_order_cuts<<<dim3(1, A), 64, 0, e->stream>>>(P);
-        k_order_list<<<dim3(list_ctas, A), 256, 0, e->stream>>>(P);
-        k_order_times<<<dim3(4 * e->n_sm, A), 256, 0, e->stream>>>(P);
+        k_order_rounds<<<dim3(maxn, A), 1024, 0, e->stream.get()>>>(P);
+        k_order_cuts<<<dim3(1, A), 64, 0, e->stream.get()>>>(P);
+        k_order_list<<<dim3(list_ctas, A), 256, 0, e->stream.get()>>>(P);
+        k_order_times<<<dim3(4 * e->n_sm, A), 256, 0, e->stream.get()>>>(P);
     }
-    k_order_sort<<<dim3(maxn, A), 1024, 0, e->stream>>>(P);
+    k_order_sort<<<dim3(maxn, A), 1024, 0, e->stream.get()>>>(P);
     e->stats.kernel_launches += 5;
 }
 
@@ -959,7 +1038,7 @@ void order_kernels(sw_engine *e, Src P, int A, int maxn) {
 int order_result(sw_engine *e) {
     const int rc = device_error(e);
     if (rc < 0) return rc;
-    const int nbatch = e->h_scal[SC_BATCH];
+    const int nbatch = e->h_scal.get()[SC_BATCH];
     e->n_tx += nbatch;
     return nbatch;
 }
@@ -972,7 +1051,7 @@ int order_output(sw_engine *e, cudaStream_t s, int base, int cnt, const OrderOut
     for (int i = 0; i < k; i++) { ev[i] = st[i].ev; ts[i] = st[i].ts; rr[i] = st[i].rr; }
     if (cnt > k) {
         const size_t n = cnt - k, at = (size_t)base + k;
-        CK(cudaMemcpyAsync(ev + k, e->d_tx + at, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(ev + k, e->d_tx.get() + at, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(ts + k, e->d_tx_ts + at, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(rr + k, e->d_tx_rr + at, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s));
     }
@@ -1003,15 +1082,8 @@ int check_views(sw_engine *const *engines, int B, const char *what, bool same_sh
 
 // the per-call block of the first engine: at least `bytes` on the device and in pinned host memory
 int views_buffer(sw_engine *e, size_t bytes) {
-    if (bytes <= e->vbuf_bytes) return 0;
-    if (e->d_vbuf) { CK(cudaFree(e->d_vbuf)); e->d_vbuf = nullptr; }
-    if (e->h_vbuf) { CK(cudaFreeHost(e->h_vbuf)); e->h_vbuf = nullptr; }
-    const size_t want = std::max(bytes, 2 * e->vbuf_bytes);
-    e->vbuf_bytes = 0;
-    CK(cudaMalloc((void **)&e->d_vbuf, want));
-    CK(cudaMallocHost((void **)&e->h_vbuf, want));
-    e->vbuf_bytes = want;
-    return 0;
+    const size_t want = std::max(bytes, 2 * e->d_vbuf.cap());
+    return grow(e, bytes, e->d_vbuf.cap(), sized(e->d_vbuf, want), sized(e->h_vbuf, want));
 }
 
 size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
@@ -1020,19 +1092,11 @@ size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 // larger ring replaces the ring after the copies and kernels that read it).  Returns the slot's index (< 0: an error);
 // the caller records stage_ev[slot] on the copy stream after its copy.
 int stage_slot(sw_engine *e, size_t bytes) {
-    if (bytes > e->stage_bytes) {
-        CK(cudaStreamSynchronize(e->copy_stream));
-        if (e->h_stage) { CK(cudaFreeHost(e->h_stage)); e->h_stage = nullptr; }
-        if (e->d_stage) { CK(cudaFree(e->d_stage)); e->d_stage = nullptr; }
-        const size_t slot = align256(std::max(bytes, 2 * e->stage_bytes));
-        e->stage_bytes = 0;
-        CK(cudaMallocHost((void **)&e->h_stage, slot * sw_engine::STAGE_SLOTS));
-        CK(cudaMalloc((void **)&e->d_stage, slot * sw_engine::STAGE_SLOTS));
-        e->stage_bytes = slot;
-    }
+    const size_t ring = align256(std::max(bytes, 2 * e->stage_bytes())) * sw_engine::STAGE_SLOTS;
+    if (grow(e, bytes, e->stage_bytes(), sized(e->h_stage, ring), sized(e->d_stage, ring)) < 0) return SW_E_CUDA;
     const int si = e->stage_next;
     e->stage_next = (si + 1) % sw_engine::STAGE_SLOTS;
-    CK(cudaEventSynchronize(e->stage_ev[si]));
+    CK(cudaEventSynchronize(e->stage_ev[si].get()));
     return si;
 }
 
@@ -1041,21 +1105,20 @@ int views_enter(sw_engine *e, sw_engine *const *views, int B) {
     for (int v = 0; v < B; v++) {
         sw_engine *x = views[v];
         if (x == e) continue;
-        cudaEvent_t ev = get_event(x);
-        CK(cudaEventRecord(ev, x->stream));
-        CK(cudaStreamWaitEvent(e->stream, ev, 0));
-        x->pool.push_back(ev);
+        Event ev = get_event(x);
+        CK(cudaEventRecord(ev.get(), x->stream.get()));
+        CK(cudaStreamWaitEvent(e->stream.get(), ev.get(), 0));
+        x->pool.push_back(std::move(ev));
     }
     return 0;
 }
 
 // ... and each view's next call runs after the batch; then the one copy of the gathered scalars and the one synchronisation
 int views_leave(sw_engine *e, sw_engine *const *views, int B, void *h_dst, const void *d_src, size_t bytes) {
-    if (!e->view_ev) CK(cudaEventCreateWithFlags(&e->view_ev, cudaEventDisableTiming));
-    CK(cudaEventRecord(e->view_ev, e->stream));
-    for (int v = 0; v < B; v++) if (views[v] != e) CK(cudaStreamWaitEvent(views[v]->stream, e->view_ev, 0));
-    CK(cudaMemcpyAsync(h_dst, d_src, bytes, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaEventRecord(e->view_ev.get(), e->stream.get()));
+    for (int v = 0; v < B; v++) if (views[v] != e) CK(cudaStreamWaitEvent(views[v]->stream.get(), e->view_ev.get(), 0));
+    CK(cudaMemcpyAsync(h_dst, d_src, bytes, cudaMemcpyDeviceToHost, e->stream.get()));
+    CK(cudaStreamSynchronize(e->stream.get()));
     e->stats.d2h_bytes += bytes;
     return 0;
 }
@@ -1099,39 +1162,37 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
     e->h_stale_cum.assign(1, 0);
     int rc = [&]() -> int {
         CK(cudaSetDevice(device));
-        CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
-        CK(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-        CK(cudaEventCreateWithFlags(&e->scan_ev, cudaEventDisableTiming));
+        CK(e->stream.create()); CK(e->copy_stream.create());
+        CK(e->scan_ev.create()); CK(e->view_ev.create());
+        for (Event &ev : e->stage_ev) CK(ev.create());
         const size_t cap = e->cap, RM = (size_t)e->Rcap * M, MP = e->MP;
-        CK(cudaMallocHost((void **)&e->h_height, sizeof(int32_t) * cap));
-        CK(cudaMallocHost((void **)&e->h_seq, sizeof(int32_t) * cap));
-        CK(cudaMallocHost((void **)&e->h_stale, cap));
-        CK(dalloc(&e->d_p0, cap)); CK(dalloc(&e->d_p1, cap)); CK(dalloc(&e->d_creator, cap)); CK(dalloc(&e->d_seq, cap));
-        CK(dalloc(&e->d_t, cap)); CK(dalloc(&e->d_sig, cap * 64)); CK(dalloc(&e->d_height, cap)); CK(dalloc(&e->d_stale, cap));
+        CK(e->h_height.alloc(cap)); CK(e->h_seq.alloc(cap)); CK(e->h_stale.alloc(cap));
+        CK(e->d_p0.alloc(cap)); CK(e->d_p1.alloc(cap)); CK(e->d_creator.alloc(cap)); CK(e->d_seq.alloc(cap));
+        CK(e->d_t.alloc(cap)); CK(e->d_sig.alloc(cap * 64)); CK(e->d_height.alloc(cap)); CK(e->d_stale.alloc(cap));
         // can_see scan scratch: per-event meta / flags / slow list, per-block tables (blocks are >= cs_min_B events)
         e->cs_min_B = std::max(256, std::min((M <= 64 ? 16 : 32) * M, 1 << 15));
         const size_t nbmax = cap / e->cs_min_B + 3;
-        CK(dalloc(&e->d_cs_meta, cap)); CK(dalloc(&e->d_cs_wr, cap)); CK(dalloc(&e->d_cs_xb, cap)); CK(dalloc(&e->d_cs_slow, cap + 4));
-        CK(dalloc(&e->d_cs_last, nbmax * M)); CK(dalloc(&e->d_cs_Q, (nbmax + 1) * M)); CK(dalloc(&e->d_cs_slowcnt, (size_t)4)); CK(dalloc(&e->d_cs_sflag, cap)); CK(dalloc(&e->d_cs_xlist, cap + 4)); CK(dalloc(&e->d_cs_slowblk, cap + 4)); CK(dalloc(&e->d_cs_blkcnt, nbmax + 1));
-        CK(dalloc(&e->d_cs_carry, MP));
-        CK(dalloc(&e->d_Wf, RM)); CK(dalloc(&e->d_cev, 2 * cap)); /* + the witness list of the current chunk */
-        CK(dalloc(&e->d_rbmeta, std::max<size_t>(256, 3 * MP + 64)));
-        CK(dalloc(&e->d_rbtot, MP)); CK(dalloc(&e->d_gchain, MP * RB_RING));
+        CK(e->d_cs_meta.alloc(cap)); CK(e->d_cs_wr.alloc(cap)); CK(e->d_cs_xb.alloc(cap)); CK(e->d_cs_slow.alloc(cap + 4));
+        CK(e->d_cs_last.alloc(nbmax * M)); CK(e->d_cs_Q.alloc((nbmax + 1) * M)); CK(e->d_cs_slowcnt.alloc(4)); CK(e->d_cs_sflag.alloc(cap)); CK(e->d_cs_xlist.alloc(cap + 4)); CK(e->d_cs_slowblk.alloc(cap + 4)); CK(e->d_cs_blkcnt.alloc(nbmax + 1));
+        CK(e->d_cs_carry.alloc(MP));
+        CK(e->d_Wf.alloc(RM)); CK(e->d_cev.alloc(2 * cap)); /* + the witness list of the current chunk */
+        CK(e->d_rbmeta.alloc(rb_meta_ints(e->MP)));
+        CK(e->d_rbtot.alloc(MP)); CK(e->d_gchain.alloc(MP * RB_RING));
         CK(cudaDeviceGetAttribute(&e->n_sm, cudaDevAttrMultiProcessorCount, device));
-        CK(dalloc(&e->d_dbg, (size_t)40)); CK(cudaMemsetAsync(e->d_dbg, 0, sizeof(long long) * 40, e->stream));
-        CK(dalloc(&e->d_row, cap * M));
+        CK(e->d_dbg.alloc(40)); CK(cudaMemsetAsync(e->d_dbg.get(), 0, sizeof(long long) * 40, e->stream.get()));
+        CK(e->d_row.alloc(cap * M));
         if (e->wide) {
-            CK(dalloc(&e->d_scw, cap * e->NJ)); CK(dalloc(&e->d_sctag, cap)); CK(dalloc(&e->d_SMw, cap * e->NJ));
-            CK(dalloc(&e->d_Sw, RM * e->NJ)); CK(dalloc(&e->d_hitmin, (size_t)3 * M));
-            CK(cudaMalloc(&e->d_xbuf, 256 + (size_t)8 * 3 * M * sizeof(u64)));
-            CK(cudaMemsetAsync(e->d_xbuf, 0, 256 + (size_t)8 * 3 * M * sizeof(u64), e->stream));
-            CK(dalloc(&e->d_xstep, (size_t)1)); CK(cudaMemsetAsync(e->d_xstep, 0, sizeof(unsigned), e->stream));
-            e->x_peer[0] = e->d_xbuf;
+            CK(e->d_scw.alloc(cap * e->NJ)); CK(e->d_sctag.alloc(cap)); CK(e->d_SMw.alloc(cap * e->NJ));
+            CK(e->d_Sw.alloc(RM * e->NJ)); CK(e->d_hitmin.alloc((size_t)3 * M));
+            CK(e->d_xbuf.alloc(256 + (size_t)8 * 3 * M * sizeof(u64)));
+            CK(cudaMemsetAsync(e->d_xbuf.get(), 0, 256 + (size_t)8 * 3 * M * sizeof(u64), e->stream.get()));
+            CK(e->d_xstep.alloc(1)); CK(cudaMemsetAsync(e->d_xstep.get(), 0, sizeof(unsigned), e->stream.get()));
+            e->x_peer[0] = e->d_xbuf.get();
         } else {
-            CK(dalloc(&e->d_sc, cap)); CK(dalloc(&e->d_res, (size_t)2 * 64 * RB_LMAX));
-            CK(dalloc(&e->d_SM, cap)); CK(dalloc(&e->d_S, RM));
+            CK(e->d_sc.alloc(cap)); CK(e->d_res.alloc((size_t)2 * 64 * RB_LMAX));
+            CK(e->d_SM.alloc(cap)); CK(e->d_S.alloc(RM));
             // the cluster round kernel: 16 CTAs with ~174 KB of shared memory each must fit one GPC
-            CK(dalloc(&e->d_rccont, (size_t)132)); CK(cudaMemsetAsync(e->d_rccont, 0, sizeof(int32_t) * 132, e->stream));
+            CK(e->d_rccont.alloc(132)); CK(cudaMemsetAsync(e->d_rccont.get(), 0, sizeof(int32_t) * 132, e->stream.get()));
             bool want = true;
             if (const char *v = getenv("SW_ROUNDS_CLUSTER")) want = atoi(v) != 0;
             if (const char *v = getenv("SW_RC_MIN_N")) e->rc_min_n = std::max(1, atoi(v));
@@ -1144,35 +1205,29 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
             e->ahead = e->rc_ok;
             if (const char *v = getenv("SW_ROUNDS_AHEAD")) e->ahead = e->ahead && atoi(v) != 0;
             if (e->ahead) {
-                CK(cudaStreamCreateWithFlags(&e->rstream, cudaStreamNonBlocking));
-                CK(cudaStreamCreateWithFlags(&e->pstream, cudaStreamNonBlocking));
-                CK(cudaEventCreateWithFlags(&e->rwait, cudaEventDisableTiming));
-                for (int b = 0; b < 2; b++) {
-                    CK(cudaEventCreateWithFlags(&e->rs_prepped[b], cudaEventDisableTiming));
-                    CK(cudaEventCreateWithFlags(&e->rs_bufdone[b], cudaEventDisableTiming));
-                }
-                CK(dalloc(&e->d_Wf2, RM)); CK(dalloc(&e->d_gchain2, MP * RB_RING));
-                CK(dalloc(&e->d_rbmeta2, 2 * rs_meta_ints(e))); CK(dalloc(&e->d_rscal, (size_t)SC_COUNT));
+                CK(e->rstream.create()); CK(e->pstream.create()); CK(e->rwait.create());
+                for (int b = 0; b < 2; b++) { CK(e->rs_prepped[b].create()); CK(e->rs_bufdone[b].create()); }
+                CK(e->d_Wf2.alloc(RM)); CK(e->d_gchain2.alloc(MP * RB_RING));
+                CK(e->d_rbmeta2.alloc(2 * rb_meta_ints(e->MP))); CK(e->d_rscal.alloc(SC_COUNT));
             }
         }
-        CK(dalloc(&e->d_round, cap)); CK(dalloc(&e->d_wit, cap)); CK(dalloc(&e->d_famous_ev, cap));
-        CK(dalloc(&e->d_W, RM)); CK(dalloc(&e->d_famous, RM));
-        CK(dalloc(&e->d_consensus, (size_t)e->Rcap)); CK(dalloc(&e->d_done, (size_t)e->Rcap)); CK(dalloc(&e->d_coin, RM));
-        CK(dalloc(&e->d_rem, (size_t)e->Rcap));
-        CK(dalloc(&e->d_stake, (size_t)M)); CK(dalloc(&e->d_scal, (size_t)SC_COUNT + scal_room(e)));
-        e->d_newc = e->d_scal + SC_COUNT;                  // (sw_decide_fame copies the scalars and the new rounds at once)
-        CK(dalloc(&e->d_lastord, MP)); CK(dalloc(&e->d_tx, 4 * cap)); CK(dalloc(&e->d_idx, cap));
-        e->d_tx_rr = e->d_tx + cap;                        // (one block: OrderParams finds both from d_tx and cap)
-        e->d_tx_ts = reinterpret_cast<double *>(e->d_tx + 2 * cap);
-        CK(dalloc(&e->d_batch_ev, cap)); CK(dalloc(&e->d_batch_seg, cap)); CK(dalloc(&e->d_perm, 2 * cap));
-        CK(dalloc(&e->d_ts, cap)); CK(dalloc(&e->d_key, cap * 8));
-        for (auto &ev : e->stage_ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        CK(e->d_round.alloc(cap)); CK(e->d_wit.alloc(cap)); CK(e->d_famous_ev.alloc(cap));
+        CK(e->d_W.alloc(RM)); CK(e->d_famous.alloc(RM));
+        CK(e->d_consensus.alloc(e->Rcap)); CK(e->d_done.alloc(e->Rcap)); CK(e->d_coin.alloc(RM));
+        CK(e->d_rem.alloc(e->Rcap));
+        CK(e->d_stake.alloc(M)); CK(e->d_scal.alloc(SC_COUNT + scal_room(e)));
+        e->d_newc = e->d_scal.get() + SC_COUNT;                  // (sw_decide_fame copies the scalars and the new rounds at once)
+        CK(e->d_lastord.alloc(MP)); CK(e->d_tx.alloc(4 * cap)); CK(e->d_idx.alloc(cap));
+        e->d_tx_rr = e->d_tx.get() + cap;                        // (one block: OrderParams finds both from d_tx and cap)
+        e->d_tx_ts = reinterpret_cast<double *>(e->d_tx.get() + 2 * cap);
+        CK(e->d_batch_ev.alloc(cap)); CK(e->d_batch_seg.alloc(cap)); CK(e->d_perm.alloc(2 * cap));
+        CK(e->d_ts.alloc(cap)); CK(e->d_key.alloc(cap * 8));
         if (stage_slot(e, unpack_bytes(sw_engine::STAGE_EVENTS)) < 0) return SW_E_CUDA;   // (the ring, sized for sw_append)
         CK(cudaFuncSetAttribute(k_stream_divide<true, StreamParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
         CK(cudaFuncSetAttribute(k_stream_divide<true, const StreamParams *>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
-        CK(cudaMallocHost((void **)&e->h_scal, sizeof(int32_t) * ((size_t)SC_COUNT + scal_room(e))));
-        e->h_newc = e->h_scal + SC_COUNT;
-        CK(cudaMemcpyAsync(e->d_stake, e->h_stake.data(), sizeof(i64) * M, cudaMemcpyHostToDevice, e->stream));
+        CK(e->h_scal.alloc(SC_COUNT + scal_room(e)));
+        e->h_newc = e->h_scal.get() + SC_COUNT;
+        CK(cudaMemcpyAsync(e->d_stake.get(), e->h_stake.data(), sizeof(i64) * M, cudaMemcpyHostToDevice, e->stream.get()));
         // kernels that need more than the default 48 KB of dynamic shared memory: the limit is a property of the kernel in
         // the whole process, so it is what the largest member count needs, whatever M this engine has
         const size_t cs_smem = (size_t)(SW_MAX_MEMBERS + CS_SV) * CS_CT * sizeof(int) + CS_TILE * sizeof(int4) + 3 * CS_TILE;
@@ -1208,21 +1263,21 @@ int append_validate(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, c
     for (int j = 0; j < n && rc == SW_OK; j++) {
         const int i = base + j, c = creator[j], a = p0[j], b = p1[j];
         if (c < 0 || c >= e->M) { rc = fail(e, SW_E_ARG, "event %d: creator %d out of range", i, c); break; }
-        e->h_stale[i] = 0;
+        e->h_stale.get()[i] = 0;
         if (a < 0 && b < 0) {
             if (e->h_head[c] >= 0) { rc = fail(e, SW_E_FORK, "event %d: second root of member %d", i, c); break; }
-            e->h_height[i] = 0;                                          // swirld.py:117-118
+            e->h_height.get()[i] = 0;                                          // swirld.py:117-118
         } else {
             if (a < 0 || b < 0 || a >= i || b >= i) { rc = fail(e, SW_E_PARENT, "event %d: parents (%d,%d) unknown", i, a, b); break; }
             if (e->h_creator[a] != c) { rc = fail(e, SW_E_PARENT, "event %d: self-parent %d has another creator", i, a); break; }
             if (e->h_creator[b] == c) { rc = fail(e, SW_E_PARENT, "event %d: other-parent %d has the same creator", i, b); break; }
             if (e->h_head[c] != a) { rc = fail(e, SW_E_FORK, "event %d: self-parent %d is not member %d's latest event (fork)", i, a, c); break; }
-            e->h_height[i] = std::max(e->h_height[a], e->h_height[b]) + 1;   // swirld.py:120
-            e->h_stale[i] = e->h_head[e->h_creator[b]] != b;             // "near fork": an older event of the peer
+            e->h_height.get()[i] = std::max(e->h_height.get()[a], e->h_height.get()[b]) + 1;   // swirld.py:120
+            e->h_stale.get()[i] = e->h_head[e->h_creator[b]] != b;             // "near fork": an older event of the peer
         }
         e->h_creator[i] = c;
         e->h_head[c] = i;
-        e->h_seq[i] = e->h_count[c]++;
+        e->h_seq.get()[i] = e->h_count[c]++;
         if (i + 1 == next_snap) { push_snapshot(e, i + 1, e->h_count); next_snap += sw_engine::SNAP; }
     }
     if (rc != SW_OK) {
@@ -1232,7 +1287,7 @@ int append_validate(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, c
         return rc;
     }
     e->h_stale_cum.resize((size_t)base + n + 1);
-    for (int j = 0; j < n; j++) e->h_stale_cum[base + j + 1] = e->h_stale_cum[base + j] + e->h_stale[base + j];
+    for (int j = 0; j < n; j++) e->h_stale_cum[base + j + 1] = e->h_stale_cum[base + j] + e->h_stale.get()[base + j];
     return SW_OK;
 }
 
@@ -1243,12 +1298,12 @@ UnpackParams append_pack(const sw_engine *e, int n, const int32_t *p0, const int
     const int base = e->n_events;
     int32_t *ints = reinterpret_cast<int32_t *>(hs);
     memcpy(ints, p0, sizeof(int32_t) * n); memcpy(ints + n, p1, sizeof(int32_t) * n); memcpy(ints + 2 * n, creator, sizeof(int32_t) * n);
-    memcpy(ints + 3 * n, e->h_seq + base, sizeof(int32_t) * n); memcpy(ints + 4 * n, e->h_height + base, sizeof(int32_t) * n);
+    memcpy(ints + 3 * n, e->h_seq.get() + base, sizeof(int32_t) * n); memcpy(ints + 4 * n, e->h_height.get() + base, sizeof(int32_t) * n);
     uint8_t *pt = hs + unpack_off_t(n);
-    memcpy(pt, t, sizeof(double) * n); memcpy(pt + (size_t)8 * n, sig, (size_t)64 * n); memcpy(pt + (size_t)72 * n, e->h_stale + base, (size_t)n);
+    memcpy(pt, t, sizeof(double) * n); memcpy(pt + (size_t)8 * n, sig, (size_t)64 * n); memcpy(pt + (size_t)72 * n, e->h_stale.get() + base, (size_t)n);
     UnpackParams U{};
-    U.base = base; U.n = n; U.stage = ds; U.p0 = e->d_p0; U.p1 = e->d_p1; U.creator = e->d_creator; U.seq = e->d_seq;
-    U.height = e->d_height; U.t = e->d_t; U.sig = e->d_sig; U.stale = e->d_stale;
+    U.base = base; U.n = n; U.stage = ds; U.p0 = e->d_p0.get(); U.p1 = e->d_p1.get(); U.creator = e->d_creator.get(); U.seq = e->d_seq.get();
+    U.height = e->d_height.get(); U.t = e->d_t.get(); U.sig = e->d_sig.get(); U.stale = e->d_stale.get();
     return U;
 }
 
@@ -1256,9 +1311,9 @@ UnpackParams append_pack(const sw_engine *e, int n, const int32_t *p0, const int
 // view's parameters (B = 1) or the device array of B views' at the start of the slot
 template <class Src>
 int unpack_staged(sw_engine *e, int si, size_t bytes, Src U, int B) {
-    cudaStream_t cs = e->copy_stream;
-    CK(cudaMemcpyAsync(e->d_stage + e->stage_bytes * si, e->h_stage + e->stage_bytes * si, bytes, cudaMemcpyHostToDevice, cs));
-    CK(cudaEventRecord(e->stage_ev[si], cs));
+    cudaStream_t cs = e->copy_stream.get();
+    CK(cudaMemcpyAsync(e->d_stage.get() + e->stage_bytes() * si, e->h_stage.get() + e->stage_bytes() * si, bytes, cudaMemcpyHostToDevice, cs));
+    CK(cudaEventRecord(e->stage_ev[si].get(), cs));
     k_unpack<<<dim3(1, B), 256, 0, cs>>>(U);
     CK(cudaGetLastError());
     e->stats.kernel_launches += 1;
@@ -1269,15 +1324,15 @@ int unpack_staged(sw_engine *e, int si, size_t bytes, Src U, int B) {
 int append_copy(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const int32_t *creator, const double *t,
                 const uint8_t *sig) {
     const int base = e->n_events;
-    cudaStream_t cs = e->copy_stream;
-    CK(cudaMemcpyAsync(e->d_p0 + base, p0, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
-    CK(cudaMemcpyAsync(e->d_p1 + base, p1, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
-    CK(cudaMemcpyAsync(e->d_creator + base, creator, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
-    CK(cudaMemcpyAsync(e->d_t + base, t, sizeof(double) * n, cudaMemcpyHostToDevice, cs));
-    CK(cudaMemcpyAsync(e->d_sig + (size_t)base * 64, sig, (size_t)64 * n, cudaMemcpyHostToDevice, cs));
-    CK(cudaMemcpyAsync(e->d_seq + base, e->h_seq + base, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
-    CK(cudaMemcpyAsync(e->d_height + base, e->h_height + base, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
-    CK(cudaMemcpyAsync(e->d_stale + base, e->h_stale + base, (size_t)n, cudaMemcpyHostToDevice, cs));
+    cudaStream_t cs = e->copy_stream.get();
+    CK(cudaMemcpyAsync(e->d_p0.get() + base, p0, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_p1.get() + base, p1, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_creator.get() + base, creator, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_t.get() + base, t, sizeof(double) * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_sig.get() + (size_t)base * 64, sig, (size_t)64 * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_seq.get() + base, e->h_seq.get() + base, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_height.get() + base, e->h_height.get() + base, sizeof(int32_t) * n, cudaMemcpyHostToDevice, cs));
+    CK(cudaMemcpyAsync(e->d_stale.get() + base, e->h_stale.get() + base, (size_t)n, cudaMemcpyHostToDevice, cs));
     return 0;
 }
 
@@ -1294,14 +1349,14 @@ int append_commit(sw_engine *e, int n, cudaStream_t st) {
     e->n_events += n;
     push_append_snapshot(e);
     if (eager) {
-        if (e->scan_ev_set) CK(cudaStreamWaitEvent(st, e->scan_ev, 0));     // never beside a scan on the compute stream
+        if (e->scan_ev_set) CK(cudaStreamWaitEvent(st, e->scan_ev.get(), 0));     // never beside a scan on the compute stream
         int rc2 = cansee_scan(e, st, e->n_events);
         if (rc2 < 0) return rc2;
     }
     // the compute stream waits for this batch only when a call first touches it (wait_appends)
-    cudaEvent_t done = get_event(e);
-    CK(cudaEventRecord(done, st));
-    e->appends.push_back({base, done});
+    Event done = get_event(e);
+    CK(cudaEventRecord(done.get(), st));
+    e->appends.push_back({base, std::move(done)});
     return 0;
 }
 
@@ -1309,10 +1364,10 @@ int append_commit(sw_engine *e, int n, cudaStream_t st) {
 StreamParams stream_params(const sw_engine *e, int first, int n) {
     StreamParams S{};
     S.M = e->M; S.first = first; S.n = n; S.Rcap = e->Rcap; S.NJ = e->NJ;
-    S.p0 = e->d_p0; S.p1 = e->d_p1; S.creator = e->d_creator; S.seq = e->d_seq; S.row = e->d_row; S.round = e->d_round;
-    S.wit = e->d_wit; S.W = e->d_W; S.Wf = e->d_Wf; S.SM = e->d_SM; S.S = e->d_S; S.SMw = e->d_SMw; S.Sw = e->d_Sw;
-    S.coin = e->d_coin; S.sig = e->d_sig; S.stake = e->d_stake; S.tot2 = 2 * e->tot; S.scal = e->d_scal;
-    S.ctot = e->d_rbtot; S.gchain = e->d_gchain; S.carry = e->d_cs_carry; S.ring = RB_RING;
+    S.p0 = e->d_p0.get(); S.p1 = e->d_p1.get(); S.creator = e->d_creator.get(); S.seq = e->d_seq.get(); S.row = e->d_row.get(); S.round = e->d_round.get();
+    S.wit = e->d_wit.get(); S.W = e->d_W.get(); S.Wf = e->d_Wf.get(); S.SM = e->d_SM.get(); S.S = e->d_S.get(); S.SMw = e->d_SMw.get(); S.Sw = e->d_Sw.get();
+    S.coin = e->d_coin.get(); S.sig = e->d_sig.get(); S.stake = e->d_stake.get(); S.tot2 = 2 * e->tot; S.scal = e->d_scal.get();
+    S.ctot = e->d_rbtot.get(); S.gchain = e->d_gchain.get(); S.carry = e->d_cs_carry.get(); S.ring = RB_RING;
     return S;
 }
 int stream_threads(int M) { return std::min(1024, std::max(32, (M + 31) / 32 * 32)); }
@@ -1323,8 +1378,8 @@ template <class Src>
 int stream_kernel(sw_engine *e, Src S, int B) {
     {
         Span sp(e, 0);
-        if (e->wide) k_stream_divide<true><<<dim3(1, B), stream_threads(e->M), stream_smem(e->M), e->stream>>>(S);
-        else k_stream_divide<false><<<dim3(1, B), stream_threads(e->M), stream_smem(e->M), e->stream>>>(S);
+        if (e->wide) k_stream_divide<true><<<dim3(1, B), stream_threads(e->M), stream_smem(e->M), e->stream.get()>>>(S);
+        else k_stream_divide<false><<<dim3(1, B), stream_threads(e->M), stream_smem(e->M), e->stream.get()>>>(S);
         CK(cudaGetLastError());
     }
     e->stats.kernel_launches += 1;
@@ -1337,7 +1392,7 @@ bool stream_path(const sw_engine *e, int first, int n) { return n <= sw_engine::
 
 // the last can_see rows were written on the compute stream: a scan on the copy stream waits for them
 int rows_written(sw_engine *e) {
-    CK(cudaEventRecord(e->scan_ev, e->stream));
+    CK(cudaEventRecord(e->scan_ev.get(), e->stream.get()));
     e->scan_ev_set = true;
     return 0;
 }
@@ -1349,7 +1404,7 @@ int rows_written(sw_engine *e) {
 int rows_ready(sw_engine *e, int first, int n, int upto = -1) {
     if (first + n <= e->n_rowed) return wait_appends(e, first + n);
     if (wait_appends(e, -1) < 0) return SW_E_CUDA;
-    const int rc = cansee_scan(e, e->stream, upto < 0 ? e->n_events : upto);
+    const int rc = cansee_scan(e, e->stream.get(), upto < 0 ? e->n_events : upto);
     return rc < 0 ? rc : rows_written(e);
 }
 
@@ -1372,19 +1427,11 @@ int stream_divided(sw_engine *e, int n) {
 template <int NC, bool UNIT>
 int chunk_views(sw_engine *e, sw_engine *const *engines, int B, const int *first, const int *n) {
     const int per_launch = e->n_sm;                         // (one CTA per view at least: its warps loop over its chains)
-    if (B > e->views_cap) {
-        if (e->d_views) cudaFree(e->d_views);
-        if (e->d_rcviews) cudaFree(e->d_rcviews);
-        e->d_views = nullptr; e->d_rcviews = nullptr;
-        CK(cudaMalloc((void **)&e->d_views, sizeof(RbParams) * B));
-        CK(cudaMalloc((void **)&e->d_rcviews, sizeof(RcParams) * B));
-        e->views_cap = B;
-    }
+    if (grow(e, B, e->d_views.cap(), sized(e->d_views, B), sized(e->d_rcviews, B)) < 0) return SW_E_CUDA;
     // one thread-block cluster per view first (swirld_rcluster.cuh); the grid-wide kernel then takes what they hand back
     bool use_rc = true;
     for (int v = 0; v < B; v++) use_rc = use_rc && engines[v]->rc_ok && n[v] >= e->rc_min_n;
     std::vector<RcParams> Qv(B);
-    if (!e->view_ev) CK(cudaEventCreateWithFlags(&e->view_ev, cudaEventDisableTiming));
     std::vector<RbParams> Rv(B);
     for (int v0 = 0; v0 < B; v0 += per_launch) {
         const int nv = std::min(per_launch, B - v0), G = e->n_sm / nv;
@@ -1393,21 +1440,22 @@ int chunk_views(sw_engine *e, sw_engine *const *engines, int B, const int *first
             if (rows_ready(x, first[v], n[v]) < 0) return SW_E_CUDA;
             // a view's window stays a round deep (16 pending events per chain) however few warps it has: they loop
             if (round_batch_prep(x, first[v], n[v], G, 16, use_rc, Rv[v], Qv[v]) < 0) { e->err = x->err; return SW_E_CUDA; }
-            cudaEvent_t ev = get_event(x);
-            CK(cudaEventRecord(ev, x->stream));
-            CK(cudaStreamWaitEvent(e->stream, ev, 0));
-            x->pool.push_back(ev);
+            Event ev = get_event(x);
+            CK(cudaEventRecord(ev.get(), x->stream.get()));
+            CK(cudaStreamWaitEvent(e->stream.get(), ev.get(), 0));
+            x->pool.push_back(std::move(ev));
         }
-        CK(cudaMemcpyAsync(e->d_views + v0, Rv.data() + v0, sizeof(RbParams) * nv, cudaMemcpyHostToDevice, e->stream));
-        cudaEvent_t a = get_event(e);
-        cudaEventRecord(a, e->stream);
-        if (use_rc) CK(cudaMemcpyAsync(e->d_rcviews + v0, Qv.data() + v0, sizeof(RcParams) * nv, cudaMemcpyHostToDevice, e->stream));
-        if (round_kernels<NC, UNIT>(e, (const RbParams *)e->d_views + v0, (const RcParams *)e->d_rcviews + v0, nv, G, use_rc, e->stream) < 0)
+        CK(cudaMemcpyAsync(e->d_views.get() + v0, Rv.data() + v0, sizeof(RbParams) * nv, cudaMemcpyHostToDevice, e->stream.get()));
+        Event a = get_event(e);
+        const cudaEvent_t start = a.get();
+        cudaEventRecord(start, e->stream.get());
+        if (use_rc) CK(cudaMemcpyAsync(e->d_rcviews.get() + v0, Qv.data() + v0, sizeof(RcParams) * nv, cudaMemcpyHostToDevice, e->stream.get()));
+        if (round_kernels<NC, UNIT>(e, (const RbParams *)e->d_views.get() + v0, (const RcParams *)e->d_rcviews.get() + v0, nv, G, use_rc, e->stream.get()) < 0)
             return SW_E_CUDA;
         count_round_kernels(e, use_rc);
-        round_span(e, a, false);
-        CK(cudaEventRecord(e->view_ev, e->stream));
-        CK(cudaStreamSynchronize(e->stream));       // (Rv / the event are reused by the next group; the views' finish kernels follow)
+        round_span(e, start, std::move(a));
+        CK(cudaEventRecord(e->view_ev.get(), e->stream.get()));
+        CK(cudaStreamSynchronize(e->stream.get()));       // (Rv / the event are reused by the next group; the views' finish kernels follow)
         for (int v = v0; v < v0 + nv; v++) {
             if (round_batch_finish<NC>(engines[v], Rv[v]) < 0) return SW_E_CUDA;
             divided(engines[v], n[v]);
@@ -1433,49 +1481,9 @@ int sw_create(int M, int capacity_events, const int64_t *stake, int coin_period,
 void sw_destroy(sw_engine *e) {
     if (!e) return;
     cudaSetDevice(e->device);
-    if (e->stream) { wait_appends(e, -1); cudaStreamSynchronize(e->stream); }
-    if (e->rstream) cudaStreamSynchronize(e->rstream);
-    if (e->pstream) cudaStreamSynchronize(e->pstream);
-    if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
+    wait_appends(e, -1);
+    sync_streams(e);
     fold_spans(e);
-    for (auto ev : e->pool) cudaEventDestroy(ev);
-    for (auto ev : e->user_ev) if (ev) cudaEventDestroy(ev);
-    if (e->scan_ev) cudaEventDestroy(e->scan_ev);
-    for (auto &p : e->rs_pieces) cudaEventDestroy(p.done);
-    for (auto ev : e->rs_free) cudaEventDestroy(ev);
-    if (e->rwait) cudaEventDestroy(e->rwait);
-    for (auto ev : e->rs_prepped) if (ev) cudaEventDestroy(ev);
-    for (auto ev : e->rs_bufdone) if (ev) cudaEventDestroy(ev);
-    if (e->view_ev) cudaEventDestroy(e->view_ev);
-    if (e->d_views) cudaFree(e->d_views);
-    if (e->d_rcviews) cudaFree(e->d_rcviews);
-    if (e->d_stviews) cudaFree(e->d_stviews);
-    if (e->d_vbuf) cudaFree(e->d_vbuf);
-    if (e->h_vbuf) cudaFreeHost(e->h_vbuf);
-    for (auto ev : e->stage_ev) if (ev) cudaEventDestroy(ev);
-    if (e->h_stage) cudaFreeHost(e->h_stage);
-    if (e->d_stage) cudaFree(e->d_stage);
-    for (int p = 0; p < 8; p++) if (e->x_peer[p] && e->x_peer[p] != e->d_xbuf) cudaIpcCloseMemHandle(e->x_peer[p]);
-    for (int p = 0; p < 8; p++) if (e->row_peer[p] && e->row_peer[p] != e->d_row) cudaIpcCloseMemHandle(e->row_peer[p]);
-    if (e->d_xflags2) cudaFree(e->d_xflags2);
-    void *ptrs[] = {e->d_rbtot, e->d_gchain, e->d_Wf, e->d_cev, e->d_rbmeta, e->d_sc, e->d_res, e->d_cs_last, e->d_cs_Q, e->d_cs_carry,
-                    e->d_cs_meta, e->d_cs_wr, e->d_cs_xb, e->d_cs_sflag, e->d_cs_xlist, e->d_cs_slowblk, e->d_cs_blkcnt, e->d_cs_slow, e->d_cs_slowcnt, e->d_stale, e->d_coin, e->d_dbg, e->d_height,
-                    e->d_p0, e->d_p1, e->d_creator, e->d_seq, e->d_t, e->d_sig, e->d_row, e->d_SM,
-                    e->d_scw, e->d_sctag, e->d_SMw, e->d_Sw, e->d_hitmin, e->d_xbuf, e->d_xstep,
-                    e->d_round, e->d_wit, e->d_famous_ev, e->d_W, e->d_S, e->d_famous, e->d_consensus,
-                    e->d_done, e->d_rem, e->d_stake, e->d_scal, e->d_lastord, e->d_tx, e->d_idx,
-                    e->d_batch_ev, e->d_batch_seg, e->d_perm, e->d_ts, e->d_key, e->d_seg_start, e->d_seg_fw,
-                    e->d_seg_nf, e->d_seg_white, e->d_rounds_in, e->d_plan, e->d_flush, e->d_rsg[0], e->d_rsg[1], e->d_rccont,
-                    e->d_Wf2, e->d_gchain2, e->d_rbmeta2, e->d_rscal};
-    for (void *p : ptrs) if (p) cudaFree(p);
-    if (e->h_scal) cudaFreeHost(e->h_scal);
-    if (e->h_height) cudaFreeHost(e->h_height);
-    if (e->h_seq) cudaFreeHost(e->h_seq);
-    if (e->h_stale) cudaFreeHost(e->h_stale);
-    if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
-    if (e->rstream) cudaStreamDestroy(e->rstream);
-    if (e->pstream) cudaStreamDestroy(e->pstream);
-    if (e->stream) cudaStreamDestroy(e->stream);
     delete e;
 }
 
@@ -1483,7 +1491,7 @@ int sw_reset(sw_engine *e) {
     if (!e) return SW_E_ARG;
     CK(cudaSetDevice(e->device));
     if (wait_appends(e, -1) < 0 || rs_drain(e) < 0) return SW_E_CUDA;
-    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaStreamSynchronize(e->stream.get()));
     fold_spans(e);
     e->h_creator.clear();
     e->ids.clear();
@@ -1497,7 +1505,7 @@ int sw_rewind(sw_engine *e) {
     if (!e) return SW_E_ARG;
     CK(cudaSetDevice(e->device));
     if (wait_appends(e, -1) < 0 || rs_drain(e) < 0) return SW_E_CUDA;
-    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaStreamSynchronize(e->stream.get()));
     fold_spans(e);
     return reset_state(e, true);
 }
@@ -1505,18 +1513,18 @@ int sw_rewind(sw_engine *e) {
 int sw_event_record(sw_engine *e, int slot) {
     if (!e || slot < 0 || slot >= 16) return fail(e, SW_E_ARG, "bad event slot");
     CK(cudaSetDevice(e->device));
-    if (!e->user_ev[slot]) CK(cudaEventCreate(&e->user_ev[slot]));
-    CK(cudaEventRecord(e->user_ev[slot], e->stream));
+    if (!e->user_ev[slot].get()) CK(e->user_ev[slot].create(true));
+    CK(cudaEventRecord(e->user_ev[slot].get(), e->stream.get()));
     return SW_OK;
 }
 
 int sw_event_elapsed_ms(sw_engine *e, int a, int b, double *ms_out) {
-    if (!e || a < 0 || a >= 16 || b < 0 || b >= 16 || !ms_out || !e->user_ev[a] || !e->user_ev[b])
+    if (!e || a < 0 || a >= 16 || b < 0 || b >= 16 || !ms_out || !e->user_ev[a].get() || !e->user_ev[b].get())
         return fail(e, SW_E_ARG, "bad event slot");
     CK(cudaSetDevice(e->device));
-    CK(cudaEventSynchronize(e->user_ev[b]));
+    CK(cudaEventSynchronize(e->user_ev[b].get()));
     float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, e->user_ev[a], e->user_ev[b]));
+    CK(cudaEventElapsedTime(&ms, e->user_ev[a].get(), e->user_ev[b].get()));
     *ms_out = ms;
     return SW_OK;
 }
@@ -1535,10 +1543,10 @@ int sw_append(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const i
         // a handful of events: pack the eight columns into one pinned block, one copy, one scatter kernel
         const int si = stage_slot(e, unpack_bytes(n));
         if (si < 0) return si;
-        const UnpackParams U = append_pack(e, n, p0, p1, creator, t, sig, e->h_stage + e->stage_bytes * si, e->d_stage + e->stage_bytes * si);
+        const UnpackParams U = append_pack(e, n, p0, p1, creator, t, sig, e->h_stage.get() + e->stage_bytes() * si, e->d_stage.get() + e->stage_bytes() * si);
         if (unpack_staged(e, si, unpack_bytes(n), U, 1) < 0) return SW_E_CUDA;
     } else if (append_copy(e, n, p0, p1, creator, t, sig) < 0) return SW_E_CUDA;
-    return append_commit(e, n, e->copy_stream);
+    return append_commit(e, n, e->copy_stream.get());
 }
 
 // Node.add_event for B node-views in one call.  Every view is validated as sw_append validates it; the views of at most
@@ -1568,7 +1576,7 @@ int sw_batch_append(sw_engine *const *engines, int B, const int *offsets, const 
         if (r < 0) { if (first_err == SW_OK) first_err = r; continue; }
         if (n == 0) continue;
         if (n <= sw_engine::STAGE_EVENTS) { packed.push_back(v); bytes += (unpack_bytes(n) + 15) & ~(size_t)15; }
-        else if (append_copy(x, n, p0 + o, p1 + o, creator + o, t + o, sig + (size_t)64 * o) < 0 || append_commit(x, n, x->copy_stream) < 0) {
+        else if (append_copy(x, n, p0 + o, p1 + o, creator + o, t + o, sig + (size_t)64 * o) < 0 || append_commit(x, n, x->copy_stream.get()) < 0) {
             e->err = x->err;
             return SW_E_CUDA;
         }
@@ -1578,7 +1586,7 @@ int sw_batch_append(sw_engine *const *engines, int B, const int *offsets, const 
     // 2. the packed views: one slot of the first engine's ring, one copy, one scatter kernel
     const int si = stage_slot(e, bytes);
     if (si < 0) return si;
-    uint8_t *hs = e->h_stage + e->stage_bytes * si, *ds = e->d_stage + e->stage_bytes * si;
+    uint8_t *hs = e->h_stage.get() + e->stage_bytes() * si, *ds = e->d_stage.get() + e->stage_bytes() * si;
     UnpackParams *U = reinterpret_cast<UnpackParams *>(hs);
     size_t off = align256(sizeof(UnpackParams) * packed.size());
     for (size_t i = 0; i < packed.size(); i++) {
@@ -1590,7 +1598,7 @@ int sw_batch_append(sw_engine *const *engines, int B, const int *offsets, const 
     if (unpack_staged(e, si, off, reinterpret_cast<const UnpackParams *>(ds), (int)packed.size()) < 0) return SW_E_CUDA;
     // each view's pending-append event comes from its own pool (wait_appends returns it there)
     for (int v : packed)
-        if (append_commit(engines[v], offsets[v + 1] - offsets[v], e->copy_stream) < 0) { e->err = engines[v]->err; return SW_E_CUDA; }
+        if (append_commit(engines[v], offsets[v + 1] - offsets[v], e->copy_stream.get()) < 0) { e->err = engines[v]->err; return SW_E_CUDA; }
     return first_err;
 }
 
@@ -1614,7 +1622,7 @@ int sw_divide_rounds(sw_engine *e, int first, int n) {
     {
         Span sp(e, 0);
         rc = ahead ? SW_NCU(e, divide_ahead, e, first, n, scan_from)
-           : e->wide ? SW_NJ(divide_rounds_wide, e, first, n) : SW_NCU(e, divide_round_batch, e, first, n, sp.s.a);
+           : e->wide ? SW_NJ(divide_rounds_wide, e, first, n) : SW_NCU(e, divide_round_batch, e, first, n, sp.a.get());
         if (rc < 0) return rc;
     }
     divided(e, n);
@@ -1651,20 +1659,14 @@ int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, c
             Sv[i] = stream_params(x, x->n_divided, sn[i]);
         }
         if (views_enter(e, sv.data(), S) < 0) return SW_E_CUDA;
-        if (S > e->stviews_cap) {
-            if (e->d_stviews) { CK(cudaStreamSynchronize(e->stream)); CK(cudaFree(e->d_stviews)); e->d_stviews = nullptr; }
-            e->stviews_cap = 0;
-            CK(cudaMalloc((void **)&e->d_stviews, sizeof(StreamParams) * S));
-            e->stviews_cap = S;
-        }
-        CK(cudaMemcpyAsync(e->d_stviews, Sv.data(), sizeof(StreamParams) * S, cudaMemcpyHostToDevice, e->stream));
+        if (grow(e, S, e->d_stviews.cap(), sized(e->d_stviews, S)) < 0) return SW_E_CUDA;
+        CK(cudaMemcpyAsync(e->d_stviews.get(), Sv.data(), sizeof(StreamParams) * S, cudaMemcpyHostToDevice, e->stream.get()));
         e->stats.h2d_bytes += sizeof(StreamParams) * S;
-        if (stream_kernel(e, (const StreamParams *)e->d_stviews, S) < 0) return SW_E_CUDA;
+        if (stream_kernel(e, (const StreamParams *)e->d_stviews.get(), S) < 0) return SW_E_CUDA;
         // each view's later work runs after the batch: no copy, no host synchronisation
-        if (!e->view_ev) CK(cudaEventCreateWithFlags(&e->view_ev, cudaEventDisableTiming));
-        CK(cudaEventRecord(e->view_ev, e->stream));
+        CK(cudaEventRecord(e->view_ev.get(), e->stream.get()));
         for (int i = 0; i < S; i++) {
-            if (sv[i] != e) CK(cudaStreamWaitEvent(sv[i]->stream, e->view_ev, 0));
+            if (sv[i] != e) CK(cudaStreamWaitEvent(sv[i]->stream.get(), e->view_ev.get(), 0));
             if (stream_divided(sv[i], sn[i]) < 0) { e->err = sv[i]->err; return SW_E_CUDA; }
         }
     }
@@ -1682,8 +1684,8 @@ int sw_decide_fame(sw_engine *e, int32_t *new_c_out, int cap) {
         CK(cudaGetLastError());
     }
     const int spec = fame_spec(e);
-    CK(cudaMemcpyAsync(e->h_scal, e->d_scal, sizeof(int32_t) * (SC_COUNT + spec), cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaMemcpyAsync(e->h_scal.get(), e->d_scal.get(), sizeof(int32_t) * (SC_COUNT + spec), cudaMemcpyDeviceToHost, e->stream.get()));
+    CK(cudaStreamSynchronize(e->stream.get()));
     if (e->spans.size() >= 256) fold_spans(e);         // (the timings are read in sw_sync / sw_stats; not on every call)
     e->stats.d2h_bytes += sizeof(int32_t) * (SC_COUNT + spec);
     int r;
@@ -1707,29 +1709,29 @@ int sw_find_order_out(sw_engine *e, const int32_t *new_c, int n, int32_t *ev_out
     int bad;
     if (!sort_rounds(e, rs.data(), n, bad)) return fail(e, SW_E_KEY, "find_order: unknown round %d", bad);
     if (order_scratch(e, n) < 0) return SW_E_CUDA;
-    CK(cudaMemcpyAsync(e->d_rounds_in, rs.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, e->stream));
-    cudaEvent_t a = get_event(e), b = get_event(e);
-    cudaEventRecord(a, e->stream);
-    OrderParams P = order_params(e, n, e->d_rounds_in);
+    CK(cudaMemcpyAsync(e->d_rounds_in.get(), rs.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, e->stream.get()));
+    Event a = get_event(e), b = get_event(e);
+    cudaEventRecord(a.get(), e->stream.get());
+    OrderParams P = order_params(e, n, e->d_rounds_in.get());
     P.out_n = want ? order_spec(e) : 0;
     order_kernels(e, P, 1, n);
     CK(cudaGetLastError());
-    cudaEventRecord(b, e->stream);
-    e->spans.push_back(TimedSpan{a, b, 2});
+    cudaEventRecord(b.get(), e->stream.get());
+    add_span(e, std::move(a), std::move(b), 2);
     const size_t bytes = sizeof(int32_t) * (SC_COUNT + 4 * (size_t)P.out_n);
-    CK(cudaMemcpyAsync(e->h_scal, e->d_scal, bytes, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));      // (rs, the host vector of the rounds, was consumed by the copy above)
+    CK(cudaMemcpyAsync(e->h_scal.get(), e->d_scal.get(), bytes, cudaMemcpyDeviceToHost, e->stream.get()));
+    CK(cudaStreamSynchronize(e->stream.get()));      // (rs, the host vector of the rounds, was consumed by the copy above)
     fold_spans(e);
     e->stats.h2d_bytes += sizeof(int32_t) * n;
     e->stats.d2h_bytes += bytes;
     const int base = e->n_tx;
     const int r = order_result(e);
     if (r <= 0 || !want) return r;
-    const int rest = order_output(e, e->stream, base, r, reinterpret_cast<const OrderOut *>(e->h_scal + SC_COUNT), P.out_n,
+    const int rest = order_output(e, e->stream.get(), base, r, reinterpret_cast<const OrderOut *>(e->h_scal.get() + SC_COUNT), P.out_n,
                                   ev_out, ts_out, rr_out);
     if (rest < 0) return rest;
     if (rest > 0) {
-        CK(cudaStreamSynchronize(e->stream));
+        CK(cudaStreamSynchronize(e->stream.get()));
         e->stats.d2h_bytes += (2 * sizeof(int32_t) + sizeof(double)) * (size_t)rest;
     }
     return r;
@@ -1749,17 +1751,17 @@ int sw_batch_decide_fame(sw_engine *const *engines, int B, int32_t *new_c_out, i
     const int S = SC_COUNT + FAME_SPEC;                // per view: the scalars and the new rounds sw_decide_fame copies
     const size_t pbytes = align256(sizeof(FameParams) * B), sbytes = sizeof(int32_t) * (size_t)S * B;
     if (views_buffer(e, pbytes + sbytes) < 0) return SW_E_CUDA;
-    FameParams *hP = reinterpret_cast<FameParams *>(e->h_vbuf);
+    FameParams *hP = reinterpret_cast<FameParams *>(e->h_vbuf.get());
     for (int v = 0; v < B; v++) hP[v] = fame_params(engines[v]);
-    const FameParams *Pv = reinterpret_cast<const FameParams *>(e->d_vbuf);
-    int32_t *d_st = reinterpret_cast<int32_t *>(e->d_vbuf + pbytes), *h_st = reinterpret_cast<int32_t *>(e->h_vbuf + pbytes);
+    const FameParams *Pv = reinterpret_cast<const FameParams *>(e->d_vbuf.get());
+    int32_t *d_st = reinterpret_cast<int32_t *>(e->d_vbuf.get() + pbytes), *h_st = reinterpret_cast<int32_t *>(e->h_vbuf.get() + pbytes);
     if (views_enter(e, engines, B) < 0) return SW_E_CUDA;
-    CK(cudaMemcpyAsync(e->d_vbuf, e->h_vbuf, sizeof(FameParams) * B, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(e->d_vbuf.get(), e->h_vbuf.get(), sizeof(FameParams) * B, cudaMemcpyHostToDevice, e->stream.get()));
     e->stats.h2d_bytes += sizeof(FameParams) * B;
     {
         Span sp(e, 1);
         fame_kernels(e, Pv, B);
-        k_views_gather<<<B, 256, 0, e->stream>>>(Pv, d_st, S);
+        k_views_gather<<<B, 256, 0, e->stream.get()>>>(Pv, d_st, S);
         CK(cudaGetLastError());
         e->stats.kernel_launches += 1;
     }
@@ -1768,7 +1770,7 @@ int sw_batch_decide_fame(sw_engine *const *engines, int B, int32_t *new_c_out, i
     int first_err = SW_OK;
     for (int v = 0; v < B; v++) {
         sw_engine *x = engines[v];
-        memcpy(x->h_scal, h_st + (size_t)S * v, sizeof(int32_t) * (SC_COUNT + fame_spec(x)));
+        memcpy(x->h_scal.get(), h_st + (size_t)S * v, sizeof(int32_t) * (SC_COUNT + fame_spec(x)));
         int r;
         if (fame_result(x, new_c_out + (size_t)cap * v, cap, r) < 0) { e->err = x->err; return SW_E_CUDA; }
         count_out[v] = r;
@@ -1828,27 +1830,27 @@ int sw_batch_find_order_out(sw_engine *const *engines, int B, const int32_t *new
     const size_t pbytes = sizeof(OrderParams) * A, inbytes = pbytes + sizeof(int32_t) * total, soff = align256(inbytes);
     const size_t sbytes = sizeof(int32_t) * (size_t)S * A;
     if (views_buffer(e, soff + sbytes) < 0) return SW_E_CUDA;
-    OrderParams *hP = reinterpret_cast<OrderParams *>(e->h_vbuf);
-    int32_t *h_rounds = reinterpret_cast<int32_t *>(e->h_vbuf + pbytes);
-    const int32_t *d_rounds = reinterpret_cast<const int32_t *>(e->d_vbuf + pbytes);
+    OrderParams *hP = reinterpret_cast<OrderParams *>(e->h_vbuf.get());
+    int32_t *h_rounds = reinterpret_cast<int32_t *>(e->h_vbuf.get() + pbytes);
+    const int32_t *d_rounds = reinterpret_cast<const int32_t *>(e->d_vbuf.get() + pbytes);
     if (total > 0) memcpy(h_rounds, rs.data(), sizeof(int32_t) * total);
     for (int i = 0; i < A; i++) {
         const int v = act_v[i];
         hP[i] = order_params(act[i], offsets[v + 1] - offsets[v], d_rounds + (offsets[v] - offsets[0]));
         hP[i].out_n = win;
     }
-    const OrderParams *Pv = reinterpret_cast<const OrderParams *>(e->d_vbuf);
-    int32_t *d_st = reinterpret_cast<int32_t *>(e->d_vbuf + soff), *h_st = reinterpret_cast<int32_t *>(e->h_vbuf + soff);
+    const OrderParams *Pv = reinterpret_cast<const OrderParams *>(e->d_vbuf.get());
+    int32_t *d_st = reinterpret_cast<int32_t *>(e->d_vbuf.get() + soff), *h_st = reinterpret_cast<int32_t *>(e->h_vbuf.get() + soff);
     if (views_enter(e, act.data(), A) < 0) return SW_E_CUDA;
-    CK(cudaMemcpyAsync(e->d_vbuf, e->h_vbuf, inbytes, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(e->d_vbuf.get(), e->h_vbuf.get(), inbytes, cudaMemcpyHostToDevice, e->stream.get()));
     e->stats.h2d_bytes += inbytes;
-    cudaEvent_t a = get_event(e), b = get_event(e);
-    cudaEventRecord(a, e->stream);
+    Event a = get_event(e), b = get_event(e);
+    cudaEventRecord(a.get(), e->stream.get());
     order_kernels(e, Pv, A, maxn);
-    k_views_gather<<<A, win ? 256 : 32, 0, e->stream>>>(Pv, d_st, S);
+    k_views_gather<<<A, win ? 256 : 32, 0, e->stream.get()>>>(Pv, d_st, S);
     CK(cudaGetLastError());
-    cudaEventRecord(b, e->stream);
-    e->spans.push_back(TimedSpan{a, b, 2});
+    cudaEventRecord(b.get(), e->stream.get());
+    add_span(e, std::move(a), std::move(b), 2);
     e->stats.kernel_launches += 1;
     if (views_leave(e, act.data(), A, h_st, d_st, sbytes) < 0) return SW_E_CUDA;
     fold_spans(e);
@@ -1857,7 +1859,7 @@ int sw_batch_find_order_out(sw_engine *const *engines, int B, const int32_t *new
     int pos = 0, vn = 0;                               // view v's output is packed at pos (out_offsets[v] .. [v+1])
     for (int i = 0; i < A; i++) {
         sw_engine *x = act[i];
-        memcpy(x->h_scal, h_st + (size_t)S * i, sizeof(int32_t) * SC_COUNT);
+        memcpy(x->h_scal.get(), h_st + (size_t)S * i, sizeof(int32_t) * SC_COUNT);
         const int base = x->n_tx;
         const int r = order_result(x);
         count_out[act_v[i]] = r;
@@ -1865,7 +1867,7 @@ int sw_batch_find_order_out(sw_engine *const *engines, int B, const int32_t *new
         if (!want) continue;
         for (; vn <= act_v[i]; vn++) out_offsets[vn] = pos;
         if (r <= 0) continue;
-        const int k = order_output(x, e->stream, base, r, reinterpret_cast<const OrderOut *>(h_st + (size_t)S * i + SC_COUNT),
+        const int k = order_output(x, e->stream.get(), base, r, reinterpret_cast<const OrderOut *>(h_st + (size_t)S * i + SC_COUNT),
                                    win, ev_out + pos, ts_out + pos, rr_out + pos);
         if (k < 0) { e->err = x->err; return k; }
         rest += k;
@@ -1873,7 +1875,7 @@ int sw_batch_find_order_out(sw_engine *const *engines, int B, const int32_t *new
     }
     if (want) for (; vn <= B; vn++) out_offsets[vn] = pos;
     if (rest > 0) {                                    // the views that ordered more than the window: one more synchronisation
-        CK(cudaStreamSynchronize(e->stream));
+        CK(cudaStreamSynchronize(e->stream.get()));
         e->stats.d2h_bytes += (2 * sizeof(int32_t) + sizeof(double)) * rest;
     }
     return first_err;
@@ -1888,8 +1890,8 @@ int sw_sync(sw_engine *e) {
     if (!e) return SW_E_ARG;
     CK(cudaSetDevice(e->device));
     if (wait_appends(e, -1) < 0) return SW_E_CUDA;
-    CK(cudaMemcpyAsync(e->h_scal, e->d_scal, sizeof(int32_t) * SC_COUNT, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaMemcpyAsync(e->h_scal.get(), e->d_scal.get(), sizeof(int32_t) * SC_COUNT, cudaMemcpyDeviceToHost, e->stream.get()));
+    CK(cudaStreamSynchronize(e->stream.get()));
     fold_spans(e);
     return device_error(e);
 }
@@ -1897,7 +1899,7 @@ int sw_sync(sw_engine *e) {
 int sw_max_round(sw_engine *e) {
     int rc = sw_sync(e);
     if (rc < 0) return rc;
-    return e->h_scal[SC_MAX_ROUND];
+    return e->h_scal.get()[SC_MAX_ROUND];
 }
 
 int sw_stats(sw_engine *e, sw_stats_t *out) {
@@ -1915,26 +1917,26 @@ int sw_stats(sw_engine *e, sw_stats_t *out) {
         CK(cudaSetDevice(e->device));                                                                \
         if (wait_appends(e, -1) < 0) return SW_E_CUDA;                                               \
         CK(cudaMemcpyAsync(out, (SRC) + (size_t)first * (WIDTH), sizeof(TYPE) * (size_t)n * (WIDTH), \
-                           cudaMemcpyDeviceToHost, e->stream));                                     \
-        CK(cudaStreamSynchronize(e->stream));                                                        \
+                           cudaMemcpyDeviceToHost, e->stream.get()));                                     \
+        CK(cudaStreamSynchronize(e->stream.get()));                                                        \
         e->stats.d2h_bytes += sizeof(TYPE) * (size_t)n * (WIDTH);                                    \
         return SW_OK;                                                                                \
     }
 
-GETTER(sw_get_round, int32_t, e->d_round, e->n_divided, 1)
-GETTER(sw_get_witness_flags, uint8_t, e->d_wit, e->n_divided, 1)
-GETTER(sw_get_famous, int8_t, e->d_famous_ev, e->n_events, 1)
-GETTER(sw_get_can_see, int32_t, e->d_row, e->n_divided, e->M)
-GETTER(sw_get_witness_table, int32_t, e->d_W, e->Rcap, e->M)
-GETTER(sw_get_transactions, int32_t, e->d_tx, e->n_tx, 1)
+GETTER(sw_get_round, int32_t, e->d_round.get(), e->n_divided, 1)
+GETTER(sw_get_witness_flags, uint8_t, e->d_wit.get(), e->n_divided, 1)
+GETTER(sw_get_famous, int8_t, e->d_famous_ev.get(), e->n_events, 1)
+GETTER(sw_get_can_see, int32_t, e->d_row.get(), e->n_divided, e->M)
+GETTER(sw_get_witness_table, int32_t, e->d_W.get(), e->Rcap, e->M)
+GETTER(sw_get_transactions, int32_t, e->d_tx.get(), e->n_tx, 1)
 GETTER(sw_get_consensus_times, double, e->d_tx_ts, e->n_tx, 1)
 GETTER(sw_get_rounds_received, int32_t, e->d_tx_rr, e->n_tx, 1)
-GETTER(sw_get_idx, int32_t, e->d_idx, e->n_events, 1)
+GETTER(sw_get_idx, int32_t, e->d_idx.get(), e->n_events, 1)
 
 int sw_get_height(sw_engine *e, int first, int n, int32_t *out) {
     if (!e || first < 0 || n < 0 || (n > 0 && !out)) return fail(e, SW_E_ARG, "bad argument");
     if (first + n > e->n_events) return fail(e, SW_E_KEY, "sw_get_height: out of range");
-    memcpy(out, e->h_height + first, sizeof(int32_t) * n);
+    memcpy(out, e->h_height.get() + first, sizeof(int32_t) * n);
     return SW_OK;
 }
 
@@ -1944,8 +1946,8 @@ int sw_get_consensus(sw_engine *e, int32_t *out, int cap) {
     if (mr < -1) return mr;
     std::vector<uint8_t> flags((size_t)mr + 2);
     if (mr >= 0) {
-        CK(cudaMemcpyAsync(flags.data(), e->d_consensus, (size_t)mr + 1, cudaMemcpyDeviceToHost, e->stream));
-        CK(cudaStreamSynchronize(e->stream));
+        CK(cudaMemcpyAsync(flags.data(), e->d_consensus.get(), (size_t)mr + 1, cudaMemcpyDeviceToHost, e->stream.get()));
+        CK(cudaStreamSynchronize(e->stream.get()));
         e->stats.d2h_bytes += mr + 1;
     }
     int cnt = 0;
@@ -1957,23 +1959,18 @@ int sw_get_consensus(sw_engine *e, int32_t *out, int cap) {
 int sw_debug_counters(sw_engine *e, int64_t *out16, int clear) {
     if (!e || !out16) return SW_E_ARG;
     CK(cudaSetDevice(e->device));
-    CK(cudaStreamSynchronize(e->stream));
-    if (e->rstream) CK(cudaStreamSynchronize(e->rstream));     // (the round stream's kernels count there too)
-    CK(cudaMemcpy(out16, e->d_dbg, sizeof(long long) * 16, cudaMemcpyDeviceToHost));
-    if (clear) CK(cudaMemset(e->d_dbg, 0, sizeof(long long) * 40));
+    CK(cudaStreamSynchronize(e->stream.get()));
+    if (e->rstream.get()) CK(cudaStreamSynchronize(e->rstream.get()));     // (the round stream's kernels count there too)
+    CK(cudaMemcpy(out16, e->d_dbg.get(), sizeof(long long) * 16, cudaMemcpyDeviceToHost));
+    if (clear) CK(cudaMemset(e->d_dbg.get(), 0, sizeof(long long) * 40));
     return SW_OK;
 }
 
 int sw_flush_l2(sw_engine *e, int64_t bytes) {
     if (!e || bytes <= 0) return SW_E_ARG;
     CK(cudaSetDevice(e->device));
-    if ((size_t)bytes > e->flush_bytes) {
-        if (e->d_flush) cudaFree(e->d_flush);
-        e->d_flush = nullptr;
-        CK(cudaMalloc(&e->d_flush, (size_t)bytes));
-        e->flush_bytes = (size_t)bytes;
-    }
-    CK(cudaMemsetAsync(e->d_flush, 0x5a, (size_t)bytes, e->stream));
+    if (grow(e, bytes, e->d_flush.cap(), sized(e->d_flush, bytes)) < 0) return SW_E_CUDA;
+    CK(cudaMemsetAsync(e->d_flush.get(), 0x5a, (size_t)bytes, e->stream.get()));
     return SW_OK;
 }
 
@@ -2052,7 +2049,7 @@ int sw_ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, co
         int rc = sw_append(e, m, c_p0.data(), c_p1.data(), c_cr.data(), c_t.data(), c_sig.data());
         if (rc < 0) return rc;
         // (pageable sources: the copies are staged before sw_append returns, the vectors may go)
-        CK(cudaStreamSynchronize(e->copy_stream));
+        CK(cudaStreamSynchronize(e->copy_stream.get()));
         for (int j = 0; j < m; j++) e->ids.emplace(key(ids + (size_t)32 * src[j]), bidx[src[j]]);
     }
     for (int i = 0; i < n; i++)
@@ -2091,8 +2088,8 @@ bool put_dev(sw_engine *e, FILE *f, const void *d, size_t bytes, std::vector<cha
     for (size_t o = 0; o < bytes; o += CH) {
         const size_t k = std::min(CH, bytes - o);
         tmp.resize(k);
-        if (cudaMemcpyAsync(tmp.data(), (const char *)d + o, k, cudaMemcpyDeviceToHost, e->stream) != cudaSuccess) return false;
-        if (cudaStreamSynchronize(e->stream) != cudaSuccess) return false;
+        if (cudaMemcpyAsync(tmp.data(), (const char *)d + o, k, cudaMemcpyDeviceToHost, e->stream.get()) != cudaSuccess) return false;
+        if (cudaStreamSynchronize(e->stream.get()) != cudaSuccess) return false;
         if (fwrite(tmp.data(), 1, k, f) != k) return false;
     }
     return true;
@@ -2109,8 +2106,8 @@ bool get_dev(sw_engine *e, FILE *f, void *d, size_t bytes, std::vector<char> &tm
         const size_t k = std::min(CH, bytes - o);
         tmp.resize(k);
         if (fread(tmp.data(), 1, k, f) != k) return false;
-        if (cudaMemcpyAsync((char *)d + o, tmp.data(), k, cudaMemcpyHostToDevice, e->stream) != cudaSuccess) return false;
-        if (cudaStreamSynchronize(e->stream) != cudaSuccess) return false;
+        if (cudaMemcpyAsync((char *)d + o, tmp.data(), k, cudaMemcpyHostToDevice, e->stream.get()) != cudaSuccess) return false;
+        if (cudaStreamSynchronize(e->stream.get()) != cudaSuccess) return false;
     }
     return true;
 }
@@ -2123,17 +2120,17 @@ struct Section { void *p; size_t bytes; bool dev; };
 std::vector<Section> ckpt_sections(sw_engine *e, const CkptHeader &H, std::vector<uint8_t> &idrec) {
     const size_t M = H.M, n = H.n_events, nd = H.n_divided, nr = H.n_rowed, NJ = H.NJ, R = H.rounds, RM = R * M;
     const size_t i4 = sizeof(int32_t), ntx = H.n_tx;
-    const Section SM = H.wide ? Section{e->d_SMw, sizeof(unsigned) * nd * NJ, true} : Section{e->d_SM, sizeof(u64) * nd, true};
-    const Section S = H.wide ? Section{e->d_Sw, sizeof(unsigned) * RM * NJ, true} : Section{e->d_S, sizeof(u64) * RM, true};
+    const Section SM = H.wide ? Section{e->d_SMw.get(), sizeof(unsigned) * nd * NJ, true} : Section{e->d_SM.get(), sizeof(u64) * nd, true};
+    const Section S = H.wide ? Section{e->d_Sw.get(), sizeof(unsigned) * RM * NJ, true} : Section{e->d_S.get(), sizeof(u64) * RM, true};
     std::vector<Section> v = {
         {e->h_creator.data(), i4 * n, false}, {e->h_head.data(), i4 * M, false}, {e->h_count.data(), i4 * M, false},
-        {e->h_height, i4 * n, false}, {e->h_seq, i4 * n, false}, {e->h_stale, n, false},
-        {e->d_p0, i4 * n, true}, {e->d_p1, i4 * n, true}, {e->d_creator, i4 * n, true}, {e->d_t, sizeof(double) * n, true},
-        {e->d_sig, 64 * n, true}, {e->d_row, i4 * nr * M, true}, {e->d_round, i4 * nd, true}, {e->d_wit, nd, true},
-        SM, {e->d_famous_ev, n, true}, {e->d_idx, i4 * n, true}, {e->d_tx, i4 * (size_t)H.n_tx, true},
-        {e->d_W, i4 * RM, true}, {e->d_Wf, i4 * RM, true}, {e->d_famous, RM, true}, {e->d_coin, RM, true},
-        S, {e->d_consensus, R, true}, {e->d_lastord, i4 * M, true}, {e->d_cs_carry, i4 * M, true}, {e->d_rbtot, i4 * M, true},
-        {e->d_gchain, i4 * M * RB_RING, true}, {e->d_scal, i4 * SC_COUNT, true}, {idrec.data(), idrec.size(), false}};
+        {e->h_height.get(), i4 * n, false}, {e->h_seq.get(), i4 * n, false}, {e->h_stale.get(), n, false},
+        {e->d_p0.get(), i4 * n, true}, {e->d_p1.get(), i4 * n, true}, {e->d_creator.get(), i4 * n, true}, {e->d_t.get(), sizeof(double) * n, true},
+        {e->d_sig.get(), 64 * n, true}, {e->d_row.get(), i4 * nr * M, true}, {e->d_round.get(), i4 * nd, true}, {e->d_wit.get(), nd, true},
+        SM, {e->d_famous_ev.get(), n, true}, {e->d_idx.get(), i4 * n, true}, {e->d_tx.get(), i4 * (size_t)H.n_tx, true},
+        {e->d_W.get(), i4 * RM, true}, {e->d_Wf.get(), i4 * RM, true}, {e->d_famous.get(), RM, true}, {e->d_coin.get(), RM, true},
+        S, {e->d_consensus.get(), R, true}, {e->d_lastord.get(), i4 * M, true}, {e->d_cs_carry.get(), i4 * M, true}, {e->d_rbtot.get(), i4 * M, true},
+        {e->d_gchain.get(), i4 * M * RB_RING, true}, {e->d_scal.get(), i4 * SC_COUNT, true}, {idrec.data(), idrec.size(), false}};
     if (H.version >= 2) { v.push_back({e->d_tx_ts, sizeof(double) * ntx, true}); v.push_back({e->d_tx_rr, i4 * ntx, true}); }
     return v;
 }
@@ -2147,7 +2144,7 @@ int sw_save(sw_engine *e, const char *path) {
     FILE *f = fopen(path, "wb");
     if (!f) return fail(e, SW_E_ARG, "sw_save: cannot open %s", path);
     const int M = e->M, n = e->n_events, nd = e->n_divided, nr = e->n_rowed;
-    const int R = std::min(e->Rcap, e->h_scal[SC_MAX_ROUND] + 2);
+    const int R = std::min(e->Rcap, e->h_scal.get()[SC_MAX_ROUND] + 2);
     CkptHeader H{};
     memcpy(H.magic, CKPT_MAGIC, 8);
     H.version = CKPT_VERSION; H.M = M; H.cap = e->cap; H.C = e->C; H.Rcap = e->Rcap; H.wide = e->wide ? 1 : 0; H.NJ = e->NJ;
@@ -2194,18 +2191,18 @@ int sw_load(const char *path, int device, int capacity_events, sw_engine **out) 
     fclose(f);
     if (!ok) { sw_destroy(e); return fail(nullptr, SW_E_ARG, "sw_load: %s is truncated or does not match its header", path); }
     // the derived columns live on the device too
-    bool ok2 = cudaMemcpy(e->d_seq, e->h_seq, sizeof(int32_t) * n, cudaMemcpyHostToDevice) == cudaSuccess
-        && cudaMemcpy(e->d_height, e->h_height, sizeof(int32_t) * n, cudaMemcpyHostToDevice) == cudaSuccess
-        && cudaMemcpy(e->d_stale, e->h_stale, (size_t)n, cudaMemcpyHostToDevice) == cudaSuccess;
+    bool ok2 = cudaMemcpy(e->d_seq.get(), e->h_seq.get(), sizeof(int32_t) * n, cudaMemcpyHostToDevice) == cudaSuccess
+        && cudaMemcpy(e->d_height.get(), e->h_height.get(), sizeof(int32_t) * n, cudaMemcpyHostToDevice) == cudaSuccess
+        && cudaMemcpy(e->d_stale.get(), e->h_stale.get(), (size_t)n, cudaMemcpyHostToDevice) == cudaSuccess;
     // a version-1 file has no times or rounds received for what it had ordered: NaN (all bits set) and -1
     if (ok2 && H.version < 2)
-        ok2 = cudaMemsetAsync(e->d_tx_ts, 0xff, sizeof(double) * (size_t)H.n_tx, e->stream) == cudaSuccess
-            && cudaMemsetAsync(e->d_tx_rr, 0xff, sizeof(int32_t) * (size_t)H.n_tx, e->stream) == cudaSuccess
-            && cudaStreamSynchronize(e->stream) == cudaSuccess;
+        ok2 = cudaMemsetAsync(e->d_tx_ts, 0xff, sizeof(double) * (size_t)H.n_tx, e->stream.get()) == cudaSuccess
+            && cudaMemsetAsync(e->d_tx_rr, 0xff, sizeof(int32_t) * (size_t)H.n_tx, e->stream.get()) == cudaSuccess
+            && cudaStreamSynchronize(e->stream.get()) == cudaSuccess;
     if (!ok2) { sw_destroy(e); return fail(nullptr, SW_E_CUDA, "sw_load: device copy failed"); }
     e->n_events = n; e->n_divided = nd; e->n_tx = H.n_tx; e->n_rowed = nr; e->rb_epoch = H.rb_epoch;
     e->h_stale_cum.assign((size_t)n + 1, 0);
-    for (int i = 0; i < n; i++) e->h_stale_cum[i + 1] = e->h_stale_cum[i] + e->h_stale[i];
+    for (int i = 0; i < n; i++) e->h_stale_cum[i + 1] = e->h_stale_cum[i] + e->h_stale.get()[i];
     std::vector<int32_t> cnt(M, 0);
     for (int i = 0; i < n; i++) {
         cnt[e->h_creator[i]]++;
@@ -2223,9 +2220,9 @@ int sw_peer_handle(sw_engine *e, void *handle_out64) {
     CK(cudaSetDevice(e->device));
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
     cudaIpcMemHandle_t h;
-    CK(cudaIpcGetMemHandle(&h, e->d_xbuf));
+    CK(cudaIpcGetMemHandle(&h, e->d_xbuf.get()));
     memcpy(handle_out64, &h, 64);
-    CK(cudaIpcGetMemHandle(&h, e->d_row));
+    CK(cudaIpcGetMemHandle(&h, e->d_row.get()));
     memcpy(reinterpret_cast<char *>(handle_out64) + 64, &h, 64);
     return SW_OK;
 }
@@ -2236,22 +2233,18 @@ int sw_peer_connect(sw_engine *e, int rank, int nranks, const void *handles) {
     if (e->n_divided > 0) return fail(e, SW_E_ARG, "sw_peer_connect: connect before the first divide_rounds");
     CK(cudaSetDevice(e->device));
     for (int p = 0; p < nranks; p++) {
-        if (p == rank) { e->x_peer[p] = e->d_xbuf; e->row_peer[p] = e->d_row; continue; }
-        cudaIpcMemHandle_t h;
-        memcpy(&h, reinterpret_cast<const char *>(handles) + (size_t)SW_PEER_HANDLE_BYTES * p, 64);
-        void *ptr = nullptr;
-        CK(cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess));
-        e->x_peer[p] = ptr;
-        memcpy(&h, reinterpret_cast<const char *>(handles) + (size_t)SW_PEER_HANDLE_BYTES * p + 64, 64);
-        ptr = nullptr;
-        CK(cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess));
-        e->row_peer[p] = reinterpret_cast<int32_t *>(ptr);
+        if (p == rank) { e->x_peer[p] = e->d_xbuf.get(); e->row_peer[p] = e->d_row.get(); continue; }
+        const char *hp = reinterpret_cast<const char *>(handles) + (size_t)SW_PEER_HANDLE_BYTES * p;
+        CK(e->x_map[p].open(hp));
+        e->x_peer[p] = e->x_map[p].get();
+        CK(e->row_map[p].open(hp + 64));
+        e->row_peer[p] = static_cast<int32_t *>(e->row_map[p].get());
     }
     // the ranks' barrier flag rows (128 bytes into the exchange buffer) as a device array
     unsigned *fl[8] = {nullptr};
     for (int p = 0; p < nranks; p++) fl[p] = reinterpret_cast<unsigned *>(reinterpret_cast<char *>(e->x_peer[p]) + 128);
-    if (!e->d_xflags2) CK(cudaMalloc((void **)&e->d_xflags2, sizeof(unsigned *) * 8));
-    CK(cudaMemcpy(e->d_xflags2, fl, sizeof fl, cudaMemcpyHostToDevice));
+    if (!e->d_xflags2.get()) CK(e->d_xflags2.alloc(8));
+    CK(cudaMemcpy(e->d_xflags2.get(), fl, sizeof fl, cudaMemcpyHostToDevice));
     e->rank = rank; e->nranks = nranks;
     return SW_OK;
 }

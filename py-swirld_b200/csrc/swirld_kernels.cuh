@@ -23,25 +23,7 @@
 typedef unsigned long long u64;
 typedef long long i64;
 
-#define SW_WC 16             // rounds of the witness table cached in shared memory
-
 enum { SC_MAX_ROUND = 0, SC_ERR = 1, SC_NEWC = 2, SC_BATCH = 3, SC_NSEG = 4, SC_MAXC = 5, SC_TICKET = 6, SC_COUNT = 8 };
-
-struct DivParams {
-    int M, first, n, Rcap;
-    const int32_t *p0, *p1, *creator;
-    int32_t *row;        // [cap][M]
-    u64 *T;              // [cap][M]
-    u64 *SM;             // [cap]
-    int32_t *round;      // [cap]
-    uint8_t *wit;        // [cap]
-    int32_t *W;          // [Rcap][M]
-    const i64 *stake;    // [M]
-    i64 tot2;            // 2 * total stake
-    int unit;            // all stakes == 1
-    int32_t *scal;       // SC_*
-    long long *dbg;      // 16 cycle counters for profiling builds of the walker, may be NULL
-};
 
 // ---------------------------------------------------------------- small helpers
 __device__ __forceinline__ i64 wsum(u64 m, int unit, const i64 *stake_s) {
