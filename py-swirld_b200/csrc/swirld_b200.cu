@@ -92,8 +92,50 @@ struct PeerMem : Handle<void *, cudaIpcCloseMemHandle> {
     }
 };
 
+// What the time of a span counts towards (fold_spans).  `scan`: a can_see scan outside any divide span, whose time is
+// divide time too; `scan_in_divide`: one inside a divide span, which counts it already; `rounds`: the round kernels.
+enum class SpanCat { divide, fame, order, scan, rounds, scan_in_divide };
+
 // `a` is `own_a`, or the start of another span, which owns it
-struct TimedSpan { cudaEvent_t a; Event own_a, b; int cat; };
+struct TimedSpan { cudaEvent_t a; Event own_a, b; SpanCat cat; };
+
+// The round stream (SW_ROUNDS_AHEAD, M <= 64, calls that go to the cluster kernel): a call whose can_see rows reach
+// beyond its end starts the round kernels of the next piece of events on `stream`, which then runs beside the call's
+// finish and fame kernels and the host's turn-around.  Round numbers are a function of the graph alone, so a piece
+// writes the final rounds of its events.  Only the rs_* functions and divide_ahead write these fields.  While `synced`:
+// - The pieces are contiguous and cover [n_divided, rounded).  A piece may span several calls; `pieces` holds those
+//   that end beyond the last call, in order.
+// - What the engine shows a caller (Wf, the ring, the counts, the round top, errors) stays the compute stream's, and
+//   only the compute stream writes it.  The round stream's kernels write copies of their own: `Wf`, `gchain` (the
+//   ring), `meta` (two chunk meta blocks: counts, offsets, barrier, witness count) and `scal` (round top, error slot);
+//   the finish kernels of each call publish the call's part of them (RbFold).
+// - Every piece ends with an event of its own.  The end of the last piece has one owner at any time: `pieces` until a
+//   call has waited for the piece, then `tail`, and `free` only once a newer piece has its own end.  So rs_drain finds
+//   it in one of the first two, and an event in `free` is recorded again only as the end of a newer piece.
+// - A piece's k_rb_prep runs on `prep`, beside the cluster kernel of the piece before it, into the meta block and the
+//   d_rsg buffer that piece does not use (`buf` alternates).  It waits for the piece before that one to have finished
+//   with them (`bufdone`), and the piece's cluster kernel waits for it (`prepped`).  d_rsg[0] is the compute stream's
+//   buffer too, which has it back after the wait of rs_drain.
+// - The round stream's ring takes a piece's events in a launch of its own at the end of the piece (k_rb_ring): the
+//   only readers of the ring slots it overwrites are this piece's cluster kernel and hand-over, which are before it on
+//   the same stream, and the next piece's kernels, which are after it; the preps never read the ring.  So no reader
+//   sees a slot overwritten too early or too late.
+struct RoundStream {
+    bool on = false;
+    Stream stream, prep;          // the round stream and its prep stream
+    Event wait;                   // both go on after what the compute stream had been given (rs_follow)
+    Event prepped[2], bufdone[2];
+    int buf = 0;                  // the buffers of the next piece
+    struct Piece { int end; Event done; };
+    std::vector<Piece> pieces;    // the pieces that end beyond the last call, in order
+    Event tail;                   // the end of the last piece, once a call has waited for it (then `pieces` is empty)
+    std::vector<Event> free;      // ends of older pieces, for newer ones to use
+    Mem<int32_t> Wf, gchain, meta, scal;
+    bool synced = false;          // the copies hold everything below `rounded`
+    int rounded = 0;              // events rounded so far (the last piece ends here)
+    unsigned epoch = 0;           // launches on the round stream (mask-cache keys of their own: the top bit set)
+    int wslot = 0;                // which of the two witness counts of d_rbmeta the next call uses
+};
 
 }  // namespace
 
@@ -108,7 +150,6 @@ struct sw_engine {
     std::vector<i64> h_stake;
     Stream stream;
     Stream copy_stream;                              // sw_append's copies run beside the kernels of earlier chunks
-    Stream rstream, pstream;                         // the round stream and its prep stream (sw_engine::ahead)
     // host mirrors for validation / views
     std::vector<int32_t> h_creator, h_head, h_count;
     Pinned<int32_t> h_height, h_seq;                 // cap entries: sources of asynchronous copies
@@ -138,31 +179,7 @@ struct sw_engine {
     Mem<int32_t> d_rsg[2], d_rccont;
     bool rc_ok = false;           // a 16-CTA cluster with its shared memory can be resident on this device
     int rc_min_n = 2048;          // shorter chunks go to the grid-wide kernel directly
-    // The rounds run ahead (SW_ROUNDS_AHEAD, M <= 64, calls that go to the cluster kernel): a call whose can_see rows reach
-    // beyond its end starts the round kernels of the next piece of events on `rstream`, which then runs beside the call's
-    // finish and fame kernels and the host's turn-around.  Round numbers are a function of the graph alone, so the piece
-    // writes the final rounds of its events; what the engine shows a caller (Wf, the ring, the counts, the round top,
-    // errors) stays the compute stream's, and the round stream keeps its own copies: `d_Wf2`, `d_gchain2`, `d_rbmeta2`
-    // (two chunk meta blocks: counts, offsets, barrier, witness count) and `d_rscal` (round top, error slot).  The pieces
-    // cover [n_divided, n_rounded); a piece may span several calls, and two stay queued beyond the last call (`rs_pieces`,
-    // each ended by its own event; `rdone`: the end of the last one -- once a call has waited for it, the event also sits
-    // in `rs_free`, which is harmless: it is recorded again only for a newer piece, which then is the last one).  A
-    // piece's k_rb_prep runs on `pstream`, beside the cluster kernel of the piece before it, into the meta block and
-    // d_rsg buffer that piece does not use (`rs_buf` alternates); it waits for the piece before that one to have finished
-    // with them (`rs_bufdone`), and the piece's cluster kernel waits for it (`rs_prepped`).
-    bool ahead = false;
-    cudaEvent_t rdone = nullptr;  // (not owned: the event of a piece, in rs_pieces or rs_free)
-    Event rwait;
-    Event rs_prepped[2], rs_bufdone[2];
-    int rs_buf = 0;               // the buffers of the next piece
-    struct RsPiece { int end; Event done; };
-    std::vector<RsPiece> rs_pieces;                  // the pieces that end beyond the last call, in order
-    std::vector<Event> rs_free;                      // their events once a call has waited for them
-    Mem<int32_t> d_Wf2, d_gchain2, d_rbmeta2, d_rscal;
-    bool rs_synced = false;       // the round stream's copies hold everything below n_rounded
-    int n_rounded = 0;            // events rounded so far (the round stream's piece ends here)
-    unsigned rs_epoch = 0;        // launches on the round stream (mask-cache keys of their own: the top bit set)
-    int wslot = 0;                // which of the two witness counts of d_rbmeta the next call uses
+    RoundStream rs;
     Mem<RcParams> d_rcviews;
     Mem<RbParams> d_views;        // sw_batch_divide_rounds: the views' parameters (owned by the first engine of a batch)
     Event view_ev;
@@ -272,16 +289,22 @@ Event get_event(sw_engine *e) {                    // a timing event: one the po
     return ev;
 }
 
-// the span from `a` to `b`, which it owns (fold_spans returns them to the pool)
-void add_span(sw_engine *e, Event a, Event b, int cat) {
-    const cudaEvent_t start = a.get();
-    e->spans.push_back(TimedSpan{start, std::move(a), std::move(b), cat});
-}
-
+// The time stream `st` takes from here to end(), or to the end of the scope: the one place timing events are recorded.
+// The span owns its events (fold_spans returns them to the pool), except that a span inside another may borrow the
+// other's start instead of recording its own (an event record costs the stream a few microseconds).
 struct Span {
-    sw_engine *e; Event a, b; int cat;
-    Span(sw_engine *e_, int cat_) : e(e_), a(get_event(e_)), b(get_event(e_)), cat(cat_) { cudaEventRecord(a.get(), e->stream.get()); }
-    ~Span() { cudaEventRecord(b.get(), e->stream.get()); add_span(e, std::move(a), std::move(b), cat); }
+    sw_engine *e; cudaStream_t st; Event a, b; cudaEvent_t start; SpanCat cat;
+    Span(sw_engine *e_, cudaStream_t st_, SpanCat cat_) : e(e_), st(st_), a(get_event(e_)), b(get_event(e_)), start(a.get()), cat(cat_) {
+        cudaEventRecord(start, st);
+    }
+    // from the start of `outer`, on its stream: for what `outer` begins with
+    Span(const Span &outer, SpanCat cat_) : e(outer.e), st(outer.st), b(get_event(outer.e)), start(outer.start), cat(cat_) {}
+    void end() {
+        if (!b.get()) return;
+        cudaEventRecord(b.get(), st);
+        e->spans.push_back(TimedSpan{start, std::move(a), std::move(b), cat});
+    }
+    ~Span() { end(); }
 };
 
 void fold_spans(sw_engine *e) {
@@ -290,12 +313,14 @@ void fold_spans(sw_engine *e) {
         if (cudaEventQuery(s.b.get()) == cudaErrorNotReady) { pending.push_back(std::move(s)); continue; }   // (a scan still running on the copy stream)
         float ms = 0.f;
         if (cudaEventElapsedTime(&ms, s.a, s.b.get()) == cudaSuccess) {
-            if (s.cat == 0) e->stats.ms_divide_rounds += ms;
-            else if (s.cat == 1) e->stats.ms_decide_fame += ms;
-            else if (s.cat == 2) e->stats.ms_find_order += ms;
-            else if (s.cat == 3) { e->stats.ms_can_see += ms; e->stats.ms_divide_rounds += ms; }
-            else if (s.cat == 4) e->stats.ms_rounds_kernel += ms;
-            else if (s.cat == 5) e->stats.ms_can_see += ms;       // (a scan inside a divide_rounds span)
+            switch (s.cat) {
+            case SpanCat::divide: e->stats.ms_divide_rounds += ms; break;
+            case SpanCat::fame: e->stats.ms_decide_fame += ms; break;
+            case SpanCat::order: e->stats.ms_find_order += ms; break;
+            case SpanCat::scan: e->stats.ms_can_see += ms; e->stats.ms_divide_rounds += ms; break;
+            case SpanCat::rounds: e->stats.ms_rounds_kernel += ms; break;
+            case SpanCat::scan_in_divide: e->stats.ms_can_see += ms; break;
+            }
         }
         if (s.own_a.get()) e->pool.push_back(std::move(s.own_a));
         e->pool.push_back(std::move(s.b));
@@ -315,9 +340,25 @@ int wait_appends(sw_engine *e, int upto) {
     return 0;
 }
 
+// The streams `after` go on once everything stream `first` has been given so far has run: `ev` marks that point (one
+// record, however many followers)
+int follow(sw_engine *e, cudaStream_t first, const std::vector<cudaStream_t> &after, cudaEvent_t ev) {
+    CK(cudaEventRecord(ev, first));
+    for (cudaStream_t s : after) CK(cudaStreamWaitEvent(s, ev, 0));
+    return 0;
+}
+
+// ... with an event borrowed from the pool of `e` (it is recorded again only after later work was queued behind the wait)
+int follow(sw_engine *e, cudaStream_t first, cudaStream_t after) {
+    Event ev = get_event(e);
+    const int rc = follow(e, first, {after}, ev.get());
+    e->pool.push_back(std::move(ev));
+    return rc;
+}
+
 // every stream of the engine idle
 int sync_streams(sw_engine *e) {
-    for (const Stream *s : {&e->stream, &e->copy_stream, &e->rstream, &e->pstream})
+    for (const Stream *s : {&e->stream, &e->copy_stream, &e->rs.stream, &e->rs.prep})
         if (s->get()) CK(cudaStreamSynchronize(s->get()));
     return 0;
 }
@@ -354,7 +395,29 @@ int device_error(sw_engine *e) {     // after a sync: did a kernel flag an error
     return 0;
 }
 
+// Everything but the ahead path writes the engine's own Wf, ring and counts: before it runs, the compute stream waits for
+// the round stream's piece, which is given up (its rounds are computed again), and so are the round stream's copies.
+// (The round stream runs its pieces in order: waiting for the end of the last one waits for all of them.)  This is the
+// one way the round stream's state is given up: after it the stream holds nothing and its copies are not valid.
+// `keys`: the caller clears the mask cache as well (reset_state), so the launch numbers that key it start again; at any
+// other time a number used before could match a mask cached by that launch.
+int rs_drain(sw_engine *e, bool keys = false) {
+    RoundStream &rs = e->rs;
+    const cudaEvent_t last = rs.pieces.empty() ? rs.tail.get() : rs.pieces.back().done.get();
+    if (rs.synced && last) CK(cudaStreamWaitEvent(e->stream.get(), last, 0));
+    rs.synced = false;
+    for (auto &p : rs.pieces) rs.free.push_back(std::move(p.done));
+    rs.pieces.clear();
+    if (rs.tail.get()) rs.free.push_back(std::move(rs.tail));
+    if (keys) rs.epoch = 0;
+    return 0;
+}
+
+// Everything back to no events divided (and none appended, unless `keep_events`), once what is queued has run
 int reset_state(sw_engine *e, bool keep_events = false) {
+    if (wait_appends(e, -1) < 0 || rs_drain(e, true) < 0) return SW_E_CUDA;      // (true: the mask cache is cleared below)
+    CK(cudaStreamSynchronize(e->stream.get()));
+    fold_spans(e);
     const size_t RM = (size_t)e->Rcap * e->M;
     k_fill_i32<<<256, 256, 0, e->stream.get()>>>(e->d_W.get(), -1, RM);
     CK(cudaMemsetAsync(e->d_famous.get(), 0xff, RM, e->stream.get()));
@@ -381,7 +444,6 @@ int reset_state(sw_engine *e, bool keep_events = false) {
     e->n_divided = e->n_tx = 0;
     e->n_rowed = 0;
     e->rb_epoch = 0;
-    e->n_rounded = 0; e->rs_epoch = 0;
     if (!keep_events) {
         e->n_events = 0;
         std::fill(e->h_head.begin(), e->h_head.end(), -1);
@@ -416,7 +478,7 @@ int cs_launches(const sw_engine *e, int first, int n) {
 // scan of a new chunk then runs beside the round kernel of the previous one).  The two never overlap: a scan
 // on one stream first waits for the last scan issued on the other (they share the scratch and the carry heads).
 // `cat`: the span category of its time (fold_spans).
-int cansee_scan(sw_engine *e, cudaStream_t st, int upto, int cat = 3) {
+int cansee_scan(sw_engine *e, cudaStream_t st, int upto, SpanCat cat = SpanCat::scan) {
     const int first = e->n_rowed, n = upto - e->n_rowed;
     if (n <= 0) return 0;
     const int M = e->M;
@@ -425,12 +487,11 @@ int cansee_scan(sw_engine *e, cudaStream_t st, int upto, int cat = 3) {
     C.p0 = e->d_p0.get(); C.p1 = e->d_p1.get(); C.creator = e->d_creator.get(); C.stale = e->d_stale.get(); C.row = e->d_row.get();
     C.meta = e->d_cs_meta.get(); C.wr = e->d_cs_wr.get(); C.xb = e->d_cs_xb.get(); C.last = e->d_cs_last.get(); C.Qtab = e->d_cs_Q.get();
     C.carry = e->d_cs_carry.get(); C.slow_list = e->d_cs_slow.get(); C.slow_cnt = e->d_cs_slowcnt.get(); C.sflag = e->d_cs_sflag.get(); C.xlist = e->d_cs_xlist.get(); C.slow_blk = e->d_cs_slowblk.get(); C.blk_cnt = e->d_cs_blkcnt.get();
-    Event a = get_event(e), b = get_event(e);
     if (n <= 24) {                                     // the reference's own cadence: a handful of events per call
-        cudaEventRecord(a.get(), st);
-        k_cs_small<<<1, std::min(1024, (M + 31) / 32 * 32), 0, st>>>(C);
-        cudaEventRecord(b.get(), st);
-        add_span(e, std::move(a), std::move(b), cat);
+        {
+            Span sp(e, st, cat);
+            k_cs_small<<<1, std::min(1024, (M + 31) / 32 * 32), 0, st>>>(C);
+        }
         CK(cudaGetLastError());
         e->stats.kernel_launches += 1;
         e->n_rowed = upto;
@@ -482,7 +543,7 @@ int cansee_scan(sw_engine *e, cudaStream_t st, int upto, int cat = 3) {
         CK(cudaMemsetAsync(e->d_cs_slowcnt.get(), 0, sizeof(int32_t) * 4, st));
         CK(cudaMemsetAsync(e->d_cs_blkcnt.get(), 0, sizeof(int32_t) * (size_t)C.nb, st));
     }
-    cudaEventRecord(a.get(), st);
+    Span sp(e, st, cat);
     k_cs_prep<<<pblocks, 256, 0, st>>>(C);
     if (C.nb > 1) {
         if (ntiles > 0) {
@@ -507,8 +568,7 @@ int cansee_scan(sw_engine *e, cudaStream_t st, int upto, int cat = 3) {
     }
     if (shard) k_cs_carry<<<(M + 255) / 256, 256, 0, st>>>(C);
     if (xbarrier() < 0) return SW_E_CUDA;                  // the whole table is in every rank's memory
-    cudaEventRecord(b.get(), st);
-    add_span(e, std::move(a), std::move(b), cat);
+    sp.end();
     CK(cudaGetLastError());
     e->stats.kernel_launches += C.nb > 1 ? 9 : 4;
     e->n_rowed = upto;
@@ -554,11 +614,11 @@ void counts_at(const sw_engine *e, int x, int32_t *out) {
 }
 
 // A chunk meta block, one layout for both kernel families (MP = max(M, 64) members): d_rbmeta of the compute stream
-// and the round stream's two blocks in d_rbmeta2, rb_meta_ints(MP) ints each
+// and the round stream's two blocks (RoundStream::meta), rb_meta_ints(MP) ints each
 struct RbMeta {
     int32_t *ccnt, *cmin, *coff;  // [MP], [MP], [MP + 1]: the chunk's per-member counts, smallest seqs, offsets (k_rb_prep)
     unsigned *bar;                // grid barrier counter of the round kernel
-    int32_t *wcnt;                // [2] witnesses of the chunk (k_rb_finish; the ahead path alternates, sw_engine::wslot)
+    int32_t *wcnt;                // [2] witnesses of the chunk (k_rb_finish; the ahead path alternates, RoundStream::wslot)
     unsigned *ticket;             // [3] k_rounds_wide's work counters
     int32_t *ctot;                // [MP] the round stream's per-member counts at the end of its piece (the compute
                                   // stream keeps its own in d_rbtot)
@@ -571,17 +631,27 @@ RbMeta rb_meta(int32_t *m, int MP) {
                   reinterpret_cast<unsigned *>(m + 3 * MP + 12), m + 3 * MP + 16};
 }
 
-// the chunk's grouping and the round kernel's barrier and witness count in block m
-void use_meta(RbParams &R, const RbMeta &m) { R.ccnt = m.ccnt; R.cmin = m.cmin; R.coff = m.coff; R.bar = m.bar; R.wcnt = m.wcnt; }
+// What the kernels of a chunk keep from chunk to chunk, and the chunk's scratch: the engine's own, which is what a
+// caller sees, or the round stream's for its buffers b (RoundStream).  `rsg`: the cluster kernel's seq-space rows.
+struct RoundTarget { RbMeta meta; int32_t *Wf, *gchain, *ctot, *scal, *rsg; };
+
+RoundTarget own_target(const sw_engine *e) {
+    return {rb_meta(e->d_rbmeta.get(), e->MP), e->d_Wf.get(), e->d_gchain.get(), e->d_rbtot.get(), e->d_scal.get(), e->d_rsg[0].get()};
+}
+
+RoundTarget rs_target(const sw_engine *e, int b) {
+    const RbMeta m = rb_meta(e->rs.meta.get() + b * rb_meta_ints(e->MP), e->MP);
+    return {m, e->rs.Wf.get(), e->rs.gchain.get(), m.ctot, e->rs.scal.get(), e->d_rsg[b].get()};
+}
 
 // what both kernel families read of the round-batch parameters: the chunk, its grouping by creator (k_rb_prep) and
 // the pass after the round kernel (k_rb_finish)
-RbParams chunk_params(const sw_engine *e, int first, int n) {
+RbParams chunk_params(const sw_engine *e, const RoundTarget &T, int first, int n) {
     RbParams R{};
     R.M = e->M; R.first = first; R.n = n; R.Rcap = e->Rcap;
     R.row = e->d_row.get(); R.p0 = e->d_p0.get(); R.creator = e->d_creator.get(); R.seq = e->d_seq.get(); R.round = e->d_round.get();
-    R.cev = e->d_cev.get(); R.ctot = e->d_rbtot.get(); R.gchain = e->d_gchain.get(); R.wit = e->d_wit.get(); R.W = e->d_W.get();
-    use_meta(R, rb_meta(e->d_rbmeta.get(), e->MP));
+    R.cev = e->d_cev.get(); R.ctot = T.ctot; R.gchain = T.gchain; R.wit = e->d_wit.get(); R.W = e->d_W.get();
+    R.ccnt = T.meta.ccnt; R.cmin = T.meta.cmin; R.coff = T.meta.coff; R.bar = T.meta.bar; R.wcnt = T.meta.wcnt;
     R.wlist = e->d_cev.get() + e->cap;
     return R;
 }
@@ -607,15 +677,27 @@ int chunk_prep(sw_engine *e, const RbParams &R, int32_t *rsg, cudaStream_t st) {
     return 0;
 }
 
-// what the round kernels read besides the chunk (the engine's Wf and scalars; the round stream swaps in its own)
-RbParams round_params(const sw_engine *e, int first, int n, int grid, int min_L) {
-    RbParams R = chunk_params(e, first, n);
+// what the round kernels read besides the chunk: Wf and the scalars of the target, launch number `epoch`
+RbParams round_params(const sw_engine *e, const RoundTarget &T, int first, int n, int grid, int min_L, unsigned epoch) {
+    RbParams R = chunk_params(e, T, first, n);
     R.L = std::max(std::min(min_L, RB_LMAX), std::min(RB_LMAX, grid * (RB_THREADS / 32) / e->M));
-    R.Wf = e->d_Wf.get(); R.sc = e->d_sc.get();
-    R.res = e->d_res.get(); R.stake = e->d_stake.get(); R.tot2 = 2 * e->tot; R.scal = e->d_scal.get();
+    R.Wf = T.Wf; R.sc = e->d_sc.get();
+    R.res = e->d_res.get(); R.stake = e->d_stake.get(); R.tot2 = 2 * e->tot; R.scal = T.scal;
     R.SM = e->d_SM.get(); R.dbg = e->d_dbg.get();
+    R.epoch = epoch;
     return R;
 }
+
+// The chunk goes to the cluster round kernel first: its parameters, with the seq-space rows of the target; the
+// cooperative kernel's R then continues from where the cluster stopped
+RcParams cluster_first(const sw_engine *e, const RoundTarget &T, RbParams &R) {
+    const RcParams Q{R, T.rsg, e->d_rccont.get()};
+    R.cont = e->d_rccont.get();
+    return Q;
+}
+
+// CTAs of one view's round kernels: 16 SMs stay free for the can_see scan of the next chunk
+int round_grid(const sw_engine *e) { return std::max(e->n_sm / 2, e->n_sm - 16); }
 
 // buffer b of the cluster kernel's seq-space rows, for n events
 int rsg_reserve(sw_engine *e, int n, int b = 0) {
@@ -625,17 +707,14 @@ int rsg_reserve(sw_engine *e, int n, int b = 0) {
 
 // rounds of the chunk by the cooperative round-batch kernel (swirld_rounds.cuh), M <= 64: parameters R + the grouping
 // of the chunk (`grid` = CTAs this view's round kernel will run on).  `rc`: the chunk goes to the cluster round kernel
-// first, with the parameters Q and the seq-space rows; R then continues from where the cluster stopped.
+// first, with the parameters Q.
 int round_batch_prep(sw_engine *e, int first, int n, int grid, int min_L, bool rc, RbParams &R, RcParams &Q) {
-    R = round_params(e, first, n, grid, min_L);
-    R.epoch = ++e->rb_epoch;
     if (rc && rsg_reserve(e, n) < 0) return SW_E_CUDA;
-    if (chunk_prep<64>(e, R, rc ? e->d_rsg[0].get() : nullptr, e->stream.get()) < 0) return SW_E_CUDA;
+    const RoundTarget T = own_target(e);
+    R = round_params(e, T, first, n, grid, min_L, ++e->rb_epoch);
+    if (chunk_prep<64>(e, R, rc ? T.rsg : nullptr, e->stream.get()) < 0) return SW_E_CUDA;
     e->stats.kernel_launches += 1;
-    if (rc) {
-        Q = RcParams{R, e->d_rsg[0].get(), e->d_rccont.get()};
-        R.cont = e->d_rccont.get();
-    }
+    if (rc) Q = cluster_first(e, T, R);
     return 0;
 }
 
@@ -704,115 +783,101 @@ void count_round_kernels(sw_engine *e, bool rc) {
     e->stats.rounds_cluster_launches += rc ? 1 : 0;
 }
 
-// The round-kernel span from `start`, which the caller recorded: `own` when the span owns it, else the start of the
-// caller's own span too (an event record costs the stream a few microseconds)
-void round_span(sw_engine *e, cudaEvent_t start, Event own = Event()) {
-    Event b = get_event(e);
-    cudaEventRecord(b.get(), e->stream.get());
-    e->spans.push_back(TimedSpan{start, std::move(own), std::move(b), 4});
-}
-
-// `start`: the event that opens the caller's span, recorded just before
+// `call`: the caller's span, opened just before: the round kernels' span starts with it
 template <int NC, bool UNIT>
-int divide_round_batch(sw_engine *e, int first, int n, cudaEvent_t start) {
-    const int grid = std::max(e->n_sm / 2, e->n_sm - 16);       // 16 SMs stay free for the can_see scan of the next chunk
+int divide_round_batch(sw_engine *e, int first, int n, const Span &call) {
+    const int grid = round_grid(e);
     const bool rc = e->rc_ok && n >= e->rc_min_n;
     RbParams R;
     RcParams Q{};
-    if (round_batch_prep(e, first, n, grid, 1, rc, R, Q) < 0 || round_kernels<NC, UNIT>(e, R, Q, 1, grid, rc, e->stream.get()) < 0)
-        return SW_E_CUDA;
-    count_round_kernels(e, rc);
-    round_span(e, start);
+    {
+        Span sp(call, SpanCat::rounds);
+        if (round_batch_prep(e, first, n, grid, 1, rc, R, Q) < 0 || round_kernels<NC, UNIT>(e, R, Q, 1, grid, rc, e->stream.get()) < 0)
+            return SW_E_CUDA;
+        count_round_kernels(e, rc);
+    }
     return round_batch_finish<NC>(e, R);
 }
 
-// ---- the rounds run ahead (sw_engine::ahead)
-// Everything but the ahead path writes the engine's own Wf, ring and counts: before it runs, the compute stream waits for
-// the round stream's piece, which is given up (its rounds are computed again), and so are the round stream's copies.
-// (The round stream runs its pieces in order: waiting for the end of the last one waits for all of them.)
-int rs_drain(sw_engine *e) {
-    if (e->rs_synced && e->rdone) CK(cudaStreamWaitEvent(e->stream.get(), e->rdone, 0));
-    e->rs_synced = false;
-    e->n_rounded = e->n_divided;
-    for (auto &p : e->rs_pieces) e->rs_free.push_back(std::move(p.done));
-    e->rs_pieces.clear();
+// ---- the rounds run ahead (RoundStream)
+int rs_create(sw_engine *e) {
+    RoundStream &rs = e->rs;
+    const size_t RM = (size_t)e->Rcap * e->M;
+    CK(rs.stream.create()); CK(rs.prep.create()); CK(rs.wait.create());
+    for (int b = 0; b < 2; b++) { CK(rs.prepped[b].create()); CK(rs.bufdone[b].create()); }
+    CK(rs.Wf.alloc(RM)); CK(rs.gchain.alloc((size_t)e->MP * RB_RING));
+    CK(rs.meta.alloc(2 * rb_meta_ints(e->MP))); CK(rs.scal.alloc(SC_COUNT));
+    rs.on = true;
     return 0;
 }
 
 // the round stream and its prep stream go on after what the compute stream has been given so far
-int rs_follow(sw_engine *e) {
-    CK(cudaEventRecord(e->rwait.get(), e->stream.get()));
-    CK(cudaStreamWaitEvent(e->rstream.get(), e->rwait.get(), 0));
-    CK(cudaStreamWaitEvent(e->pstream.get(), e->rwait.get(), 0));
-    return 0;
-}
+int rs_follow(sw_engine *e) { return follow(e, e->stream.get(), {e->rs.stream.get(), e->rs.prep.get()}, e->rs.wait.get()); }
 
 // the round stream's copies of the engine's Wf, ring and scalars, at the first call of a run of ahead calls
 int rs_sync(sw_engine *e) {
-    if (e->rs_synced) return 0;
+    RoundStream &rs = e->rs;
+    if (rs.synced) return 0;
     if (rs_follow(e) < 0) return SW_E_CUDA;
-    CK(cudaMemcpyAsync(e->d_Wf2.get(), e->d_Wf.get(), sizeof(int32_t) * e->Rcap * e->M, cudaMemcpyDeviceToDevice, e->rstream.get()));
-    CK(cudaMemcpyAsync(e->d_gchain2.get(), e->d_gchain.get(), sizeof(int32_t) * e->MP * RB_RING, cudaMemcpyDeviceToDevice, e->rstream.get()));
-    CK(cudaMemcpyAsync(e->d_rscal.get(), e->d_scal.get(), sizeof(int32_t) * SC_COUNT, cudaMemcpyDeviceToDevice, e->rstream.get()));
+    CK(cudaMemcpyAsync(rs.Wf.get(), e->d_Wf.get(), sizeof(int32_t) * e->Rcap * e->M, cudaMemcpyDeviceToDevice, rs.stream.get()));
+    CK(cudaMemcpyAsync(rs.gchain.get(), e->d_gchain.get(), sizeof(int32_t) * e->MP * RB_RING, cudaMemcpyDeviceToDevice, rs.stream.get()));
+    CK(cudaMemcpyAsync(rs.scal.get(), e->d_scal.get(), sizeof(int32_t) * SC_COUNT, cudaMemcpyDeviceToDevice, rs.stream.get()));
     CK(cudaMemsetAsync(rb_meta(e->d_rbmeta.get(), e->MP).wcnt, 0, 2 * sizeof(int32_t), e->stream.get()));
-    e->wslot = 0;
-    e->n_rounded = e->n_divided;
-    e->rs_synced = true;
+    rs.wslot = 0;
+    rs.rounded = e->n_divided;
+    rs.synced = true;
     return 0;
 }
 
-// Rounds of [first, first+n) on the round stream's meta, ring, Wf and scalars.  The caller has made `pstream` wait for the
-// piece's rows.  k_rb_prep runs there, into the buffers the piece before this one does not use, once the piece before
-// that one has finished with them; then on the round stream k_rounds_cluster and the hand-over launch of k_rounds_batch,
-// after the prep.  An event of its own marks the end (rs_pieces), and `rdone` is it too.  Last, the round stream's ring
-// takes the piece's events (k_rb_ring): the only readers of the ring slots it overwrites are this piece's cluster kernel
-// and hand-over, which are before it on the same stream, and the next piece's kernels, which are after it; the preps
-// never read the ring.  So no reader sees a slot overwritten too early or too late.
+// Rounds of [first, first+n) on the round stream's target, in the order RoundStream states.  The caller has made the
+// prep stream wait for the piece's rows.  k_rb_prep runs there; then on the round stream, after the prep,
+// k_rounds_cluster and the hand-over launch of k_rounds_batch, the piece's end, and last the ring update.
 template <int NC, bool UNIT>
 int rs_piece(sw_engine *e, int first, int n) {
-    const int b = e->rs_buf;
-    e->rs_buf ^= 1;
+    RoundStream &rs = e->rs;
+    const int b = rs.buf;
+    rs.buf ^= 1;
     if (rsg_reserve(e, n, b) < 0) return SW_E_CUDA;
-    const int grid = std::max(e->n_sm / 2, e->n_sm - 16);
-    RbParams R = round_params(e, first, n, grid, 1);
-    const RbMeta m = rb_meta(e->d_rbmeta2.get() + b * rb_meta_ints(e->MP), e->MP);
-    use_meta(R, m);
-    R.ctot = m.ctot; R.gchain = e->d_gchain2.get(); R.Wf = e->d_Wf2.get(); R.scal = e->d_rscal.get();
-    R.epoch = 0x80000000u | ++e->rs_epoch;
-    CK(cudaStreamWaitEvent(e->pstream.get(), e->rs_bufdone[b].get(), 0));
-    if (chunk_prep<64>(e, R, e->d_rsg[b].get(), e->pstream.get()) < 0) return SW_E_CUDA;
-    CK(cudaEventRecord(e->rs_prepped[b].get(), e->pstream.get()));
-    CK(cudaStreamWaitEvent(e->rstream.get(), e->rs_prepped[b].get(), 0));
-    const RcParams Q{R, e->d_rsg[b].get(), e->d_rccont.get()};
-    R.cont = e->d_rccont.get();
-    if (round_kernels<NC, UNIT>(e, R, Q, 1, grid, true, e->rstream.get()) < 0) return SW_E_CUDA;
-    CK(cudaEventRecord(e->rs_bufdone[b].get(), e->rstream.get()));
+    const int grid = round_grid(e);
+    const RoundTarget T = rs_target(e, b);
+    RbParams R = round_params(e, T, first, n, grid, 1, 0x80000000u | ++rs.epoch);
+    CK(cudaStreamWaitEvent(rs.prep.get(), rs.bufdone[b].get(), 0));
+    if (chunk_prep<64>(e, R, T.rsg, rs.prep.get()) < 0) return SW_E_CUDA;
+    if (follow(e, rs.prep.get(), {rs.stream.get()}, rs.prepped[b].get()) < 0) return SW_E_CUDA;
+    const RcParams Q = cluster_first(e, T, R);
+    if (round_kernels<NC, UNIT>(e, R, Q, 1, grid, true, rs.stream.get()) < 0) return SW_E_CUDA;
+    CK(cudaEventRecord(rs.bufdone[b].get(), rs.stream.get()));
+    if (rs.tail.get()) rs.free.push_back(std::move(rs.tail));      // (the piece that ended there is the last one no more)
     Event done;
-    if (!e->rs_free.empty()) { done = std::move(e->rs_free.back()); e->rs_free.pop_back(); }
+    if (!rs.free.empty()) { done = std::move(rs.free.back()); rs.free.pop_back(); }
     else CK(done.create());
-    e->rs_pieces.push_back({first + n, std::move(done)});
-    e->rdone = e->rs_pieces.back().done.get();
-    CK(cudaEventRecord(e->rdone, e->rstream.get()));
+    CK(cudaEventRecord(done.get(), rs.stream.get()));
+    rs.pieces.push_back({first + n, std::move(done)});
     RbRing G;
-    G.ring = e->d_gchain2.get(); G.creator = e->d_creator.get(); G.seq = e->d_seq.get(); G.rfirst = first; G.rn = n;
+    G.ring = T.gchain; G.creator = e->d_creator.get(); G.seq = e->d_seq.get(); G.rfirst = first; G.rn = n;
     counts_at(e, first + n, G.ctot);
-    k_rb_ring<<<std::max(1, std::min(2 * e->n_sm, (n + 255) / 256)), 256, 0, e->rstream.get()>>>(G);
+    k_rb_ring<<<std::max(1, std::min(2 * e->n_sm, (n + 255) / 256)), 256, 0, rs.stream.get()>>>(G);
     CK(cudaGetLastError());
-    e->n_rounded = first + n;
+    rs.rounded = first + n;
     return 0;
 }
 
-bool ahead_path(const sw_engine *e, int n) { return e->ahead && !e->wide && e->rc_ok && n >= e->rc_min_n && e->nranks == 1; }
+bool ahead_path(const sw_engine *e, int n) { return e->rs.on && !e->wide && e->rc_ok && n >= e->rc_min_n && e->nranks == 1; }
 
 // A piece queued ahead covers up to RS_CALLS call lengths of rows, and half the rows left at most, so that near the end
 // of the rows the pieces shrink back to one call: every call after the last piece would wait for all of that piece's
 // rounds before its finish and fame kernels could run.
 constexpr int RS_CALLS = 8;
 
-int rows_written(sw_engine *e);
+// the last can_see rows were written on the compute stream: a scan on the copy stream waits for them
+int rows_written(sw_engine *e) {
+    CK(cudaEventRecord(e->scan_ev.get(), e->stream.get()));
+    e->scan_ev_set = true;
+    return 0;
+}
 
 int rs_ahead_len(const sw_engine *e, int n) {
-    const int avail = e->n_rowed - e->n_rounded;
+    const int avail = e->n_rowed - e->rs.rounded;
     return std::min(avail, n * std::max(1, std::min(RS_CALLS, avail / n / 2)));
 }
 
@@ -825,44 +890,47 @@ int rs_ahead_len(const sw_engine *e, int n) {
 // rows, from there (sw_divide_rounds); the rest are scanned here, beside the call's piece, and charged as one scan.
 template <int NC, bool UNIT>
 int divide_ahead(sw_engine *e, int first, int n, int scan_from) {
+    RoundStream &rs = e->rs;
     const int end = first + n;
     if (rs_sync(e) < 0) return SW_E_CUDA;
-    const bool cover = e->n_rounded < end;
-    if (cover && (rs_follow(e) < 0 || rs_piece<NC, UNIT>(e, e->n_rounded, end - e->n_rounded) < 0))
+    const bool cover = rs.rounded < end;
+    if (cover && (rs_follow(e) < 0 || rs_piece<NC, UNIT>(e, rs.rounded, end - rs.rounded) < 0))
         return SW_E_CUDA;
     if (scan_from >= 0) {
         // (after the piece's k_rb_prep: its cluster kernel is then the first to claim the SMs the prep frees, and the
         //  scan takes what the cluster leaves)
-        if (cover) CK(cudaStreamWaitEvent(e->stream.get(), e->rs_prepped[e->rs_buf ^ 1].get(), 0));
+        if (cover) CK(cudaStreamWaitEvent(e->stream.get(), rs.prepped[rs.buf ^ 1].get(), 0));
         const i64 kl = e->stats.kernel_launches;
-        if (cansee_scan(e, e->stream.get(), e->n_events, 5) < 0 || rows_written(e) < 0) return SW_E_CUDA;
+        if (cansee_scan(e, e->stream.get(), e->n_events, SpanCat::scan_in_divide) < 0 || rows_written(e) < 0) return SW_E_CUDA;
         e->stats.kernel_launches = kl + cs_launches(e, scan_from, e->n_events - scan_from) - cs_launches(e, scan_from, end - scan_from);
     }
-    // (the pieces are contiguous from n_divided and the last ends at n_rounded >= end: one of them holds the call's end)
+    // (the pieces are contiguous from n_divided and the last ends at `rounded` >= end: one of them holds the call's end)
     size_t k = 0;
-    while (k + 1 < e->rs_pieces.size() && e->rs_pieces[k].end < end) k++;
-    if (e->rs_pieces.empty() || e->rs_pieces[k].end < end) return fail(e, SW_E_CUDA, "divide_ahead: no piece holds the call's end");
-    CK(cudaStreamWaitEvent(e->stream.get(), e->rs_pieces[k].done.get(), 0));
-    if (e->rs_pieces[k].end == end) k++;
-    for (size_t i = 0; i < k; i++) e->rs_free.push_back(std::move(e->rs_pieces[i].done));
-    e->rs_pieces.erase(e->rs_pieces.begin(), e->rs_pieces.begin() + k);
-    const RbMeta m = rb_meta(e->d_rbmeta.get(), e->MP);
-    RbParams R = chunk_params(e, first, n);
-    R.SM = e->d_SM.get(); R.wcnt = m.wcnt + e->wslot;
+    while (k + 1 < rs.pieces.size() && rs.pieces[k].end < end) k++;
+    if (rs.pieces.empty() || rs.pieces[k].end < end) return fail(e, SW_E_CUDA, "divide_ahead: no piece holds the call's end");
+    CK(cudaStreamWaitEvent(e->stream.get(), rs.pieces[k].done.get(), 0));
+    if (rs.pieces[k].end == end) k++;
+    // the pieces the call has waited for leave the queue; the end of the last piece of all stays findable (rs_drain)
+    if (k == rs.pieces.size()) { rs.tail = std::move(rs.pieces.back().done); k--; rs.pieces.pop_back(); }
+    for (size_t i = 0; i < k; i++) rs.free.push_back(std::move(rs.pieces[i].done));
+    rs.pieces.erase(rs.pieces.begin(), rs.pieces.begin() + k);
+    const RoundTarget T = own_target(e);
+    RbParams R = chunk_params(e, T, first, n);
+    R.SM = e->d_SM.get(); R.wcnt = T.meta.wcnt + rs.wslot;
     RbFold F{};
-    F.on = 1; F.Wf = e->d_Wf.get(); F.scal = e->d_scal.get(); F.wnext = m.wcnt + (e->wslot ^ 1); F.rscal = e->d_rscal.get();
+    F.on = 1; F.Wf = T.Wf; F.scal = T.scal; F.wnext = T.meta.wcnt + (rs.wslot ^ 1); F.rscal = rs.scal.get();
     counts_at(e, end, F.ctot);
-    e->wslot ^= 1;
+    rs.wslot ^= 1;
     e->rb_epoch++;
     e->stats.kernel_launches += 1;                      // (k_rb_prep)
     count_round_kernels(e, true);
     if (round_batch_finish<NC>(e, R, F) < 0) return SW_E_CUDA;
-    while (e->rs_pieces.size() < 2) {
-        const int len = rs_ahead_len(e, n), next = e->n_rounded + len;
+    while (rs.pieces.size() < 2) {
+        const int len = rs_ahead_len(e, n), next = rs.rounded + len;
         if (len < e->rc_min_n) break;
-        for (auto &a : e->appends) if (a.base < next) CK(cudaStreamWaitEvent(e->pstream.get(), a.done.get(), 0));
-        if (e->scan_ev_set) CK(cudaStreamWaitEvent(e->pstream.get(), e->scan_ev.get(), 0));
-        if (rs_piece<NC, UNIT>(e, e->n_rounded, len) < 0) return SW_E_CUDA;
+        for (auto &a : e->appends) if (a.base < next) CK(cudaStreamWaitEvent(rs.prep.get(), a.done.get(), 0));
+        if (e->scan_ev_set) CK(cudaStreamWaitEvent(rs.prep.get(), e->scan_ev.get(), 0));
+        if (rs_piece<NC, UNIT>(e, rs.rounded, len) < 0) return SW_E_CUDA;
     }
     return 0;
 }
@@ -873,7 +941,7 @@ size_t rounds_wide_smem(int M) { return (size_t)(2 * M + 16 * M + 1 + 32 + (RW_T
 template <int NJ>
 int divide_rounds_wide(sw_engine *e, int first, int n) {
     const int M = e->M;
-    const RbParams T = chunk_params(e, first, n);       // the grouping and the finish kernel shared with the M <= 64 path
+    const RbParams T = chunk_params(e, own_target(e), first, n);    // the grouping and the finish kernel shared with the M <= 64 path
     if (chunk_prep<SW_MAX_MEMBERS>(e, T, nullptr, e->stream.get()) < 0) return SW_E_CUDA;
     e->stats.kernel_launches += 1;
     RwParams R{};
@@ -897,11 +965,8 @@ int divide_rounds_wide(sw_engine *e, int first, int n) {
     CK(cudaFuncSetAttribute(k_rounds_wide<NJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     void *args[] = {(void *)&R};
     {
-        Event a = get_event(e), b = get_event(e);
-        cudaEventRecord(a.get(), e->stream.get());
+        Span sp(e, e->stream.get(), SpanCat::rounds);
         CK(cudaLaunchCooperativeKernel((void *)k_rounds_wide<NJ>, dim3(grid), dim3(RW_THREADS), args, smem, e->stream.get()));
-        cudaEventRecord(b.get(), e->stream.get());
-        add_span(e, std::move(a), std::move(b), 4);
     }
     k_rb_finish<<<std::max(1, std::min(2 * e->n_sm, (n + 255) / 256)), 256, 0, e->stream.get()>>>(T, RbFold{});
     k_w_seenmask<NJ><<<std::max(1, std::min(8 * e->n_sm, (n + 7) / 8)), 256, 0, e->stream.get()>>>(M, first, n, e->Rcap, e->d_row.get(), e->d_round.get(), e->d_W.get(), e->d_SMw.get());
@@ -1102,21 +1167,21 @@ int stage_slot(sw_engine *e, size_t bytes) {
 
 // the batch runs on the stream of `e`, the first engine: after everything each view has queued on its own
 int views_enter(sw_engine *e, sw_engine *const *views, int B) {
-    for (int v = 0; v < B; v++) {
-        sw_engine *x = views[v];
-        if (x == e) continue;
-        Event ev = get_event(x);
-        CK(cudaEventRecord(ev.get(), x->stream.get()));
-        CK(cudaStreamWaitEvent(e->stream.get(), ev.get(), 0));
-        x->pool.push_back(std::move(ev));
-    }
+    for (int v = 0; v < B; v++)
+        if (views[v] != e && follow(views[v], views[v]->stream.get(), e->stream.get()) < 0) { e->err = views[v]->err; return SW_E_CUDA; }
     return 0;
 }
 
-// ... and each view's next call runs after the batch; then the one copy of the gathered scalars and the one synchronisation
+// ... and each view's next call runs after what the batch has queued there so far
+int views_resume(sw_engine *e, sw_engine *const *views, int B) {
+    std::vector<cudaStream_t> others;
+    for (int v = 0; v < B; v++) if (views[v] != e) others.push_back(views[v]->stream.get());
+    return follow(e, e->stream.get(), others, e->view_ev.get());
+}
+
+// the views resume; then the one copy of the gathered scalars and the one synchronisation
 int views_leave(sw_engine *e, sw_engine *const *views, int B, void *h_dst, const void *d_src, size_t bytes) {
-    CK(cudaEventRecord(e->view_ev.get(), e->stream.get()));
-    for (int v = 0; v < B; v++) if (views[v] != e) CK(cudaStreamWaitEvent(views[v]->stream.get(), e->view_ev.get(), 0));
+    if (views_resume(e, views, B) < 0) return SW_E_CUDA;
     CK(cudaMemcpyAsync(h_dst, d_src, bytes, cudaMemcpyDeviceToHost, e->stream.get()));
     CK(cudaStreamSynchronize(e->stream.get()));
     e->stats.d2h_bytes += bytes;
@@ -1202,14 +1267,9 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
                 e->rc_ok = er == cudaSuccess && ncl >= 1;
                 if (er != cudaSuccess) (void)cudaGetLastError();
             }
-            e->ahead = e->rc_ok;
-            if (const char *v = getenv("SW_ROUNDS_AHEAD")) e->ahead = e->ahead && atoi(v) != 0;
-            if (e->ahead) {
-                CK(e->rstream.create()); CK(e->pstream.create()); CK(e->rwait.create());
-                for (int b = 0; b < 2; b++) { CK(e->rs_prepped[b].create()); CK(e->rs_bufdone[b].create()); }
-                CK(e->d_Wf2.alloc(RM)); CK(e->d_gchain2.alloc(MP * RB_RING));
-                CK(e->d_rbmeta2.alloc(2 * rb_meta_ints(e->MP))); CK(e->d_rscal.alloc(SC_COUNT));
-            }
+            bool ahead = e->rc_ok;
+            if (const char *v = getenv("SW_ROUNDS_AHEAD")) ahead = ahead && atoi(v) != 0;
+            if (ahead && rs_create(e) < 0) return SW_E_CUDA;
         }
         CK(e->d_round.alloc(cap)); CK(e->d_wit.alloc(cap)); CK(e->d_famous_ev.alloc(cap));
         CK(e->d_W.alloc(RM)); CK(e->d_famous.alloc(RM));
@@ -1377,7 +1437,7 @@ size_t stream_smem(int M) { return (size_t)M * 8 + 32 * 8 + (size_t)3 * M * 4 + 
 template <class Src>
 int stream_kernel(sw_engine *e, Src S, int B) {
     {
-        Span sp(e, 0);
+        Span sp(e, e->stream.get(), SpanCat::divide);
         if (e->wide) k_stream_divide<true><<<dim3(1, B), stream_threads(e->M), stream_smem(e->M), e->stream.get()>>>(S);
         else k_stream_divide<false><<<dim3(1, B), stream_threads(e->M), stream_smem(e->M), e->stream.get()>>>(S);
         CK(cudaGetLastError());
@@ -1389,13 +1449,6 @@ int stream_kernel(sw_engine *e, Src S, int B) {
 // the reference's own cadence (one sync per call): a call of at most STREAM_N events whose rows are current is divided
 // in ONE launch (swirld_stream.cuh)
 bool stream_path(const sw_engine *e, int first, int n) { return n <= sw_engine::STREAM_N && e->n_rowed == first; }
-
-// the last can_see rows were written on the compute stream: a scan on the copy stream waits for them
-int rows_written(sw_engine *e) {
-    CK(cudaEventRecord(e->scan_ev.get(), e->stream.get()));
-    e->scan_ev_set = true;
-    return 0;
-}
 
 // Before a chunk [first, first+n) on the compute stream: rows behind (small appends, or after sw_rewind) are scanned
 // there, for everything appended so far and after the copies of EVERY appended batch (the scan reads the columns of
@@ -1440,22 +1493,17 @@ int chunk_views(sw_engine *e, sw_engine *const *engines, int B, const int *first
             if (rows_ready(x, first[v], n[v]) < 0) return SW_E_CUDA;
             // a view's window stays a round deep (16 pending events per chain) however few warps it has: they loop
             if (round_batch_prep(x, first[v], n[v], G, 16, use_rc, Rv[v], Qv[v]) < 0) { e->err = x->err; return SW_E_CUDA; }
-            Event ev = get_event(x);
-            CK(cudaEventRecord(ev.get(), x->stream.get()));
-            CK(cudaStreamWaitEvent(e->stream.get(), ev.get(), 0));
-            x->pool.push_back(std::move(ev));
+            if (follow(x, x->stream.get(), e->stream.get()) < 0) { e->err = x->err; return SW_E_CUDA; }
         }
         CK(cudaMemcpyAsync(e->d_views.get() + v0, Rv.data() + v0, sizeof(RbParams) * nv, cudaMemcpyHostToDevice, e->stream.get()));
-        Event a = get_event(e);
-        const cudaEvent_t start = a.get();
-        cudaEventRecord(start, e->stream.get());
-        if (use_rc) CK(cudaMemcpyAsync(e->d_rcviews.get() + v0, Qv.data() + v0, sizeof(RcParams) * nv, cudaMemcpyHostToDevice, e->stream.get()));
-        if (round_kernels<NC, UNIT>(e, (const RbParams *)e->d_views.get() + v0, (const RcParams *)e->d_rcviews.get() + v0, nv, G, use_rc, e->stream.get()) < 0)
-            return SW_E_CUDA;
-        count_round_kernels(e, use_rc);
-        round_span(e, start, std::move(a));
-        CK(cudaEventRecord(e->view_ev.get(), e->stream.get()));
-        CK(cudaStreamSynchronize(e->stream.get()));       // (Rv / the event are reused by the next group; the views' finish kernels follow)
+        {
+            Span sp(e, e->stream.get(), SpanCat::rounds);
+            if (use_rc) CK(cudaMemcpyAsync(e->d_rcviews.get() + v0, Qv.data() + v0, sizeof(RcParams) * nv, cudaMemcpyHostToDevice, e->stream.get()));
+            if (round_kernels<NC, UNIT>(e, (const RbParams *)e->d_views.get() + v0, (const RcParams *)e->d_rcviews.get() + v0, nv, G, use_rc, e->stream.get()) < 0)
+                return SW_E_CUDA;
+            count_round_kernels(e, use_rc);
+        }
+        CK(cudaStreamSynchronize(e->stream.get()));       // (Rv is reused by the next group; the views' finish kernels follow)
         for (int v = v0; v < v0 + nv; v++) {
             if (round_batch_finish<NC>(engines[v], Rv[v]) < 0) return SW_E_CUDA;
             divided(engines[v], n[v]);
@@ -1490,9 +1538,6 @@ void sw_destroy(sw_engine *e) {
 int sw_reset(sw_engine *e) {
     if (!e) return SW_E_ARG;
     CK(cudaSetDevice(e->device));
-    if (wait_appends(e, -1) < 0 || rs_drain(e) < 0) return SW_E_CUDA;
-    CK(cudaStreamSynchronize(e->stream.get()));
-    fold_spans(e);
     e->h_creator.clear();
     e->ids.clear();
     e->h_stale_cum.assign(1, 0);
@@ -1504,9 +1549,6 @@ int sw_reset(sw_engine *e) {
 int sw_rewind(sw_engine *e) {
     if (!e) return SW_E_ARG;
     CK(cudaSetDevice(e->device));
-    if (wait_appends(e, -1) < 0 || rs_drain(e) < 0) return SW_E_CUDA;
-    CK(cudaStreamSynchronize(e->stream.get()));
-    fold_spans(e);
     return reset_state(e, true);
 }
 
@@ -1620,9 +1662,9 @@ int sw_divide_rounds(sw_engine *e, int first, int n) {
     int rc = rows_ready(e, first, n, scan_from >= 0 ? first + n : -1);
     if (rc < 0) return rc;
     {
-        Span sp(e, 0);
+        Span sp(e, e->stream.get(), SpanCat::divide);
         rc = ahead ? SW_NCU(e, divide_ahead, e, first, n, scan_from)
-           : e->wide ? SW_NJ(divide_rounds_wide, e, first, n) : SW_NCU(e, divide_round_batch, e, first, n, sp.a.get());
+           : e->wide ? SW_NJ(divide_rounds_wide, e, first, n) : SW_NCU(e, divide_round_batch, e, first, n, sp);
         if (rc < 0) return rc;
     }
     divided(e, n);
@@ -1664,11 +1706,9 @@ int sw_batch_divide_rounds(sw_engine *const *engines, int B, const int *first, c
         e->stats.h2d_bytes += sizeof(StreamParams) * S;
         if (stream_kernel(e, (const StreamParams *)e->d_stviews.get(), S) < 0) return SW_E_CUDA;
         // each view's later work runs after the batch: no copy, no host synchronisation
-        CK(cudaEventRecord(e->view_ev.get(), e->stream.get()));
-        for (int i = 0; i < S; i++) {
-            if (sv[i] != e) CK(cudaStreamWaitEvent(sv[i]->stream.get(), e->view_ev.get(), 0));
+        if (views_resume(e, sv.data(), S) < 0) return SW_E_CUDA;
+        for (int i = 0; i < S; i++)
             if (stream_divided(sv[i], sn[i]) < 0) { e->err = sv[i]->err; return SW_E_CUDA; }
-        }
     }
     if (!cv.empty()) return SW_NCU(cv[0], chunk_views, e, cv.data(), (int)cv.size(), cfirst.data(), cn.data());
     return SW_OK;
@@ -1679,7 +1719,7 @@ int sw_decide_fame(sw_engine *e, int32_t *new_c_out, int cap) {
     CK(cudaSetDevice(e->device));
     if (e->n_divided == 0) return fail(e, SW_E_ARG, "decide_fame: no witnesses yet (max() of an empty dict, swirld.py:225)");
     {
-        Span sp(e, 1);
+        Span sp(e, e->stream.get(), SpanCat::fame);
         fame_kernels(e, fame_params(e), 1);
         CK(cudaGetLastError());
     }
@@ -1710,14 +1750,13 @@ int sw_find_order_out(sw_engine *e, const int32_t *new_c, int n, int32_t *ev_out
     if (!sort_rounds(e, rs.data(), n, bad)) return fail(e, SW_E_KEY, "find_order: unknown round %d", bad);
     if (order_scratch(e, n) < 0) return SW_E_CUDA;
     CK(cudaMemcpyAsync(e->d_rounds_in.get(), rs.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, e->stream.get()));
-    Event a = get_event(e), b = get_event(e);
-    cudaEventRecord(a.get(), e->stream.get());
     OrderParams P = order_params(e, n, e->d_rounds_in.get());
     P.out_n = want ? order_spec(e) : 0;
-    order_kernels(e, P, 1, n);
-    CK(cudaGetLastError());
-    cudaEventRecord(b.get(), e->stream.get());
-    add_span(e, std::move(a), std::move(b), 2);
+    {
+        Span sp(e, e->stream.get(), SpanCat::order);
+        order_kernels(e, P, 1, n);
+        CK(cudaGetLastError());
+    }
     const size_t bytes = sizeof(int32_t) * (SC_COUNT + 4 * (size_t)P.out_n);
     CK(cudaMemcpyAsync(e->h_scal.get(), e->d_scal.get(), bytes, cudaMemcpyDeviceToHost, e->stream.get()));
     CK(cudaStreamSynchronize(e->stream.get()));      // (rs, the host vector of the rounds, was consumed by the copy above)
@@ -1759,7 +1798,7 @@ int sw_batch_decide_fame(sw_engine *const *engines, int B, int32_t *new_c_out, i
     CK(cudaMemcpyAsync(e->d_vbuf.get(), e->h_vbuf.get(), sizeof(FameParams) * B, cudaMemcpyHostToDevice, e->stream.get()));
     e->stats.h2d_bytes += sizeof(FameParams) * B;
     {
-        Span sp(e, 1);
+        Span sp(e, e->stream.get(), SpanCat::fame);
         fame_kernels(e, Pv, B);
         k_views_gather<<<B, 256, 0, e->stream.get()>>>(Pv, d_st, S);
         CK(cudaGetLastError());
@@ -1844,14 +1883,13 @@ int sw_batch_find_order_out(sw_engine *const *engines, int B, const int32_t *new
     if (views_enter(e, act.data(), A) < 0) return SW_E_CUDA;
     CK(cudaMemcpyAsync(e->d_vbuf.get(), e->h_vbuf.get(), inbytes, cudaMemcpyHostToDevice, e->stream.get()));
     e->stats.h2d_bytes += inbytes;
-    Event a = get_event(e), b = get_event(e);
-    cudaEventRecord(a.get(), e->stream.get());
-    order_kernels(e, Pv, A, maxn);
-    k_views_gather<<<A, win ? 256 : 32, 0, e->stream.get()>>>(Pv, d_st, S);
-    CK(cudaGetLastError());
-    cudaEventRecord(b.get(), e->stream.get());
-    add_span(e, std::move(a), std::move(b), 2);
-    e->stats.kernel_launches += 1;
+    {
+        Span sp(e, e->stream.get(), SpanCat::order);
+        order_kernels(e, Pv, A, maxn);
+        k_views_gather<<<A, win ? 256 : 32, 0, e->stream.get()>>>(Pv, d_st, S);
+        CK(cudaGetLastError());
+        e->stats.kernel_launches += 1;
+    }
     if (views_leave(e, act.data(), A, h_st, d_st, sbytes) < 0) return SW_E_CUDA;
     fold_spans(e);
     int first_err = SW_OK;
@@ -1960,7 +1998,7 @@ int sw_debug_counters(sw_engine *e, int64_t *out16, int clear) {
     if (!e || !out16) return SW_E_ARG;
     CK(cudaSetDevice(e->device));
     CK(cudaStreamSynchronize(e->stream.get()));
-    if (e->rstream.get()) CK(cudaStreamSynchronize(e->rstream.get()));     // (the round stream's kernels count there too)
+    if (e->rs.on) CK(cudaStreamSynchronize(e->rs.stream.get()));     // (the round stream's kernels count there too)
     CK(cudaMemcpy(out16, e->d_dbg.get(), sizeof(long long) * 16, cudaMemcpyDeviceToHost));
     if (clear) CK(cudaMemset(e->d_dbg.get(), 0, sizeof(long long) * 40));
     return SW_OK;
