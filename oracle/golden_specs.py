@@ -70,6 +70,18 @@ SPECS = {
 # 400 turns, real signatures, so not reproducible from a seed: the fixture stores the trace itself)
 NODE_FIXTURES = ["node_m4_t400_s5_n0", "node_m4_t400_s5_n1"]
 
+# node views of generator traces (traces.node_view: one member's arrival order, one call per sync), stored like
+# NODE_FIXTURES with the reference's replay: name -> (generator, kwargs, node)
+VIEW_FIXTURES = {
+    # a partition that heals: the node's syncs after the heal bring thousands of events, stale parents far behind
+    "view_g5_m8_n12000_s3_x0": ("partition", dict(M=8, N=12000, seed=3, split=4, start=2000, end=9000), 0),
+    # the two-word masks, roots out of member order
+    "view_g1_m33_n6000_s7_x5": ("gossip", dict(M=33, N=6000, seed=7), 5),
+    # two cliques with rare cross links: long bursts from the other clique (at p_cross = 0.002 no round of an 8000-event
+    # view reaches consensus)
+    "view_g2_m16_n8000_s1_x0": ("adversarial", dict(M=16, N=8000, seed=1, p_cross=0.004, p_stale=0.3), 0),
+}
+
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
                           "tests", "golden")
 
@@ -82,3 +94,10 @@ def make_trace(name):
 
 def path(name):
     return os.path.join(GOLDEN_DIR, name + ".npz")
+
+
+def make_view(name):
+    """(view trace, call sizes) of VIEW_FIXTURES[name]."""
+    from swirld_b200 import traces
+    gen, kw, node = VIEW_FIXTURES[name]
+    return traces.node_view(getattr(traces, gen)(**kw), node)

@@ -5,6 +5,7 @@ on the traces and call schedules of oracle/golden_specs.py.
 With a checkout of py-swirld at $SWIRLD_REFERENCE:
     python oracle/make_golden.py [name ...]
     python oracle/make_golden.py --nodes     # golden_specs.NODE_FIXTURES, from a fresh simulation
+    python oracle/make_golden.py --views [name ...]   # golden_specs.VIEW_FIXTURES
 
 Each fixture holds, in index space: round[N], witness_table[R,M], famous[N]
 (-1 = no entry), consensus[], transactions[], the per-call new_c lists
@@ -77,10 +78,26 @@ def main_nodes():
         print("%-24s N=%d calls=%d ordered=%d" % (name, tr.N, len(sizes), len(r["transactions"])), flush=True)
 
 
+def main_views(names):
+    """Each fixture: a node view of a generator trace (golden_specs.VIEW_FIXTURES) and the reference's replay of it
+    with one call per sync, stored as main_nodes stores its fixtures."""
+    for name in names:
+        tr, sizes = gs.make_view(name)
+        t0 = time.time()
+        r = rh.run_reference(tr, sizes)
+        np.savez_compressed(gs.path(name), M=tr.M, p0=tr.p0, p1=tr.p1, creator=tr.creator, t=tr.t, sig=tr.sig,
+                            sizes=np.array(sizes, np.int32), round=r["round"], famous=r["famous"],
+                            consensus=r["consensus"], transactions=r["transactions"])
+        print("%-28s N=%d calls=%d ordered=%d  (%.1fs)" % (name, tr.N, len(sizes), len(r["transactions"]),
+                                                           time.time() - t0), flush=True)
+
+
 if __name__ == "__main__":
     if not rh.reference_available():
         sys.exit("set SWIRLD_REFERENCE to a checkout of py-swirld")
     if sys.argv[1:] == ["--nodes"]:
         main_nodes()
+    elif sys.argv[1:2] == ["--views"]:
+        main_views(sys.argv[2:] or list(gs.VIEW_FIXTURES))
     else:
         main(sys.argv[1:] or list(gs.SPECS))

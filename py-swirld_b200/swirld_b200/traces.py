@@ -295,6 +295,56 @@ def chunks(n: int, k: int):
         first += cnt
 
 
+def can_see_rows(tr: Trace) -> np.ndarray:
+    """int32[N, M]: row[i][m] = the latest event of member m that event i sees (itself in its own column), -1 none --
+    the max-plus recurrence over the parents (swirld.py:203-205), one pass in index order."""
+    row = np.full((tr.N, tr.M), -1, np.int32)
+    p0, p1, cr = tr.p0.tolist(), tr.p1.tolist(), tr.creator.tolist()
+    for i in range(tr.N):
+        if p0[i] >= 0:
+            np.maximum(row[p0[i]], row[p1[i]], out=row[i])
+        row[i, cr[i]] = i
+    return row
+
+
+def node_view(base: Trace, X: int, rows: np.ndarray | None = None):
+    """Node X's own view of the gossip that ``base`` records: (view trace, call sizes).
+
+    In ``base`` event i is its creator syncing with a peer and creating i (the process gossip() draws), so X holds an
+    event once one of X's own events sees it.  With x_1 < x_2 < ... X's events and row() the can_see rows of ``base``,
+    an event e of member m is in the view iff e <= row(x_last)[m], and arrives with X's sync j: the first j with
+    row(x_j)[m] >= e.  The view lists its events by (sync, base index): what each sync brought, parents first, then
+    X's new event last.  Parents are remapped, ``t`` and ``sig`` travel with their event.  sizes[j] is the number of
+    events of sync j: one divide_rounds call per sync, as the reference's Node.main makes them (swirld.py:324-328).
+    ``rows``: can_see_rows(base), to share one pass among the views of every member (node_views)."""
+    rows = can_see_rows(base) if rows is None else rows
+    chain = np.flatnonzero(base.creator == X)
+    assert chain.size, "member %d has no event" % X
+    R = rows[chain]                                   # [J, M], every column non-decreasing along X's chain
+    ev = np.arange(base.N)
+    m = base.creator.astype(np.int64)
+    inside = ev <= R[-1][m]
+    key = np.full(base.N, -1, np.int64)
+    for c in range(base.M):                           # one searchsorted per member, over X's chain
+        mine = np.flatnonzero(inside & (m == c))
+        key[mine] = np.searchsorted(R[:, c], mine, side="left")
+    keep = np.flatnonzero(inside)
+    order = keep[np.lexsort((keep, key[keep]))]
+    new = np.full(base.N, -1, np.int64)
+    new[order] = np.arange(order.size)
+    remap = lambda p: np.where(p >= 0, new[np.maximum(p, 0)], -1).astype(np.int32)
+    view = Trace(base.M, remap(base.p0[order]), remap(base.p1[order]), base.creator[order].copy(), base.t[order].copy(),
+                 base.sig[order].copy(), "view%d[%s]" % (X, base.name))
+    sizes = np.bincount(key[order], minlength=chain.size)
+    return view, [int(s) for s in sizes]
+
+
+def node_views(base: Trace):
+    """node_view(base, X) of every member X, from one can_see pass over ``base``."""
+    rows = can_see_rows(base)
+    return [node_view(base, X, rows) for X in range(base.M)]
+
+
 def heights(tr: Trace) -> np.ndarray:
     """Topological level of each event (swirld.py:114-120)."""
     h = np.zeros(tr.N, dtype=np.int32)

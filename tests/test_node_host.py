@@ -50,14 +50,20 @@ def test_each_node_matches_oracle_replay(sim):
 
 
 def test_each_node_matches_reference_replay():
-    """Two nodes' arrival traces and call schedules from a simulation like `sim`, stored with the reference's replay
-    of each (tests/golden, oracle/make_golden.py --nodes): the oracle's replay must equal it."""
+    """Two nodes' arrival traces and call schedules from a simulation like `sim`, and three node views of generator
+    traces at 8, 16 and 33 members (traces.node_view), stored with the reference's replay of each (tests/golden,
+    oracle/make_golden.py --nodes / --views): the oracle's replay must equal it."""
     import golden_specs as gs
     import numpy as np
     from swirld_b200.traces import Trace
-    for name in gs.NODE_FIXTURES:
+    for name in gs.NODE_FIXTURES + list(gs.VIEW_FIXTURES):
         z = np.load(gs.path(name))
         tr = Trace(int(z["M"]), z["p0"], z["p1"], z["creator"], z["t"], z["sig"], name)
+        if name in gs.VIEW_FIXTURES:                     # node_view still builds the view the reference replayed
+            view, sizes = gs.make_view(name)
+            assert sizes == z["sizes"].tolist(), name
+            for k in ("p0", "p1", "creator", "t", "sig"):
+                assert np.array_equal(getattr(view, k), z[k]), "%s: %s differs from node_view's" % (name, k)
         assert_same(z, node_sim.replay_oracle(tr, z["sizes"].tolist()), KEYS, name + ": oracle replay vs reference")
 
 
