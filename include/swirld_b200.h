@@ -203,9 +203,34 @@ int sw_debug_counters(sw_engine *e, int64_t *out16, int clear);
  * batch; a cycle returns SW_E_ARG like toposort's ValueError), validated like sw_append validates (unknown parent,
  * parent shape, fork -- such an event, and whatever depends on it, is skipped: index -1), appended by ONE sw_append in
  * that order and entered in the engine's id -> index map.  index_out[i] = arrival index of input event i.  Returns
- * the number of events appended.  Signature checks (Ed25519) stay with the caller (libsodium, out of scope). */
+ * the number of events appended.  It checks no signature and no id: sw_ingest_verified does both on the GPU. */
 int sw_ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const uint8_t *p1_ids,
               const int32_t *creator, const double *t, const uint8_t *sig, int32_t *index_out);
+
+/* ---- is_valid_event's crypto (swirld.py:97-103) on the GPU: Ed25519 signatures with libsodium's verdicts, BLAKE2b ids.
+ * The members' Ed25519 public keys, M x 32 bytes (member m = row m, the member order of the stake).  May be called
+ * again to replace them.  A key libsodium would refuse (y not canonical, not on the curve, small order) is accepted
+ * here and every signature under it then fails, as crypto_sign_verify_detached fails for it.  sw_reset and sw_rewind
+ * keep the keys; they are not part of the checkpoint (an engine from sw_load has none until this is called). */
+int sw_set_member_keys(sw_engine *e, const uint8_t *pk);
+
+/* For n events: flags_out[i] bit 0 = sig[i] (64 bytes) is a valid Ed25519 signature by member creator[i] of
+ * msg[msg_off[i] .. msg_off[i+1]) exactly when libsodium's crypto_sign_verify_detached (>= 1.0.18) accepts it; bit 1 =
+ * BLAKE2b-256(pre[pre_off[i] .. pre_off[i+1])) == ids[i] (32 bytes).  Offsets are n+1 int64, monotone, starting at 0.
+ * SW_E_ARG before anything runs, flags_out unwritten, for no keys, a creator out of range or bad offsets.  Runs on the
+ * engine's stream (sw_event_record slots can bracket it); synchronous: returns SW_OK once flags_out is written. */
+int sw_verify_events(sw_engine *e, int n, const int32_t *creator, const uint8_t *sig,
+                     const uint8_t *msg, const int64_t *msg_off, const uint8_t *pre, const int64_t *pre_off,
+                     const uint8_t *ids, uint8_t *flags_out);
+
+/* sw_ingest, and also: every NEW event of the batch (an id the engine does not know yet, swirld.py:130) must pass
+ * sw_verify_events with flags == 3, or it is skipped like an invalid event (index -1), and so is whatever depends on
+ * it.  A known id is not checked again.  Only the new events go to the GPU, in one sw_verify_events pass.  SW_E_ARG
+ * before anything runs for no keys or bad offsets (msg_off / pre_off as sw_verify_events, n+1 entries). */
+int sw_ingest_verified(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const uint8_t *p1_ids,
+                       const int32_t *creator, const double *t, const uint8_t *sig,
+                       const uint8_t *msg, const int64_t *msg_off, const uint8_t *pre, const int64_t *pre_off,
+                       int32_t *index_out);
 int sw_lookup(sw_engine *e, int n, const uint8_t *ids, int32_t *index_out);   /* id -> arrival index, -1 unknown */
 
 /* ---- checkpoint / resume (the reference keeps its state in memory only and uses pickle on the wire, swirld.py:129,160):

@@ -9,6 +9,7 @@
 #include "swirld_rcluster.cuh"
 #include "swirld_wide.cuh"
 #include "swirld_stream.cuh"
+#include "swirld_verify.cuh"
 
 #include <cstdlib>
 #include "../../include/swirld_b200.h"
@@ -247,6 +248,13 @@ struct sw_engine {
     std::vector<TimedSpan> spans;
     std::vector<Event> pool;      // timing events no span or append holds
     std::unordered_map<Id32, int32_t, Id32Hash> ids;     // sw_ingest: event id -> arrival index
+    // sw_verify_events (swirld_verify.cuh): the members' keys, libsodium's verdict on each key alone, [1..15](-A) per
+    // member and [1..15]B; a call's inputs go over in one copy from h_vin, and its flags come back through h_vflags
+    bool have_keys = false, have_base = false;
+    Mem<uint8_t> d_vkeys, d_vkey_ok;
+    Mem<swv::gc> d_vatab, d_vbtab;
+    Pinned<uint8_t> h_vin, h_vflags;
+    Mem<uint8_t> d_vin, d_vk, d_vflags;
     sw_stats_t stats{};
     std::string err;
     size_t stage_bytes() const { return d_stage.cap() / STAGE_SLOTS; }
@@ -1512,11 +1520,80 @@ int chunk_views(sw_engine *e, sw_engine *const *engines, int B, const int *first
     return SW_OK;
 }
 
+// sw_verify_events' refusals, before anything runs: keys, creators, offsets (n + 1 of them, from 0, monotone)
+int verify_args(sw_engine *e, const char *what, int n, const int32_t *creator, const int64_t *msg_off,
+                const int64_t *pre_off, bool check_creators) {
+    if (!e->have_keys) return fail(e, SW_E_ARG, "%s: no member keys (sw_set_member_keys)", what);
+    for (const int64_t *off : {msg_off, pre_off}) {
+        if (off[0] != 0) return fail(e, SW_E_ARG, "%s: offsets must start at 0", what);
+        for (int i = 0; i < n; i++)
+            if (off[i + 1] < off[i]) return fail(e, SW_E_ARG, "%s: offsets are not monotone at %d", what, i);
+    }
+    if (check_creators)
+        for (int i = 0; i < n; i++)
+            if (creator[i] < 0 || creator[i] >= e->M) return fail(e, SW_E_ARG, "%s: creator %d of event %d out of range", what, creator[i], i);
+    return 0;
+}
+
+// Verify events sel[0..n) of the caller's columns (sel null: events 0..n), flags into flags_out[0..n): the columns
+// are packed into one pinned block and go over in one copy; both kernels run on the compute stream; one sync.
+int verify_run(sw_engine *e, int n, const int *sel, const int32_t *creator, const uint8_t *sig, const uint8_t *msg,
+               const int64_t *msg_off, const uint8_t *pre, const int64_t *pre_off, const uint8_t *ids, uint8_t *flags_out) {
+    if (n == 0) return SW_OK;
+    auto src = [&](int j) { return sel ? sel[j] : j; };
+    size_t mbytes = 0, pbytes = 0;
+    for (int j = 0; j < n; j++) {
+        mbytes += (size_t)(msg_off[src(j) + 1] - msg_off[src(j)]);
+        pbytes += (size_t)(pre_off[src(j) + 1] - pre_off[src(j)]);
+    }
+    // the block: creator | msg_off | pre_off | sig | ids | msg | pre, each section 256-byte aligned
+    const size_t o_moff = align256(sizeof(int32_t) * n), o_poff = o_moff + align256(sizeof(int64_t) * (n + 1));
+    const size_t o_sig = o_poff + align256(sizeof(int64_t) * (n + 1)), o_ids = o_sig + align256((size_t)64 * n);
+    const size_t o_msg = o_ids + align256((size_t)32 * n), o_pre = o_msg + align256(mbytes), bytes = o_pre + pbytes;
+    const size_t want = std::max(bytes, 2 * e->d_vin.cap());
+    if (grow(e, bytes, e->d_vin.cap(), sized(e->d_vin, want), sized(e->h_vin, want)) < 0) return SW_E_CUDA;
+    const size_t wn = std::max((size_t)n, 2 * e->d_vflags.cap());
+    if (grow(e, n, e->d_vflags.cap(), sized(e->d_vflags, wn), sized(e->h_vflags, wn), sized(e->d_vk, 32 * wn)) < 0) return SW_E_CUDA;
+    uint8_t *h = e->h_vin.get();
+    int32_t *cr = (int32_t *)h;
+    int64_t *mo = (int64_t *)(h + o_moff), *po = (int64_t *)(h + o_poff);
+    mo[0] = po[0] = 0;
+    for (int j = 0; j < n; j++) {
+        const int i = src(j);
+        const int64_t ml = msg_off[i + 1] - msg_off[i], pl = pre_off[i + 1] - pre_off[i];
+        cr[j] = creator[i];
+        memcpy(h + o_sig + (size_t)64 * j, sig + (size_t)64 * i, 64);
+        memcpy(h + o_ids + (size_t)32 * j, ids + (size_t)32 * i, 32);
+        if (ml) memcpy(h + o_msg + mo[j], msg + msg_off[i], ml);
+        if (pl) memcpy(h + o_pre + po[j], pre + pre_off[i], pl);
+        mo[j + 1] = mo[j] + ml;
+        po[j + 1] = po[j] + pl;
+    }
+    cudaStream_t st = e->stream.get();
+    uint8_t *d = e->d_vin.get();
+    CK(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st));
+    const int nb_hash = (int)std::min<long>((n + 255) / 256, 8L * e->n_sm);
+    k_verify_hash<<<nb_hash, 256, 0, st>>>(n, (const int32_t *)d, d + o_sig, e->d_vkeys.get(), d + o_msg,
+                                           (const int64_t *)(d + o_moff), d + o_pre, (const int64_t *)(d + o_poff),
+                                           d + o_ids, e->d_vk.get(), e->d_vflags.get());
+    const int nb_curve = (int)std::min<long>((n + 127) / 128, 16L * e->n_sm);
+    k_verify_curve<<<nb_curve, 128, 0, st>>>(n, (const int32_t *)d, d + o_sig, e->d_vkey_ok.get(), e->d_vatab.get(),
+                                             e->d_vbtab.get(), e->d_vk.get(), e->d_vflags.get());
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(e->h_vflags.get(), e->d_vflags.get(), n, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    memcpy(flags_out, e->h_vflags.get(), n);
+    e->stats.kernel_launches += 2;
+    e->stats.h2d_bytes += (i64)bytes;
+    e->stats.d2h_bytes += n;
+    return SW_OK;
+}
+
 }  // namespace
 
 extern "C" {
 
-int sw_version(void) { return 204; }
+int sw_version(void) { return 205; }
 
 const char *sw_last_error(const sw_engine *e) { return e ? e->err.c_str() : g_create_error.c_str(); }
 
@@ -2013,10 +2090,14 @@ int sw_flush_l2(sw_engine *e, int64_t bytes) {
 }
 
 // ---- ingest: what Node.sync does between the wire and divide_rounds (swirld.py:129-136, utils.py:8-21), natively
-int sw_ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const uint8_t *p1_ids,
-              const int32_t *creator, const double *t, const uint8_t *sig, int32_t *index_out) {
-    if (!e || n < 0 || (n > 0 && (!ids || !p0_ids || !p1_ids || !creator || !t || !sig || !index_out))) return fail(e, SW_E_ARG, "bad argument");
-    auto key = [](const uint8_t *p) { Id32 k; memcpy(k.data(), p, 32); return k; };
+namespace {
+Id32 id_key(const uint8_t *p) { Id32 k; memcpy(k.data(), p, 32); return k; }
+
+// sw_ingest and sw_ingest_verified: `ok` (null: all) is a per-event verdict; a new event without it is skipped like an
+// invalid one, and so is whatever depends on it
+int ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const uint8_t *p1_ids,
+           const int32_t *creator, const double *t, const uint8_t *sig, const uint8_t *ok, int32_t *index_out) {
+    const auto key = id_key;
     const Id32 zero{};
     // 1. which events are new, and where each new id sits in the batch
     std::unordered_map<Id32, int, Id32Hash> inbatch;
@@ -2070,7 +2151,7 @@ int sw_ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, co
     for (int i : order) {
         const int c = creator[i];
         int a, b;
-        if (c < 0 || c >= e->M || !resolve(i, 0, a) || !resolve(i, 1, b)) continue;
+        if ((ok && !ok[i]) || c < 0 || c >= e->M || !resolve(i, 0, a) || !resolve(i, 1, b)) continue;
         if (a < 0 && b < 0) { if (head[c] >= 0) continue; }                         // a second root: fork
         else if (a < 0 || b < 0 || creator_of(a) != c || creator_of(b) == c || head[c] != a) continue;   // swirld.py:104-108 + fork-free
         if (next_index >= e->cap) return fail(e, SW_E_CAPACITY, "capacity_events=%d exceeded", e->cap);
@@ -2093,6 +2174,75 @@ int sw_ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, co
     for (int i = 0; i < n; i++)
         if (index_out[i] < 0) { auto it = e->ids.find(key(ids + (size_t)32 * i)); index_out[i] = it == e->ids.end() ? -1 : it->second; }
     return m;
+}
+}  // namespace
+
+int sw_ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const uint8_t *p1_ids,
+              const int32_t *creator, const double *t, const uint8_t *sig, int32_t *index_out) {
+    if (!e || n < 0 || (n > 0 && (!ids || !p0_ids || !p1_ids || !creator || !t || !sig || !index_out))) return fail(e, SW_E_ARG, "bad argument");
+    return ingest(e, n, ids, p0_ids, p1_ids, creator, t, sig, nullptr, index_out);
+}
+
+int sw_set_member_keys(sw_engine *e, const uint8_t *pk) {
+    if (!e || !pk) return fail(e, SW_E_ARG, "bad argument");
+    CK(cudaSetDevice(e->device));
+    const size_t M = e->M;
+    if (grow(e, M, e->d_vkey_ok.cap(), sized(e->d_vkeys, 32 * M), sized(e->d_vkey_ok, M), sized(e->d_vatab, swv::TAB * M)) < 0) return SW_E_CUDA;
+    cudaStream_t st = e->stream.get();
+    if (!e->have_base) {            // [1..15]B, from the base point's encoding, once per engine
+        if (grow(e, swv::TAB, e->d_vbtab.cap(), sized(e->d_vbtab, swv::TAB)) < 0) return SW_E_CUDA;
+        k_verify_tables<<<1, 32, 0, st>>>(1, nullptr, nullptr, e->d_vbtab.get());
+        e->stats.kernel_launches += 1;
+    }
+    CK(cudaMemcpyAsync(e->d_vkeys.get(), pk, 32 * M, cudaMemcpyHostToDevice, st));
+    k_verify_tables<<<(int)((M + 63) / 64), 64, 0, st>>>((int)M, e->d_vkeys.get(), e->d_vkey_ok.get(), e->d_vatab.get());
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    e->stats.kernel_launches += 1;
+    e->stats.h2d_bytes += (i64)(32 * M);
+    e->have_keys = e->have_base = true;
+    return SW_OK;
+}
+
+int sw_verify_events(sw_engine *e, int n, const int32_t *creator, const uint8_t *sig,
+                     const uint8_t *msg, const int64_t *msg_off, const uint8_t *pre, const int64_t *pre_off,
+                     const uint8_t *ids, uint8_t *flags_out) {
+    if (!e || n < 0 || (n > 0 && (!creator || !sig || !msg_off || !pre_off || !ids || !flags_out)))
+        return fail(e, SW_E_ARG, "bad argument");
+    CK(cudaSetDevice(e->device));
+    if (n > 0 && ((!msg && msg_off[n] > 0) || (!pre && pre_off[n] > 0))) return fail(e, SW_E_ARG, "bad argument");
+    const int64_t zero = 0;
+    const int rc = verify_args(e, "sw_verify_events", n, creator, n ? msg_off : &zero, n ? pre_off : &zero, true);
+    return rc < 0 ? rc : verify_run(e, n, nullptr, creator, sig, msg, msg_off, pre, pre_off, ids, flags_out);
+}
+
+int sw_ingest_verified(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const uint8_t *p1_ids,
+                       const int32_t *creator, const double *t, const uint8_t *sig,
+                       const uint8_t *msg, const int64_t *msg_off, const uint8_t *pre, const int64_t *pre_off,
+                       int32_t *index_out) {
+    if (!e || n < 0 || (n > 0 && (!ids || !p0_ids || !p1_ids || !creator || !t || !sig || !index_out || !msg_off || !pre_off)))
+        return fail(e, SW_E_ARG, "bad argument");
+    CK(cudaSetDevice(e->device));
+    if (n > 0 && ((!msg && msg_off[n] > 0) || (!pre && pre_off[n] > 0))) return fail(e, SW_E_ARG, "bad argument");
+    const int64_t zero = 0;
+    int rc = verify_args(e, "sw_ingest_verified", n, creator, n ? msg_off : &zero, n ? pre_off : &zero, false);
+    if (rc < 0) return rc;
+    // the new ids (the first event of each, as ingest counts it) whose creator is a member: only they are verified; a
+    // new event with another creator is skipped by ingest anyway
+    std::vector<int> fresh;
+    {
+        std::unordered_map<Id32, int, Id32Hash> seen;
+        for (int i = 0; i < n; i++) {
+            const Id32 k = id_key(ids + (size_t)32 * i);
+            if (e->ids.count(k) || !seen.emplace(k, i).second) continue;
+            if (creator[i] >= 0 && creator[i] < e->M) fresh.push_back(i);
+        }
+    }
+    std::vector<uint8_t> flags(fresh.size()), ok(n, 1);
+    rc = verify_run(e, (int)fresh.size(), fresh.data(), creator, sig, msg, msg_off, pre, pre_off, ids, flags.data());
+    if (rc < 0) return rc;
+    for (size_t j = 0; j < fresh.size(); j++) ok[fresh[j]] = flags[j] == 3;
+    return ingest(e, n, ids, p0_ids, p1_ids, creator, t, sig, ok.data(), index_out);
 }
 
 int sw_lookup(sw_engine *e, int n, const uint8_t *ids, int32_t *index_out) {

@@ -28,6 +28,7 @@ SYMBOLS = [
     "sw_save", "sw_load", "sw_members", "sw_ingest", "sw_lookup", "sw_batch_divide_rounds",
     "sw_batch_decide_fame", "sw_batch_find_order", "sw_batch_append",
     "sw_get_consensus_times", "sw_get_rounds_received", "sw_find_order_out", "sw_batch_find_order_out",
+    "sw_set_member_keys", "sw_verify_events", "sw_ingest_verified",
 ]
 
 
@@ -90,6 +91,9 @@ def load_library(path: str = LIB_PATH):
     L.sw_members.argtypes = [vp]
     L.sw_ingest.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp]
     L.sw_lookup.argtypes = [vp, i32, vp, vp]
+    L.sw_set_member_keys.argtypes = [vp, vp]
+    L.sw_verify_events.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.sw_ingest_verified.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.sw_batch_divide_rounds.argtypes = [vp, i32, vp, vp]
     L.sw_batch_decide_fame.argtypes = [vp, i32, vp, i32, vp]
     L.sw_batch_find_order.argtypes = [vp, i32, vp, vp, vp]
@@ -104,6 +108,15 @@ def load_library(path: str = LIB_PATH):
 
 def _ptr(a: np.ndarray):
     return a.ctypes.data_as(C.c_void_p)
+
+
+def _packed(items):
+    """A sequence of bytes as (their concatenation, n+1 int64 offsets)."""
+    items = [bytes(b) for b in items]
+    off = np.zeros(len(items) + 1, np.int64)
+    off[1:] = np.cumsum([len(b) for b in items])
+    cat = np.frombuffer(b"".join(items), np.uint8) if off[-1] else np.zeros(1, np.uint8)
+    return np.ascontiguousarray(cat), off
 
 
 class Engine:
@@ -188,9 +201,11 @@ class Engine:
         assert p1.shape[0] == n and creator.shape[0] == n and t.shape[0] == n and sig.size == 64 * n
         self._chk(self._lib.sw_append(self._h, n, _ptr(p0), _ptr(p1), _ptr(creator), _ptr(t), _ptr(sig)))
 
-    def ingest(self, ids, p0_ids, p1_ids, creator, t, sig):
+    def ingest(self, ids, p0_ids, p1_ids, creator, t, sig, msgs=None, preimages=None):
         """sw_ingest: events named by 32-byte ids (parents by id, zeros = none), any order; returns the arrival index
-        of every input event (-1 = rejected) and the number appended."""
+        of every input event (-1 = rejected) and the number appended.  With msgs (the signed bytes, dumps(ev[:-1])) and
+        preimages (dumps(ev), whose BLAKE2b is the id) it is sw_ingest_verified: a new event whose signature or id
+        fails on the GPU is rejected too, with whatever depends on it."""
         ids = np.ascontiguousarray(ids, np.uint8).reshape(-1, 32)
         n = ids.shape[0]
         p0_ids = np.ascontiguousarray(p0_ids, np.uint8).reshape(n, 32)
@@ -198,8 +213,38 @@ class Engine:
         creator = np.ascontiguousarray(creator, np.int32); t = np.ascontiguousarray(t, np.float64)
         sig = np.ascontiguousarray(sig, np.uint8).reshape(n, 64)
         out = np.empty(n, np.int32)
+        if msgs is not None and preimages is not None:
+            assert len(msgs) == n and len(preimages) == n
+            (msg, moff), (pre, poff) = _packed(msgs), _packed(preimages)
+            m = self._chk(self._lib.sw_ingest_verified(self._h, n, _ptr(ids), _ptr(p0_ids), _ptr(p1_ids), _ptr(creator),
+                                                       _ptr(t), _ptr(sig), _ptr(msg), _ptr(moff), _ptr(pre), _ptr(poff),
+                                                       _ptr(out)))
+            return out, m
         m = self._chk(self._lib.sw_ingest(self._h, n, _ptr(ids), _ptr(p0_ids), _ptr(p1_ids), _ptr(creator), _ptr(t), _ptr(sig), _ptr(out)))
         return out, m
+
+    def set_member_keys(self, pks):
+        """sw_set_member_keys: the members' Ed25519 public keys, an (M, 32) uint8 array or M values of 32 bytes."""
+        if isinstance(pks, np.ndarray):
+            a = np.ascontiguousarray(pks, np.uint8).reshape(-1)
+        else:
+            a = np.frombuffer(b"".join(bytes(p) for p in pks), np.uint8).copy()
+        assert a.size == 32 * self.M, "need %d keys of 32 bytes" % self.M
+        self._chk(self._lib.sw_set_member_keys(self._h, _ptr(a)))
+
+    def verify_events(self, creator, sig, msgs, preimages, ids):
+        """sw_verify_events: per event, bit 0 = sig is creator's valid Ed25519 signature of msgs[i] (libsodium's
+        verdict), bit 1 = BLAKE2b-256(preimages[i]) == ids[i].  Returns the flags as a uint8 array."""
+        creator = np.ascontiguousarray(creator, np.int32)
+        n = creator.shape[0]
+        sig = np.ascontiguousarray(sig, np.uint8).reshape(n, 64) if n else np.zeros((1, 64), np.uint8)
+        ids = np.ascontiguousarray(ids, np.uint8).reshape(n, 32) if n else np.zeros((1, 32), np.uint8)
+        assert len(msgs) == n and len(preimages) == n
+        (msg, moff), (pre, poff) = _packed(msgs), _packed(preimages)
+        out = np.zeros(max(n, 1), np.uint8)
+        self._chk(self._lib.sw_verify_events(self._h, n, _ptr(creator), _ptr(sig), _ptr(msg), _ptr(moff), _ptr(pre),
+                                             _ptr(poff), _ptr(ids), _ptr(out)))
+        return out[:n]
 
     def lookup(self, ids):
         ids = np.ascontiguousarray(ids, np.uint8).reshape(-1, 32)
