@@ -231,6 +231,27 @@ int sw_ingest_verified(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p
                        const int32_t *creator, const double *t, const uint8_t *sig,
                        const uint8_t *msg, const int64_t *msg_off, const uint8_t *pre, const int64_t *pre_off,
                        int32_t *index_out);
+/* sw_ingest_verified for B independent node-views in one call (each node of the simulation ingests the reply of its
+ * sync, swirld.py:129-136): view v ingests rows offsets[v] .. offsets[v+1] of the concatenated columns (as
+ * sw_batch_append lays them out); msg_off / pre_off have offsets[B] + 1 entries over the whole concatenation, monotone
+ * from 0, and index_out is laid out like the rows.  Each view ends with exactly the state, index_out and count its own
+ * sw_ingest_verified of its rows would have given it.  The events the views would verify are verified ONCE per distinct
+ * event: copies in several views share one verdict when their creator has the same 32-byte key in each view's key set
+ * and their id, signature, message and preimage are byte-identical (a copy tampered under the same id is another event).
+ * All of them go to the GPU in one copy and two kernels on the first engine's stream, with one synchronisation;
+ * *n_verified_out (may be NULL) gets their number.  The accepted events append as sw_batch_append appends them.  The
+ * views may differ in M and key sets; they share one device.  Launches and timings are charged to the first engine.
+ * Argument errors refuse the whole call before anything runs, leave count_out unwritten and put the message in the
+ * first engine's sw_last_error: B < 1, a NULL or repeated engine, views on different devices or peer-connected to other
+ * GPUs (SW_E_UNSUPPORTED), a view with no member keys, bad row or byte offsets (SW_E_ARG).  A view's own failure (a
+ * batch that is not a DAG, SW_E_ARG; capacity, SW_E_CAPACITY) changes nothing of that view: count_out[v] gets the code
+ * and the message is in that view's sw_last_error; the other views ingest normally (count_out[v] = events appended).
+ * Returns SW_OK when every view succeeded, else the first failing view's code. */
+int sw_batch_ingest_verified(sw_engine *const *engines, int B, const int *offsets,
+                             const uint8_t *ids, const uint8_t *p0_ids, const uint8_t *p1_ids,
+                             const int32_t *creator, const double *t, const uint8_t *sig,
+                             const uint8_t *msg, const int64_t *msg_off, const uint8_t *pre, const int64_t *pre_off,
+                             int32_t *index_out, int32_t *count_out, int32_t *n_verified_out);
 int sw_lookup(sw_engine *e, int n, const uint8_t *ids, int32_t *index_out);   /* id -> arrival index, -1 unknown */
 
 /* ---- checkpoint / resume (the reference keeps its state in memory only and uses pickle on the wire, swirld.py:129,160):

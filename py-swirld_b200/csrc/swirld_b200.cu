@@ -21,6 +21,7 @@
 #include <array>
 #include <string>
 #include <unordered_map>
+#include <unordered_set>
 #include <utility>
 #include <vector>
 
@@ -249,8 +250,10 @@ struct sw_engine {
     std::vector<Event> pool;      // timing events no span or append holds
     std::unordered_map<Id32, int32_t, Id32Hash> ids;     // sw_ingest: event id -> arrival index
     // sw_verify_events (swirld_verify.cuh): the members' keys, libsodium's verdict on each key alone, [1..15](-A) per
-    // member and [1..15]B; a call's inputs go over in one copy from h_vin, and its flags come back through h_vflags
+    // member and [1..15]B; a call's inputs go over in one copy from h_vin, and its flags come back through h_vflags.
+    // h_vkeys: the keys again on the host, where sw_batch_ingest_verified compares the views' keys
     bool have_keys = false, have_base = false;
+    std::vector<uint8_t> h_vkeys;
     Mem<uint8_t> d_vkeys, d_vkey_ok;
     Mem<swv::gc> d_vatab, d_vbtab;
     Pinned<uint8_t> h_vin, h_vflags;
@@ -1537,8 +1540,11 @@ int verify_args(sw_engine *e, const char *what, int n, const int32_t *creator, c
 
 // Verify events sel[0..n) of the caller's columns (sel null: events 0..n), flags into flags_out[0..n): the columns
 // are packed into one pinned block and go over in one copy; both kernels run on the compute stream; one sync.
-int verify_run(sw_engine *e, int n, const int *sel, const int32_t *creator, const uint8_t *sig, const uint8_t *msg,
-               const int64_t *msg_off, const uint8_t *pre, const int64_t *pre_off, const uint8_t *ids, uint8_t *flags_out) {
+// Keys: event j's creator is a member of views[set[j]], one of nviews engines on the device of e (set null: of e); the
+// views' key sets then go over in the same block, and the kernels read event j's from there.
+int verify_run(sw_engine *e, int n, const int *sel, const int *set, sw_engine *const *views, int nviews,
+               const int32_t *creator, const uint8_t *sig, const uint8_t *msg, const int64_t *msg_off, const uint8_t *pre,
+               const int64_t *pre_off, const uint8_t *ids, uint8_t *flags_out) {
     if (n == 0) return SW_OK;
     auto src = [&](int j) { return sel ? sel[j] : j; };
     size_t mbytes = 0, pbytes = 0;
@@ -1546,8 +1552,11 @@ int verify_run(sw_engine *e, int n, const int *sel, const int32_t *creator, cons
         mbytes += (size_t)(msg_off[src(j) + 1] - msg_off[src(j)]);
         pbytes += (size_t)(pre_off[src(j) + 1] - pre_off[src(j)]);
     }
-    // the block: creator | msg_off | pre_off | sig | ids | msg | pre, each section 256-byte aligned
-    const size_t o_moff = align256(sizeof(int32_t) * n), o_poff = o_moff + align256(sizeof(int64_t) * (n + 1));
+    // the block: creator | set | key sets | msg_off | pre_off | sig | ids | msg | pre, each section 256-byte aligned
+    // (set and key sets are empty for one engine's keys)
+    const size_t nsets = set ? (size_t)nviews : 0;
+    const size_t o_set = align256(sizeof(int32_t) * n), o_ks = o_set + align256(set ? sizeof(int32_t) * n : 0);
+    const size_t o_moff = o_ks + align256(sizeof(KeySet) * nsets), o_poff = o_moff + align256(sizeof(int64_t) * (n + 1));
     const size_t o_sig = o_poff + align256(sizeof(int64_t) * (n + 1)), o_ids = o_sig + align256((size_t)64 * n);
     const size_t o_msg = o_ids + align256((size_t)32 * n), o_pre = o_msg + align256(mbytes), bytes = o_pre + pbytes;
     const size_t want = std::max(bytes, 2 * e->d_vin.cap());
@@ -1555,13 +1564,16 @@ int verify_run(sw_engine *e, int n, const int *sel, const int32_t *creator, cons
     const size_t wn = std::max((size_t)n, 2 * e->d_vflags.cap());
     if (grow(e, n, e->d_vflags.cap(), sized(e->d_vflags, wn), sized(e->h_vflags, wn), sized(e->d_vk, 32 * wn)) < 0) return SW_E_CUDA;
     uint8_t *h = e->h_vin.get();
-    int32_t *cr = (int32_t *)h;
+    int32_t *cr = (int32_t *)h, *vs = (int32_t *)(h + o_set);
+    KeySet *ks = (KeySet *)(h + o_ks);
+    for (size_t v = 0; v < nsets; v++) ks[v] = KeySet{views[v]->d_vkeys.get(), views[v]->d_vkey_ok.get(), views[v]->d_vatab.get()};
     int64_t *mo = (int64_t *)(h + o_moff), *po = (int64_t *)(h + o_poff);
     mo[0] = po[0] = 0;
     for (int j = 0; j < n; j++) {
         const int i = src(j);
         const int64_t ml = msg_off[i + 1] - msg_off[i], pl = pre_off[i + 1] - pre_off[i];
         cr[j] = creator[i];
+        if (set) vs[j] = set[j];
         memcpy(h + o_sig + (size_t)64 * j, sig + (size_t)64 * i, 64);
         memcpy(h + o_ids + (size_t)32 * j, ids + (size_t)32 * i, 32);
         if (ml) memcpy(h + o_msg + mo[j], msg + msg_off[i], ml);
@@ -1572,13 +1584,21 @@ int verify_run(sw_engine *e, int n, const int *sel, const int32_t *creator, cons
     cudaStream_t st = e->stream.get();
     uint8_t *d = e->d_vin.get();
     CK(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st));
+    const int32_t *dcr = (const int32_t *)d, *dset = set ? (const int32_t *)(d + o_set) : nullptr;
+    const int64_t *dmo = (const int64_t *)(d + o_moff), *dpo = (const int64_t *)(d + o_poff);
     const int nb_hash = (int)std::min<long>((n + 255) / 256, 8L * e->n_sm);
-    k_verify_hash<<<nb_hash, 256, 0, st>>>(n, (const int32_t *)d, d + o_sig, e->d_vkeys.get(), d + o_msg,
-                                           (const int64_t *)(d + o_moff), d + o_pre, (const int64_t *)(d + o_poff),
-                                           d + o_ids, e->d_vk.get(), e->d_vflags.get());
     const int nb_curve = (int)std::min<long>((n + 127) / 128, 16L * e->n_sm);
-    k_verify_curve<<<nb_curve, 128, 0, st>>>(n, (const int32_t *)d, d + o_sig, e->d_vkey_ok.get(), e->d_vatab.get(),
-                                             e->d_vbtab.get(), e->d_vk.get(), e->d_vflags.get());
+    if (set) {
+        const KeySet *dks = (const KeySet *)(d + o_ks);
+        k_verify_hash<<<nb_hash, 256, 0, st>>>(n, dcr, dset, dks, d + o_sig, d + o_msg, dmo, d + o_pre, dpo, d + o_ids,
+                                               e->d_vk.get(), e->d_vflags.get());
+        k_verify_curve<<<nb_curve, 128, 0, st>>>(n, dcr, dset, dks, d + o_sig, e->d_vbtab.get(), e->d_vk.get(), e->d_vflags.get());
+    } else {
+        const KeySet K{e->d_vkeys.get(), e->d_vkey_ok.get(), e->d_vatab.get()};
+        k_verify_hash<<<nb_hash, 256, 0, st>>>(n, dcr, dset, K, d + o_sig, d + o_msg, dmo, d + o_pre, dpo, d + o_ids,
+                                               e->d_vk.get(), e->d_vflags.get());
+        k_verify_curve<<<nb_curve, 128, 0, st>>>(n, dcr, dset, K, d + o_sig, e->d_vbtab.get(), e->d_vk.get(), e->d_vflags.get());
+    }
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(e->h_vflags.get(), e->d_vflags.get(), n, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -1589,11 +1609,57 @@ int verify_run(sw_engine *e, int n, const int *sel, const int32_t *creator, cons
     return SW_OK;
 }
 
+// Node.add_event for B node-views whose arguments are checked (sw_batch_append, sw_batch_ingest_verified): view v
+// appends rows offsets[v] .. offsets[v+1] of the concatenated columns.  Every view is validated as sw_append validates
+// it; the views of at most STAGE_EVENTS events go over packed in ONE block (their parameters first) and are scattered by
+// ONE k_unpack, on the first engine's copy stream; larger views make the copies their sw_append makes, on their own copy
+// streams.  rc_out[v] is view v's code; returns the first failing view's code (SW_E_CUDA: the call stopped there).
+int append_views(sw_engine *const *engines, int B, const int *offsets, const int32_t *p0, const int32_t *p1,
+                 const int32_t *creator, const double *t, const uint8_t *sig, int32_t *rc_out) {
+    sw_engine *e = engines[0];
+    // 1. every view's checks; a view that fails them keeps its state and its error
+    std::vector<int> packed;
+    size_t bytes = 0;
+    int first_err = SW_OK;
+    for (int v = 0; v < B; v++) {
+        sw_engine *x = engines[v];
+        const int o = offsets[v], n = offsets[v + 1] - o;
+        int r = n > 0 ? append_validate(x, n, p0 + o, p1 + o, creator + o) : SW_OK;
+        rc_out[v] = r;
+        if (r < 0) { if (first_err == SW_OK) first_err = r; continue; }
+        if (n == 0) continue;
+        if (n <= sw_engine::STAGE_EVENTS) { packed.push_back(v); bytes += (unpack_bytes(n) + 15) & ~(size_t)15; }
+        else if (append_copy(x, n, p0 + o, p1 + o, creator + o, t + o, sig + (size_t)64 * o) < 0 || append_commit(x, n, x->copy_stream.get()) < 0) {
+            e->err = x->err;
+            return SW_E_CUDA;
+        }
+    }
+    if (packed.empty()) return first_err;
+    bytes += align256(sizeof(UnpackParams) * packed.size());
+    // 2. the packed views: one slot of the first engine's ring, one copy, one scatter kernel
+    const int si = stage_slot(e, bytes);
+    if (si < 0) return si;
+    uint8_t *hs = e->h_stage.get() + e->stage_bytes() * si, *ds = e->d_stage.get() + e->stage_bytes() * si;
+    UnpackParams *U = reinterpret_cast<UnpackParams *>(hs);
+    size_t off = align256(sizeof(UnpackParams) * packed.size());
+    for (size_t i = 0; i < packed.size(); i++) {
+        sw_engine *x = engines[packed[i]];
+        const int o = offsets[packed[i]], n = offsets[packed[i] + 1] - o;
+        U[i] = append_pack(x, n, p0 + o, p1 + o, creator + o, t + o, sig + (size_t)64 * o, hs + off, ds + off);
+        off += (unpack_bytes(n) + 15) & ~(size_t)15;
+    }
+    if (unpack_staged(e, si, off, reinterpret_cast<const UnpackParams *>(ds), (int)packed.size()) < 0) return SW_E_CUDA;
+    // each view's pending-append event comes from its own pool (wait_appends returns it there)
+    for (int v : packed)
+        if (append_commit(engines[v], offsets[v + 1] - offsets[v], e->copy_stream.get()) < 0) { e->err = engines[v]->err; return SW_E_CUDA; }
+    return first_err;
+}
+
 }  // namespace
 
 extern "C" {
 
-int sw_version(void) { return 205; }
+int sw_version(void) { return 206; }
 
 const char *sw_last_error(const sw_engine *e) { return e ? e->err.c_str() : g_create_error.c_str(); }
 
@@ -1668,9 +1734,7 @@ int sw_append(sw_engine *e, int n, const int32_t *p0, const int32_t *p1, const i
     return append_commit(e, n, e->copy_stream.get());
 }
 
-// Node.add_event for B node-views in one call.  Every view is validated as sw_append validates it; the views of at most
-// STAGE_EVENTS events go over packed in ONE block (their parameters first) and are scattered by ONE k_unpack, on the
-// first engine's copy stream; larger views make the copies their sw_append makes, on their own copy streams.
+// Node.add_event for B node-views in one call (append_views)
 int sw_batch_append(sw_engine *const *engines, int B, const int *offsets, const int32_t *p0, const int32_t *p1,
                     const int32_t *creator, const double *t, const uint8_t *sig, int32_t *rc_out) {
     sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
@@ -1683,42 +1747,7 @@ int sw_batch_append(sw_engine *const *engines, int B, const int *offsets, const 
             return fail(e, SW_E_ARG, "sw_batch_append: offsets[%d] = %d > offsets[%d] = %d", v, offsets[v], v + 1, offsets[v + 1]);
     if (offsets[B] > offsets[0] && (!p0 || !p1 || !creator || !t || !sig)) return fail(e, SW_E_ARG, "bad argument");
     CK(cudaSetDevice(e->device));
-    // 1. every view's checks; a view that fails them keeps its state and its error
-    std::vector<int> packed;
-    size_t bytes = 0;
-    int first_err = SW_OK;
-    for (int v = 0; v < B; v++) {
-        sw_engine *x = engines[v];
-        const int o = offsets[v], n = offsets[v + 1] - o;
-        int r = n > 0 ? append_validate(x, n, p0 + o, p1 + o, creator + o) : SW_OK;
-        rc_out[v] = r;
-        if (r < 0) { if (first_err == SW_OK) first_err = r; continue; }
-        if (n == 0) continue;
-        if (n <= sw_engine::STAGE_EVENTS) { packed.push_back(v); bytes += (unpack_bytes(n) + 15) & ~(size_t)15; }
-        else if (append_copy(x, n, p0 + o, p1 + o, creator + o, t + o, sig + (size_t)64 * o) < 0 || append_commit(x, n, x->copy_stream.get()) < 0) {
-            e->err = x->err;
-            return SW_E_CUDA;
-        }
-    }
-    if (packed.empty()) return first_err;
-    bytes += align256(sizeof(UnpackParams) * packed.size());
-    // 2. the packed views: one slot of the first engine's ring, one copy, one scatter kernel
-    const int si = stage_slot(e, bytes);
-    if (si < 0) return si;
-    uint8_t *hs = e->h_stage.get() + e->stage_bytes() * si, *ds = e->d_stage.get() + e->stage_bytes() * si;
-    UnpackParams *U = reinterpret_cast<UnpackParams *>(hs);
-    size_t off = align256(sizeof(UnpackParams) * packed.size());
-    for (size_t i = 0; i < packed.size(); i++) {
-        sw_engine *x = engines[packed[i]];
-        const int o = offsets[packed[i]], n = offsets[packed[i] + 1] - o;
-        U[i] = append_pack(x, n, p0 + o, p1 + o, creator + o, t + o, sig + (size_t)64 * o, hs + off, ds + off);
-        off += (unpack_bytes(n) + 15) & ~(size_t)15;
-    }
-    if (unpack_staged(e, si, off, reinterpret_cast<const UnpackParams *>(ds), (int)packed.size()) < 0) return SW_E_CUDA;
-    // each view's pending-append event comes from its own pool (wait_appends returns it there)
-    for (int v : packed)
-        if (append_commit(engines[v], offsets[v + 1] - offsets[v], e->copy_stream.get()) < 0) { e->err = engines[v]->err; return SW_E_CUDA; }
-    return first_err;
+    return append_views(engines, B, offsets, p0, p1, creator, t, sig, rc_out);
 }
 
 int sw_divide_rounds(sw_engine *e, int first, int n) {
@@ -2093,10 +2122,22 @@ int sw_flush_l2(sw_engine *e, int64_t bytes) {
 namespace {
 Id32 id_key(const uint8_t *p) { Id32 k; memcpy(k.data(), p, 32); return k; }
 
-// sw_ingest and sw_ingest_verified: `ok` (null: all) is a per-event verdict; a new event without it is skipped like an
-// invalid one, and so is whatever depends on it
-int ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const uint8_t *p1_ids,
-           const int32_t *creator, const double *t, const uint8_t *sig, const uint8_t *ok, int32_t *index_out) {
+// What an ingest appends, decided before anything is appended: the accepted events' columns in parents-first order,
+// and the input row each comes from
+struct IngestPlan {
+    std::vector<int32_t> p0, p1, cr, src;
+    std::vector<double> t;
+    std::vector<uint8_t> sig;
+    int size() const { return (int)src.size(); }
+};
+
+// The plan of sw_ingest and sw_ingest_verified (and of each view of sw_batch_ingest_verified): `ok` (null: all) is a
+// per-event verdict; a new event without it is skipped like an invalid one, and so is whatever depends on it.
+// index_out gets the known ids' indices and -1 for the rest.  Nothing of the engine changes; the accepted events take
+// the indices n_events, n_events + 1, ... in plan order.
+int ingest_plan(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const uint8_t *p1_ids,
+                const int32_t *creator, const double *t, const uint8_t *sig, const uint8_t *ok, int32_t *index_out,
+                IngestPlan &P) {
     const auto key = id_key;
     const Id32 zero{};
     // 1. which events are new, and where each new id sits in the batch
@@ -2135,8 +2176,6 @@ int ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const
     }
     // 3. validate in that order against a scratch copy of the chain heads; what fails (and what hangs below it) is skipped
     std::vector<int32_t> head(e->h_head), bidx(n, -1), bcreator;
-    std::vector<int32_t> c_p0, c_p1, c_cr, src;
-    std::vector<double> c_t;
     int next_index = e->n_events;
     auto resolve = [&](int i, int which, int &out) -> bool {        // parent id -> arrival index (-1: no parent)
         const Id32 k = key((which ? p1_ids : p0_ids) + (size_t)32 * i);
@@ -2158,21 +2197,35 @@ int ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const
         bidx[i] = next_index++;
         head[c] = bidx[i];
         bcreator.push_back(c);
-        c_p0.push_back(a); c_p1.push_back(b); c_cr.push_back(c); c_t.push_back(t[i]); src.push_back(i);
+        P.p0.push_back(a); P.p1.push_back(b); P.cr.push_back(c); P.t.push_back(t[i]); P.src.push_back(i);
     }
-    // 4. one sw_append for the accepted events, then the ids
-    const int m = (int)src.size();
+    P.sig.resize((size_t)64 * P.size());
+    for (int j = 0; j < P.size(); j++) memcpy(P.sig.data() + (size_t)64 * j, sig + (size_t)64 * P.src[j], 64);
+    return SW_OK;
+}
+
+// After the plan's events were appended (they are the engine's last P.size()): enter their ids, and fill index_out
+void ingest_commit(sw_engine *e, int n, const uint8_t *ids, const IngestPlan &P, int32_t *index_out) {
+    const int base = e->n_events - P.size();
+    for (int j = 0; j < P.size(); j++) e->ids.emplace(id_key(ids + (size_t)32 * P.src[j]), base + j);
+    for (int i = 0; i < n; i++)
+        if (index_out[i] < 0) { auto it = e->ids.find(id_key(ids + (size_t)32 * i)); index_out[i] = it == e->ids.end() ? -1 : it->second; }
+}
+
+// sw_ingest and sw_ingest_verified: the plan, ONE sw_append, the ids
+int ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const uint8_t *p1_ids,
+           const int32_t *creator, const double *t, const uint8_t *sig, const uint8_t *ok, int32_t *index_out) {
+    IngestPlan P;
+    int rc = ingest_plan(e, n, ids, p0_ids, p1_ids, creator, t, sig, ok, index_out, P);
+    if (rc < 0) return rc;
+    const int m = P.size();
     if (m > 0) {
-        std::vector<uint8_t> c_sig((size_t)64 * m);
-        for (int j = 0; j < m; j++) memcpy(c_sig.data() + (size_t)64 * j, sig + (size_t)64 * src[j], 64);
-        int rc = sw_append(e, m, c_p0.data(), c_p1.data(), c_cr.data(), c_t.data(), c_sig.data());
+        rc = sw_append(e, m, P.p0.data(), P.p1.data(), P.cr.data(), P.t.data(), P.sig.data());
         if (rc < 0) return rc;
         // (pageable sources: the copies are staged before sw_append returns, the vectors may go)
         CK(cudaStreamSynchronize(e->copy_stream.get()));
-        for (int j = 0; j < m; j++) e->ids.emplace(key(ids + (size_t)32 * src[j]), bidx[src[j]]);
     }
-    for (int i = 0; i < n; i++)
-        if (index_out[i] < 0) { auto it = e->ids.find(key(ids + (size_t)32 * i)); index_out[i] = it == e->ids.end() ? -1 : it->second; }
+    ingest_commit(e, n, ids, P, index_out);
     return m;
 }
 }  // namespace
@@ -2194,6 +2247,7 @@ int sw_set_member_keys(sw_engine *e, const uint8_t *pk) {
         k_verify_tables<<<1, 32, 0, st>>>(1, nullptr, nullptr, e->d_vbtab.get());
         e->stats.kernel_launches += 1;
     }
+    e->h_vkeys.assign(pk, pk + 32 * M);
     CK(cudaMemcpyAsync(e->d_vkeys.get(), pk, 32 * M, cudaMemcpyHostToDevice, st));
     k_verify_tables<<<(int)((M + 63) / 64), 64, 0, st>>>((int)M, e->d_vkeys.get(), e->d_vkey_ok.get(), e->d_vatab.get());
     CK(cudaGetLastError());
@@ -2213,7 +2267,7 @@ int sw_verify_events(sw_engine *e, int n, const int32_t *creator, const uint8_t 
     if (n > 0 && ((!msg && msg_off[n] > 0) || (!pre && pre_off[n] > 0))) return fail(e, SW_E_ARG, "bad argument");
     const int64_t zero = 0;
     const int rc = verify_args(e, "sw_verify_events", n, creator, n ? msg_off : &zero, n ? pre_off : &zero, true);
-    return rc < 0 ? rc : verify_run(e, n, nullptr, creator, sig, msg, msg_off, pre, pre_off, ids, flags_out);
+    return rc < 0 ? rc : verify_run(e, n, nullptr, nullptr, nullptr, 0, creator, sig, msg, msg_off, pre, pre_off, ids, flags_out);
 }
 
 int sw_ingest_verified(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const uint8_t *p1_ids,
@@ -2239,10 +2293,108 @@ int sw_ingest_verified(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p
         }
     }
     std::vector<uint8_t> flags(fresh.size()), ok(n, 1);
-    rc = verify_run(e, (int)fresh.size(), fresh.data(), creator, sig, msg, msg_off, pre, pre_off, ids, flags.data());
+    rc = verify_run(e, (int)fresh.size(), fresh.data(), nullptr, nullptr, 0, creator, sig, msg, msg_off, pre, pre_off, ids, flags.data());
     if (rc < 0) return rc;
     for (size_t j = 0; j < fresh.size(); j++) ok[fresh[j]] = flags[j] == 3;
     return ingest(e, n, ids, p0_ids, p1_ids, creator, t, sig, ok.data(), index_out);
+}
+
+// Node.sync's ingest for B node-views in one call.  Each view plans what its sw_ingest_verified would plan, but the
+// events the views would verify go to the GPU once per distinct event, all in one block on the first engine's stream,
+// and the accepted events of every view go over through append_views.
+int sw_batch_ingest_verified(sw_engine *const *engines, int B, const int *offsets, const uint8_t *ids,
+                             const uint8_t *p0_ids, const uint8_t *p1_ids, const int32_t *creator, const double *t,
+                             const uint8_t *sig, const uint8_t *msg, const int64_t *msg_off, const uint8_t *pre,
+                             const int64_t *pre_off, int32_t *index_out, int32_t *count_out, int32_t *n_verified_out) {
+    const char *what = "sw_batch_ingest_verified";
+    sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
+    if (!e || !offsets || !count_out || !msg_off || !pre_off) return fail(e, SW_E_ARG, "bad argument");
+    int rc = check_views(engines, B, what, false);
+    if (rc < 0) return rc;
+    for (int v = 0; v < B; v++)
+        if (!engines[v]->have_keys) return fail(e, SW_E_ARG, "%s: view %d has no member keys (sw_set_member_keys)", what, v);
+    if (offsets[0] < 0) return fail(e, SW_E_ARG, "%s: offsets[0] = %d", what, offsets[0]);
+    for (int v = 0; v < B; v++)
+        if (offsets[v + 1] < offsets[v])
+            return fail(e, SW_E_ARG, "%s: offsets[%d] = %d > offsets[%d] = %d", what, v, offsets[v], v + 1, offsets[v + 1]);
+    const int N = offsets[B];
+    if (N > 0 && (!ids || !p0_ids || !p1_ids || !creator || !t || !sig || !index_out)) return fail(e, SW_E_ARG, "bad argument");
+    rc = verify_args(e, what, N, creator, msg_off, pre_off, false);
+    if (rc < 0) return rc;
+    if ((!msg && msg_off[N] > 0) || (!pre && pre_off[N] > 0)) return fail(e, SW_E_ARG, "bad argument");
+    CK(cudaSetDevice(e->device));
+
+    // 1. the events each view would verify (new to the view, the first row of their id among the view's rows, a
+    //    member's creator), merged across views when their verdict must be the same: the same key, and byte-identical
+    //    id, signature, message and preimage.  Distinct event k is first seen at row rep[k] of view vset[k].
+    std::vector<int> rep, vset, distinct(N, -1);                    // distinct[r]: row r's distinct event (-1: none)
+    std::unordered_map<Id32, std::vector<int>, Id32Hash> by_id;      // id -> its distinct events
+    auto span_eq = [](const uint8_t *base, const int64_t *off, int r, int q) {
+        const int64_t len = off[r + 1] - off[r];
+        return len == off[q + 1] - off[q] && (len == 0 || !memcmp(base + off[r], base + off[q], len));
+    };
+    auto same = [&](int r, int v, int k) {
+        const int q = rep[k];
+        return !memcmp(engines[v]->h_vkeys.data() + (size_t)32 * creator[r], engines[vset[k]]->h_vkeys.data() + (size_t)32 * creator[q], 32) &&
+               !memcmp(sig + (size_t)64 * r, sig + (size_t)64 * q, 64) && span_eq(msg, msg_off, r, q) && span_eq(pre, pre_off, r, q);
+    };
+    for (int v = 0; v < B; v++) {
+        const sw_engine *x = engines[v];
+        std::unordered_set<Id32, Id32Hash> seen;
+        for (int r = offsets[v]; r < offsets[v + 1]; r++) {
+            const Id32 k = id_key(ids + (size_t)32 * r);
+            if (x->ids.count(k) || !seen.insert(k).second || creator[r] < 0 || creator[r] >= x->M) continue;
+            std::vector<int> &cands = by_id[k];
+            int d = -1;
+            for (int c : cands) if (same(r, v, c)) { d = c; break; }
+            if (d < 0) { d = (int)rep.size(); rep.push_back(r); vset.push_back(v); cands.push_back(d); }
+            distinct[r] = d;
+        }
+    }
+    // 2. each distinct event once on the GPU
+    std::vector<uint8_t> flags(rep.size());
+    rc = verify_run(e, (int)rep.size(), rep.data(), vset.data(), engines, B, creator, sig, msg, msg_off, pre, pre_off, ids, flags.data());
+    if (rc < 0) return rc;
+    if (n_verified_out) *n_verified_out = (int32_t)rep.size();
+    // 3. every view's plan with its verdicts; a view that fails keeps its state and its error, and appends nothing
+    std::vector<IngestPlan> plans(B);
+    std::vector<int> aoff(B + 1, 0);
+    std::vector<uint8_t> ok;
+    for (int v = 0; v < B; v++) {
+        const int o = offsets[v], n = offsets[v + 1] - o;
+        ok.assign(n, 1);
+        for (int i = 0; i < n; i++) if (distinct[o + i] >= 0) ok[i] = flags[distinct[o + i]] == 3;
+        count_out[v] = ingest_plan(engines[v], n, ids + (size_t)32 * o, p0_ids + (size_t)32 * o, p1_ids + (size_t)32 * o,
+                                   creator + o, t + o, sig + (size_t)64 * o, ok.data(), index_out + o, plans[v]);
+        if (count_out[v] < 0) plans[v] = IngestPlan();
+        aoff[v + 1] = aoff[v] + plans[v].size();
+    }
+    // 4. the accepted events, concatenated, through the path of sw_batch_append
+    const int A = aoff[B];
+    std::vector<int32_t> c_p0(A), c_p1(A), c_cr(A), arc(B);
+    std::vector<double> c_t(A);
+    std::vector<uint8_t> c_sig((size_t)64 * A);
+    for (int v = 0; v < B; v++) {
+        const IngestPlan &P = plans[v];
+        const int o = aoff[v], m = P.size();
+        std::copy_n(P.p0.data(), m, c_p0.data() + o); std::copy_n(P.p1.data(), m, c_p1.data() + o); std::copy_n(P.cr.data(), m, c_cr.data() + o);
+        std::copy_n(P.t.data(), m, c_t.data() + o); std::copy_n(P.sig.data(), (size_t)64 * m, c_sig.data() + (size_t)64 * o);
+    }
+    if (A > 0 && append_views(engines, B, aoff.data(), c_p0.data(), c_p1.data(), c_cr.data(), c_t.data(), c_sig.data(), arc.data()) == SW_E_CUDA)
+        return SW_E_CUDA;
+    // (pageable sources: the large views' copies are staged once their copy streams are done, then the vectors may go)
+    for (int v = 0; v < B; v++)
+        if (aoff[v + 1] - aoff[v] > sw_engine::STAGE_EVENTS) CK(cudaStreamSynchronize(engines[v]->copy_stream.get()));
+    // 5. the ids of what each view appended
+    int first_err = SW_OK;
+    for (int v = 0; v < B; v++) {
+        if (count_out[v] >= 0 && arc[v] < 0) count_out[v] = arc[v];
+        if (count_out[v] < 0) { if (first_err == SW_OK) first_err = count_out[v]; continue; }
+        const int o = offsets[v];
+        ingest_commit(engines[v], offsets[v + 1] - o, ids + (size_t)32 * o, plans[v], index_out + o);
+        count_out[v] = plans[v].size();
+    }
+    return first_err;
 }
 
 int sw_lookup(sw_engine *e, int n, const uint8_t *ids, int32_t *index_out) {

@@ -444,16 +444,25 @@ __global__ void k_verify_tables(int count, const uint8_t *__restrict__ keys, uin
     }
 }
 
+// Where an event's key set comes from: one set for every event of the launch (by value: the single-view calls), or a
+// device array of the node-views' sets, event i's being Kv[set[i]] (sw_batch_ingest_verified).  A set is the members'
+// keys (32 bytes each), libsodium's verdict on each key alone and [1..15](-A) per member.
+struct KeySet { const uint8_t *keys; const uint8_t *key_ok; const swv::gc *Atab; };
+__device__ __forceinline__ const KeySet &key_set(const KeySet &K, const int32_t *, int) { return K; }
+__device__ __forceinline__ const KeySet &key_set(const KeySet *Kv, const int32_t *set, int i) { return Kv[set[i]]; }
+
 // The byte-serial half: k = SHA-512(R || A || M) mod L into k_out, and bit 1 of flags (the id is BLAKE2b-256 of the
 // preimage); bit 0 is cleared here and set by k_verify_curve.
-__global__ void __launch_bounds__(256) k_verify_hash(int n, const int32_t *__restrict__ creator, const uint8_t *__restrict__ sig,
-                                                     const uint8_t *__restrict__ keys, const uint8_t *__restrict__ msg,
+template <class Keys>
+__global__ void __launch_bounds__(256) k_verify_hash(int n, const int32_t *__restrict__ creator, const int32_t *__restrict__ set,
+                                                     Keys K, const uint8_t *__restrict__ sig, const uint8_t *__restrict__ msg,
                                                      const int64_t *__restrict__ msg_off, const uint8_t *__restrict__ pre,
                                                      const int64_t *__restrict__ pre_off, const uint8_t *__restrict__ ids,
                                                      uint8_t *__restrict__ k_out, uint8_t *__restrict__ flags) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const int64_t m0 = msg_off[i], p0 = pre_off[i];
-        swv::challenge(k_out + 32 * (size_t)i, sig + 64 * (size_t)i, keys + 32 * (size_t)creator[i], msg + m0, msg_off[i + 1] - m0);
+        const uint8_t *A = key_set(K, set, i).keys + 32 * (size_t)creator[i];
+        swv::challenge(k_out + 32 * (size_t)i, sig + 64 * (size_t)i, A, msg + m0, msg_off[i + 1] - m0);
         uint8_t dg[32];
         const uint8_t *p = pre + p0;
         swv::blake2b_256(dg, pre_off[i + 1] - p0, [&](int64_t j) -> uint8_t { return p[j]; });
@@ -465,15 +474,16 @@ __global__ void __launch_bounds__(256) k_verify_hash(int n, const int32_t *__res
 }
 
 // The curve half: bit 0 of flags for events whose key and S libsodium accepts and whose equation holds.
-__global__ void __launch_bounds__(128) k_verify_curve(int n, const int32_t *__restrict__ creator, const uint8_t *__restrict__ sig,
-                                                      const uint8_t *__restrict__ key_ok, const swv::gc *__restrict__ Atab,
-                                                      const swv::gc *__restrict__ Btab, const uint8_t *__restrict__ k,
-                                                      uint8_t *__restrict__ flags) {
+template <class Keys>
+__global__ void __launch_bounds__(128) k_verify_curve(int n, const int32_t *__restrict__ creator, const int32_t *__restrict__ set,
+                                                      Keys K, const uint8_t *__restrict__ sig, const swv::gc *__restrict__ Btab,
+                                                      const uint8_t *__restrict__ k, uint8_t *__restrict__ flags) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const int c = creator[i];
+        const KeySet &ks = key_set(K, set, i);
         const uint8_t *s = sig + 64 * (size_t)i;
-        if (key_ok[c] && swv::sc_canonical(s + 32) &&
-            swv::signature_equation(s, k + 32 * (size_t)i, Btab, Atab + (size_t)swv::TAB * c))
+        if (ks.key_ok[c] && swv::sc_canonical(s + 32) &&
+            swv::signature_equation(s, k + 32 * (size_t)i, Btab, ks.Atab + (size_t)swv::TAB * c))
             flags[i] |= 1;
     }
 }

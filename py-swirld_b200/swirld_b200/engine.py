@@ -28,7 +28,7 @@ SYMBOLS = [
     "sw_save", "sw_load", "sw_members", "sw_ingest", "sw_lookup", "sw_batch_divide_rounds",
     "sw_batch_decide_fame", "sw_batch_find_order", "sw_batch_append",
     "sw_get_consensus_times", "sw_get_rounds_received", "sw_find_order_out", "sw_batch_find_order_out",
-    "sw_set_member_keys", "sw_verify_events", "sw_ingest_verified",
+    "sw_set_member_keys", "sw_verify_events", "sw_ingest_verified", "sw_batch_ingest_verified",
 ]
 
 
@@ -100,6 +100,7 @@ def load_library(path: str = LIB_PATH):
     L.sw_find_order_out.argtypes = [vp, vp, i32, vp, vp, vp, i32]
     L.sw_batch_find_order_out.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, i32]
     L.sw_batch_append.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp]
+    L.sw_batch_ingest_verified.argtypes = [vp, i32] + [vp] * 14
     L.sw_save.argtypes = [vp, C.c_char_p]
     L.sw_load.argtypes = [C.c_char_p, i32, i32, P(vp)]
     _lib = L
@@ -458,6 +459,47 @@ def batch_append(engines, columns):
     if rc < 0 and not (rcs < 0).any():
         engines[0]._chk(rc)                # refused as a whole: nothing ran, rc_out was not written
     return _per_view("batch_append", engines, list(ns), rcs)
+
+
+def batch_ingest(engines, batches):
+    """sw_batch_ingest_verified: Engine.ingest with msgs and preimages for several node-views (one device) in one call;
+    batches[v] = (ids, p0_ids, p1_ids, creator, t, sig, msgs, preimages) of view v.  Every event the views would verify
+    is verified once on the GPU, however many views receive it.  Returns ([(index_out, appended) per view], the number
+    of events verified).  Argument errors raise at once; a view whose batch is not a DAG or that runs out of capacity
+    ingests nothing, and those failures raise as an ExceptionGroup after every other view has ingested (see
+    _per_view; the group's .n_verified holds the count)."""
+    B = len(engines)
+    assert len(batches) == B
+    if B == 0:
+        return [], 0
+    cols, msgs, pres = [], [], []
+    for ids, p0_ids, p1_ids, creator, t, sig, m, p in batches:
+        ids = np.asarray(ids, np.uint8).reshape(-1, 32)
+        n = ids.shape[0]
+        cols.append((ids, np.asarray(p0_ids, np.uint8).reshape(n, 32), np.asarray(p1_ids, np.uint8).reshape(n, 32),
+                     np.asarray(creator, np.int32).reshape(n), np.asarray(t, np.float64).reshape(n),
+                     np.asarray(sig, np.uint8).reshape(n, 64)))
+        assert len(m) == n and len(p) == n
+        msgs += list(m)
+        pres += list(p)
+    ns = [c[0].shape[0] for c in cols]
+    cat = [np.ascontiguousarray(np.concatenate([c[k] for c in cols]).reshape(-1)) for k in range(6)]
+    (msg, moff), (pre, poff) = _packed(msgs), _packed(pres)
+    offs = np.zeros(B + 1, np.int32)
+    offs[1:] = np.cumsum(ns)
+    out = np.empty(max(1, int(offs[-1])), np.int32)
+    cnt = np.zeros(B, np.int32)
+    nv = C.c_int32(0)
+    rc = engines[0]._lib.sw_batch_ingest_verified(_handles(engines), B, _ptr(offs), *[_ptr(a) for a in cat], _ptr(msg),
+                                                  _ptr(moff), _ptr(pre), _ptr(poff), _ptr(out), _ptr(cnt), C.byref(nv))
+    if rc < 0 and not (cnt < 0).any():
+        engines[0]._chk(rc)                # refused as a whole: nothing ran, count_out was not written
+    res = [(out[a:b].copy(), int(m)) for a, b, m in zip(offs[:-1].tolist(), offs[1:].tolist(), cnt)]
+    try:
+        return _per_view("batch_ingest", engines, res, cnt), nv.value
+    except ExceptionGroup as g:
+        g.n_verified = nv.value
+        raise
 
 
 def batch_find_order(engines, new_cs):
