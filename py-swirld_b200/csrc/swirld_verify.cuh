@@ -407,11 +407,10 @@ SWV_HDI void challenge(uint8_t *k, const uint8_t *R, const uint8_t *A, const uin
     sc_reduce512(k, h);
 }
 SWV_HD int nibble(const uint8_t *s, int w) { return (s[w >> 1] >> (4 * (w & 1))) & 15; }
-// Does [S]B + [k](-A) encode to R, and is it not of small order?  Btab = [1..15]B, Atab = [1..15](-A); S < L checked
-// by the caller.  Four bits of both scalars per step: four doublings, then at most one addition from each table.
-SWV_HDI bool signature_equation(const uint8_t *sig, const uint8_t *k, const gc *Btab, const gc *Atab) {
-    const uint8_t *S = sig + 32;
-    ge acc = ge_identity();
+// [S]B + [k](-A), Btab = [1..15]B, Atab = [1..15](-A).  Four bits of both scalars per step: four doublings, then at
+// most one addition from each table.
+SWV_HD void double_scalar(ge &acc, const uint8_t *S, const uint8_t *k, const gc *Btab, const gc *Atab) {
+    acc = ge_identity();
     bool started = false;
     for (int w = 63; w >= 0; w--) {
         if (started) { acc = ge_dbl(acc); acc = ge_dbl(acc); acc = ge_dbl(acc); acc = ge_dbl(acc); }
@@ -419,6 +418,11 @@ SWV_HDI bool signature_equation(const uint8_t *sig, const uint8_t *k, const gc *
         if (s) { acc = ge_add(acc, Btab[s - 1]); started = true; }
         if (a) { acc = ge_add(acc, Atab[a - 1]); started = true; }
     }
+}
+// Does [S]B + [k](-A) encode to R, and is it not of small order?  S < L is checked by the caller.
+SWV_HDI bool signature_equation(const uint8_t *sig, const uint8_t *k, const gc *Btab, const gc *Atab) {
+    ge acc;
+    double_scalar(acc, sig + 32, k, Btab, Atab);
     uint8_t enc[32];
     ge_encode(enc, acc);
     for (int i = 0; i < 32; i++) if (enc[i] != sig[i]) return false;

@@ -5,7 +5,7 @@ of everything, rounds, witnesses, fame, consensus, order and can_see.  The repli
 gossip's source) holds beyond the receiving view's events, with tampered copies (signature, signed bytes, preimage),
 resends of known events and duplicate rows mixed in.  Covered: shared keys at 1 to 64 views on both kernel families
 and above 64 members; one id intact in one view and tampered in another; views of different member counts and key
-sets in one call; a view whose rows are not a DAG and one out of capacity; refusals; the launches per call; and the
+sets in one call; events merged by their creator's key, not its member index; a view whose rows are not a DAG and one out of capacity; refusals; the launches per call; and the
 reference's main loop over 16 views against the oracle."""
 import ctypes as C
 import random
@@ -253,6 +253,42 @@ def test_different_key_sets():
     assert shared > 0
     assert views.engs[4].n_events == 0 and len(views.known[1]) > 0
     for v in range(5):
+        _same_state(views.engs[v], twins[v], views.seen[v])
+        _same_consensus(views.engs[v], twins[v])
+    _close(*views.engs, *twins)
+
+
+# ---------------------------------------------------------------- 3b. merging by key, not by member index
+def test_merge_by_key_not_member_index():
+    """One graph in three views.  View 1 numbers the members in another order (its keys permuted, every creator index
+    renumbered to match), so a shared event has another creator index there than in view 0 under the same key: it
+    is verified once.  View 2 holds member j's key at member i too, so member i's events have the same index as in
+    view 0 under another key: they fail there alone, with everything below them, and are not merged with view 0's."""
+    M, i, j = 8, 2, 5
+    g = Gossip(M, 500, seed=41, step=60)
+    perm = list(range(M))
+    random.Random(4).shuffle(perm)                           # the source's member c is view 1's member perm[c]
+    assert all(perm[c] != c for c in (i, j))
+    keys1 = [None] * M
+    for c in range(M):
+        keys1[perm[c]] = g.pks[c]
+    keys2 = list(g.pks)
+    keys2[i] = g.pks[j]
+    views = Views([(g, g.pks), (g, keys1), (g, keys2)], seed=6)
+    twins = _twins(views)
+    shared01 = 0
+    for _ in range(12):
+        rows = views.rows()
+        rows[1] = [x[:4] + (perm[x[4]],) for x in rows[1]]
+        alone = [views.expected_verified(rows, [v]) for v in range(3)]
+        shared01 += alone[0] + alone[1] - views.expected_verified(rows, [0, 1])
+        nv, ts = _turn(views, twins, rows)
+        assert ts == sum(alone)
+    assert shared01 > 0
+    assert len(views.known[1]) > 100
+    own2 = {x[4] for x in views.known[2].values()}
+    assert i not in own2 and j in own2
+    for v in range(3):
         _same_state(views.engs[v], twins[v], views.seen[v])
         _same_consensus(views.engs[v], twins[v])
     _close(*views.engs, *twins)

@@ -258,4 +258,37 @@ def build(seed=1):
         if j % 4 == 0:
             sig[63] &= 0x0f                                # S < 2^252 < L: canonical, so the equation decides
         cases.append(case("random", pk, bytes(sig), m))
+
+    # (the families below draw from their own generator, so the ones above stay what they were)
+    rng = random.Random(seed + 1000)
+    # 7. ground: valid signatures whose S or k has four zero nibbles at nibble w..w+3 (w = 59: S or k < 2^236, the
+    # top 16 bits below 2^252 clear), found by grinding the message, about 2^16 tries each
+    for which in ("S", "k"):
+        for w in (59, 30, 0):
+            a = rng.randrange(1, L)
+            A = base_mul(a)
+            r = rng.randrange(1, L)
+            R = base_mul(r)
+            pre = rng.randbytes(20)
+            for ctr in range(1 << 24):
+                m = pre + ctr.to_bytes(4, "little")
+                k = challenge(R, A, m)
+                S = (r + k * a) % L
+                if (((S if which == "S" else k) >> (4 * w)) & 0xFFFF) == 0:
+                    break
+            cases.append(case("ground", A, R + S.to_bytes(32, "little"), m))
+
+    # 8. s_high: canonical S in [2^252, L) (the top nibble is 1, k's is almost surely 0) with random R; no such S of a
+    # valid signature can be found, so libsodium refuses every one
+    for j in range(12):
+        pk = signers[j % len(signers)][0]
+        S = (1 << 252) + [0, 1, L - (1 << 252) - 1][j] if j < 3 else (1 << 252) + rng.randrange(L - (1 << 252))
+        R = base_mul(rng.randrange(1, L)) if j % 2 else rng.randbytes(32)
+        cases.append(case("s_high", pk, R + S.to_bytes(32, "little"), rng.randbytes(40)))
+
+    # 9. long_msg: valid signatures over messages whose SHA-512 length needs more than 16 bits
+    for n in ((1 << 16) - 1, 1 << 16, (1 << 16) + 1, 1 << 20):
+        pk, sk = signers[n % len(signers)]
+        m = rng.randbytes(n)
+        cases.append(case("long_msg", pk, sign(sk, m), m))
     return cases
