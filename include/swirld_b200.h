@@ -254,6 +254,48 @@ int sw_batch_ingest_verified(sw_engine *const *engines, int B, const int *offset
                              int32_t *index_out, int32_t *count_out, int32_t *n_verified_out);
 int sw_lookup(sw_engine *e, int n, const uint8_t *ids, int32_t *index_out);   /* id -> arrival index, -1 unknown */
 
+/* Every event's 32-byte id from the engine's id map (sw_ingest), by arrival index, for [first, first+n) of the appended
+ * events: 32 zero bytes for an event that has none (it came through sw_append).  SW_E_KEY for a range beyond them. */
+int sw_get_ids(sw_engine *e, int first, int n, uint8_t *out);
+
+/* ---- sync: the sending end of Node.sync (swirld.py:125-126, 154-161), selected on the GPU from the can_see table.
+ * The requester's summary (swirld.py:125-126): heights_out[c] = height[can_see[head][c]], the height of the latest
+ * event of member c that `head` sees, -1 where it sees none; M entries.  `head` must be divided (head < sw_n_divided),
+ * else SW_E_ARG.  Synchronous; reads what pending appends and their can_see scans write, and neither waits for nor
+ * gives up rounds computed ahead (SW_ROUNDS_AHEAD). */
+int sw_sync_summary(sw_engine *e, int head, int32_t *heights_out);
+
+/* The responder's reply to a summary (ask_sync, swirld.py:154-161, utils.py:24-34): the events a BFS from `head` over
+ * the parents the requester lacks yields, which on a fork-free graph are
+ *     {head} u { x < head : x <= can_see[head][creator x]  and  (summary[creator x] = -1  or  height[x] > summary[creator x]) }
+ * in ascending arrival index (a topological order: sw_ingest takes the rows as they are).  `head` is in the reply even
+ * when the requester has it.  PRECONDITION: summary (M entries) comes from a view of the same fork-free gossip, as
+ * sw_sync_summary makes it; for an arbitrary summary the closed form can select events the BFS does not reach.
+ * index_out[0..count) gets the events; each row pointer that is not NULL gets their columns in sw_ingest's layout:
+ * ids / p0_ids / p1_ids 32 bytes each (from the id map; parents of a root are 32 zero bytes), creator, t, sig 64 bytes.
+ * Returns the count, also in *count_out.  Errors, before anything is written: NULL engine, summary or count_out, cap < 0,
+ * a head that is not divided or a summary entry < -1 (SW_E_ARG); an id column asked for while a selected event (or a
+ * parent it names) has no id, i.e. came through sw_append (SW_E_ARG); a reply of more than `cap` events: only
+ * *count_out is written, with the exact count (SW_E_CAPACITY).  Three launches and one synchronisation; stream
+ * ordering as sw_sync_summary. */
+int sw_sync_reply(sw_engine *e, int head, const int32_t *summary, int cap, int32_t *index_out, int32_t *count_out,
+                  uint8_t *ids, uint8_t *p0_ids, uint8_t *p1_ids, int32_t *creator, double *t, uint8_t *sig);
+
+/* sw_sync_summary and sw_sync_reply for B independent node-views in one call: view v answers with heads[v].  The views
+ * share one device and may differ in M.  Summaries (in and out) are concatenated by view, M of that view each.  The
+ * reply rows come out concatenated by view, view v's at offsets_out[v] .. offsets_out[v+1] (B+1 entries), exactly as
+ * sw_batch_ingest_verified takes them, and counts_out[v] is view v's count; each view's rows equal its own single
+ * call's byte for byte.  The same launches as one single call, on the first engine's stream, and one synchronisation.
+ * Argument errors refuse the whole call before anything runs or is written (message in the first engine's
+ * sw_last_error): B < 1, a NULL or repeated engine (SW_E_ARG), views on different devices or peer-connected to other
+ * GPUs (SW_E_UNSUPPORTED), a head out of range or not divided, a summary entry < -1 (SW_E_ARG); for the reply also a
+ * missing id as sw_sync_reply (SW_E_ARG).  A total above `cap` writes only counts_out, with exact counts, and returns
+ * SW_E_CAPACITY. */
+int sw_batch_sync_summary(sw_engine *const *engines, int B, const int *heads, int32_t *out);
+int sw_batch_sync_reply(sw_engine *const *engines, int B, const int *heads, const int32_t *summaries, int cap,
+                        int32_t *offsets_out, int32_t *counts_out, int32_t *index_out, uint8_t *ids, uint8_t *p0_ids,
+                        uint8_t *p1_ids, int32_t *creator, double *t, uint8_t *sig);
+
 /* ---- checkpoint / resume (the reference keeps its state in memory only and uses pickle on the wire, swirld.py:129,160):
  * the engine's whole state -- event columns, can_see table, rounds, witness / fame tables, order -- as one binary file
  * of SoA sections.  sw_load builds a new engine from it (capacity_events 0 = the saved capacity; never less than the

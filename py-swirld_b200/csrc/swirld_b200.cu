@@ -10,6 +10,7 @@
 #include "swirld_wide.cuh"
 #include "swirld_stream.cuh"
 #include "swirld_verify.cuh"
+#include "swirld_sync.cuh"
 
 #include <cstdlib>
 #include "../../include/swirld_b200.h"
@@ -249,6 +250,12 @@ struct sw_engine {
     std::vector<TimedSpan> spans;
     std::vector<Event> pool;      // timing events no span or append holds
     std::unordered_map<Id32, int32_t, Id32Hash> ids;     // sw_ingest: event id -> arrival index
+    std::vector<Id32> id_of;                             // ... and back: arrival index -> id (zero: none), n_events or fewer
+    // sw_sync_summary / sw_sync_reply (swirld_sync.cuh, owned by the first engine of a batch): the call's parameters,
+    // tile starts and summaries go over in one copy from h_sync_in into d_sync, which also holds the tile scratch; the
+    // kernels write their output straight into h_sync_out (pinned, so the device reaches it through unified addressing)
+    Mem<char> d_sync;
+    Pinned<char> h_sync_in, h_sync_out;
     // sw_verify_events (swirld_verify.cuh): the members' keys, libsodium's verdict on each key alone, [1..15](-A) per
     // member and [1..15]B; a call's inputs go over in one copy from h_vin, and its flags come back through h_vflags.
     // h_vkeys: the keys again on the host, where sw_batch_ingest_verified compares the views' keys
@@ -1137,7 +1144,8 @@ int order_output(sw_engine *e, cudaStream_t s, int base, int cnt, const OrderOut
 // ---- several node-views per call (sw_batch_*)
 // The checks shared by the batched calls: they refuse the whole batch before anything runs (the message goes to the first
 // engine).  `same_shape`: the views must also share M and the kernel family (all but sw_batch_append).
-int check_views(sw_engine *const *engines, int B, const char *what, bool same_shape) {
+// `drain`: give up the views' round-stream pieces (every call that writes consensus state; the sync calls only read rows)
+int check_views(sw_engine *const *engines, int B, const char *what, bool same_shape, bool drain = true) {
     sw_engine *e = engines[0];
     std::vector<const sw_engine *> seen(engines, engines + B);
     for (int v = 0; v < B; v++)
@@ -1151,7 +1159,7 @@ int check_views(sw_engine *const *engines, int B, const char *what, bool same_sh
                         same_shape ? "have one member count and one kernel family" : "be");
         if (x->nranks > 1) return fail(e, SW_E_UNSUPPORTED, "%s: view %d is one rank of a multi-GPU engine", what, v);
     }
-    for (int v = 0; v < B; v++)
+    for (int v = 0; v < B && drain; v++)
         if (rs_drain(engines[v]) < 0) { e->err = engines[v]->err; return SW_E_CUDA; }
     return 0;
 }
@@ -1659,7 +1667,7 @@ int append_views(sw_engine *const *engines, int B, const int *offsets, const int
 
 extern "C" {
 
-int sw_version(void) { return 206; }
+int sw_version(void) { return 207; }
 
 const char *sw_last_error(const sw_engine *e) { return e ? e->err.c_str() : g_create_error.c_str(); }
 
@@ -1683,6 +1691,7 @@ int sw_reset(sw_engine *e) {
     CK(cudaSetDevice(e->device));
     e->h_creator.clear();
     e->ids.clear();
+    e->id_of.clear();
     e->h_stale_cum.assign(1, 0);
     int rc = reset_state(e);
     memset(&e->stats, 0, sizeof e->stats);
@@ -2207,7 +2216,12 @@ int ingest_plan(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, 
 // After the plan's events were appended (they are the engine's last P.size()): enter their ids, and fill index_out
 void ingest_commit(sw_engine *e, int n, const uint8_t *ids, const IngestPlan &P, int32_t *index_out) {
     const int base = e->n_events - P.size();
-    for (int j = 0; j < P.size(); j++) e->ids.emplace(id_key(ids + (size_t)32 * P.src[j]), base + j);
+    if (e->id_of.size() < (size_t)e->n_events) e->id_of.resize(e->n_events, Id32{});
+    for (int j = 0; j < P.size(); j++) {
+        const Id32 k = id_key(ids + (size_t)32 * P.src[j]);
+        e->ids.emplace(k, base + j);
+        e->id_of[base + j] = k;
+    }
     for (int i = 0; i < n; i++)
         if (index_out[i] < 0) { auto it = e->ids.find(id_key(ids + (size_t)32 * i)); index_out[i] = it == e->ids.end() ? -1 : it->second; }
 }
@@ -2408,6 +2422,261 @@ int sw_lookup(sw_engine *e, int n, const uint8_t *ids, int32_t *index_out) {
     return SW_OK;
 }
 
+int sw_get_ids(sw_engine *e, int first, int n, uint8_t *out) {
+    if (!e || first < 0 || n < 0 || (n > 0 && !out)) return fail(e, SW_E_ARG, "bad argument");
+    if ((i64)first + n > e->n_events) return fail(e, SW_E_KEY, "sw_get_ids: [%d,%d) out of range", first, first + n);
+    for (int i = 0; i < n; i++) {
+        const size_t x = (size_t)first + i;
+        if (x < e->id_of.size()) memcpy(out + (size_t)32 * i, e->id_of[x].data(), 32);
+        else memset(out + (size_t)32 * i, 0, 32);
+    }
+    return SW_OK;
+}
+
+// ---- sync: the sending end of Node.sync (swirld.py:125-126, 154-161, utils.py:24-34), selected on the GPU
+namespace {
+// The refusals the sync calls share: view v's head must be divided (its can_see row is complete), and its summary
+// entries heights or -1
+int sync_args(sw_engine *e, const sw_engine *x, int v, int head, const int32_t *summary, const char *what) {
+    if (head < 0 || head >= x->n_divided)
+        return fail(e, SW_E_ARG, "%s: view %d: head %d is not a divided event (%d divided)", what, v, head, x->n_divided);
+    for (int c = 0; summary && c < x->M; c++)
+        if (summary[c] < -1) return fail(e, SW_E_ARG, "%s: view %d: summary[%d] = %d < -1", what, v, c, summary[c]);
+    return 0;
+}
+
+SyncParams sync_params(const sw_engine *x, int head) {
+    SyncParams P{};
+    P.row = x->d_row.get(); P.height = x->d_height.get(); P.creator = x->d_creator.get(); P.p0 = x->d_p0.get(); P.p1 = x->d_p1.get();
+    P.t = x->d_t.get(); P.sig = x->d_sig.get(); P.M = x->M; P.head = head;
+    return P;
+}
+
+// The kernels of a sync call run on the stream of `e`, the first view's, after the copies each view has appended (the
+// rows of its divided events are written there or on its compute stream): what sw_get_can_see waits for.  No view
+// waits for or gives up a round-stream piece, which writes rounds only.
+int sync_enter(sw_engine *e, sw_engine *const *views, int B) {
+    for (int v = 0; v < B; v++)
+        if (wait_appends(views[v], -1) < 0) { e->err = views[v]->err; return SW_E_CUDA; }
+    return views_enter(e, views, B);
+}
+
+extern "C++" template <class T> T *sec(char *base, size_t off) { return reinterpret_cast<T *>(base + off); }
+
+// The summaries of B views (heads[v] divided, checked) into out, concatenated by view: one launch, one synchronisation.
+// `batch`: the parameters go over as the device array of the views (the batched instance), else by value (B = 1).
+int sync_summary(sw_engine *e, sw_engine *const *views, int B, const int *heads, int32_t *out, bool batch) {
+    size_t MT = 0;
+    for (int v = 0; v < B; v++) MT += views[v]->M;
+    const size_t in_bytes = align256(sizeof(SyncParams) * B), out_bytes = sizeof(int32_t) * MT;
+    if (grow(e, in_bytes, e->d_sync.cap(), sized(e->d_sync, std::max(in_bytes, 2 * e->d_sync.cap())),
+             sized(e->h_sync_in, std::max(in_bytes, 2 * e->d_sync.cap()))) < 0 ||
+        grow(e, out_bytes, e->h_sync_out.cap(), sized(e->h_sync_out, std::max(out_bytes, 2 * e->h_sync_out.cap()))) < 0)
+        return SW_E_CUDA;
+    if (sync_enter(e, views, B) < 0) return SW_E_CUDA;
+    int32_t *hout = sec<int32_t>(e->h_sync_out.get(), 0);
+    SyncParams *Pv = sec<SyncParams>(e->h_sync_in.get(), 0);
+    for (int v = 0, o = 0; v < B; o += views[v]->M, v++) {
+        Pv[v] = sync_params(views[v], heads[v]);
+        Pv[v].heights_out = hout + o;
+    }
+    cudaStream_t st = e->stream.get();
+    if (batch) {
+        CK(cudaMemcpyAsync(e->d_sync.get(), Pv, sizeof(SyncParams) * B, cudaMemcpyHostToDevice, st));
+        k_sync_summary<<<dim3(1, B), SY_THREADS, 0, st>>>((const SyncParams *)e->d_sync.get());
+        e->stats.h2d_bytes += sizeof(SyncParams) * B;
+    } else {
+        k_sync_summary<<<1, SY_THREADS, 0, st>>>(Pv[0]);
+    }
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    memcpy(out, hout, out_bytes);
+    e->stats.kernel_launches += 1;
+    e->stats.d2h_bytes += out_bytes;
+    return SW_OK;
+}
+
+// Where a sync reply's columns sit in the output block, for `rows` rows
+struct ReplyLayout {
+    size_t hdr, index, creator, p0, p1, t, sig, bytes;
+    ReplyLayout(int B, size_t rows) {
+        hdr = 0; index = align256(sizeof(int32_t) * (2 * B + 2)); creator = index + align256(4 * rows);
+        p0 = creator + align256(4 * rows); p1 = p0 + align256(4 * rows); t = p1 + align256(4 * rows);
+        sig = t + align256(8 * rows); bytes = sig + 64 * rows;
+    }
+};
+
+// A view's reply rows and the rows' ids, copied out of the output block: `j` rows from block row `at` to caller row
+// `to`.  The id columns need an id for every selected event and every parent it names.
+struct ReplyOut {
+    int32_t *index; uint8_t *ids, *p0_ids, *p1_ids; int32_t *creator; double *t; uint8_t *sig;
+};
+
+int reply_ids_ok(sw_engine *e, const sw_engine *x, int v, const ReplyLayout &L, char *blk, int at, int n, const ReplyOut &O,
+                 const char *what) {
+    const Id32 zero{};
+    auto has = [&](int i) { return i < 0 || ((size_t)i < x->id_of.size() && x->id_of[i] != zero); };
+    for (int j = at; j < at + n; j++) {
+        const int i = sec<int32_t>(blk, L.index)[j];
+        if ((O.ids && !has(i)) || (O.p0_ids && !has(sec<int32_t>(blk, L.p0)[j])) || (O.p1_ids && !has(sec<int32_t>(blk, L.p1)[j])))
+            return fail(e, SW_E_ARG, "%s: view %d: event %d of the reply (or a parent) has no id (it came through sw_append)", what, v, i);
+    }
+    return 0;
+}
+
+void reply_copy(const sw_engine *x, const ReplyLayout &L, char *blk, int at, int n, const ReplyOut &O) {
+    const int32_t *ix = sec<int32_t>(blk, L.index) + at, *p0 = sec<int32_t>(blk, L.p0) + at, *p1 = sec<int32_t>(blk, L.p1) + at;
+    if (O.index) memcpy(O.index + at, ix, 4 * (size_t)n);
+    if (O.creator) memcpy(O.creator + at, sec<int32_t>(blk, L.creator) + at, 4 * (size_t)n);
+    if (O.t) memcpy(O.t + at, sec<double>(blk, L.t) + at, 8 * (size_t)n);
+    if (O.sig) memcpy(O.sig + (size_t)64 * at, sec<uint8_t>(blk, L.sig) + (size_t)64 * at, (size_t)64 * n);
+    auto put = [&](uint8_t *dst, const int32_t *src) {
+        if (!dst) return;
+        for (int j = 0; j < n; j++) {
+            if (src[j] < 0) memset(dst + (size_t)32 * (at + j), 0, 32);
+            else memcpy(dst + (size_t)32 * (at + j), x->id_of[src[j]].data(), 32);
+        }
+    };
+    put(O.ids, ix); put(O.p0_ids, p0); put(O.p1_ids, p1);
+}
+
+// The replies of B views (arguments checked) to the summaries, concatenated by view: count, scan and select in three
+// launches on the first view's stream, one synchronisation.  counts_out[v] / offsets_out[0..B] are written when the
+// call succeeds; on SW_E_CAPACITY (the replies hold more than `cap` rows) only counts_out is.
+int sync_reply(sw_engine *e, sw_engine *const *views, int B, const int *heads, const int32_t *summaries, int cap,
+               int32_t *counts_out, int32_t *offsets_out, const ReplyOut &O, bool batch, const char *what) {
+    // tiles of [0, head] per view, and the most rows the replies can hold
+    std::vector<int32_t> tile0(B + 1, 0);
+    size_t MT = 0, bound = 0;
+    int maxtiles = 0, maxM = 0;
+    for (int v = 0; v < B; v++) {
+        const int nt = (heads[v] + SY_TILE) / SY_TILE;
+        tile0[v + 1] = tile0[v] + nt;
+        maxtiles = std::max(maxtiles, nt);
+        maxM = std::max(maxM, views[v]->M);
+        MT += views[v]->M;
+        bound += (size_t)heads[v] + 1;
+    }
+    const int T = tile0[B];
+    const size_t rows = std::min<size_t>((size_t)std::max(cap, 0), bound);
+    // the input block: parameters | tile starts | summaries, then the device-only scratch: tile counts | offsets | fits
+    const size_t o_t0 = align256(sizeof(SyncParams) * B), o_sum = o_t0 + align256(sizeof(int32_t) * (B + 1));
+    const size_t in_bytes = o_sum + align256(sizeof(int32_t) * MT);
+    const size_t o_cnt = in_bytes, o_off = o_cnt + align256(sizeof(int32_t) * T), o_fits = o_off + align256(sizeof(int32_t) * (T + 1));
+    const size_t dev_bytes = o_fits + 256;
+    const ReplyLayout L(B, rows);
+    if (grow(e, dev_bytes, e->d_sync.cap(), sized(e->d_sync, std::max(dev_bytes, 2 * e->d_sync.cap())),
+             sized(e->h_sync_in, std::max(dev_bytes, 2 * e->d_sync.cap()))) < 0 ||
+        grow(e, L.bytes, e->h_sync_out.cap(), sized(e->h_sync_out, std::max(L.bytes, 2 * e->h_sync_out.cap()))) < 0)
+        return SW_E_CUDA;
+    if (sync_enter(e, views, B) < 0) return SW_E_CUDA;
+    char *hin = e->h_sync_in.get(), *din = e->d_sync.get(), *blk = e->h_sync_out.get();
+    SyncParams *Pv = sec<SyncParams>(hin, 0);
+    memcpy(hin + o_t0, tile0.data(), sizeof(int32_t) * (B + 1));
+    memcpy(hin + o_sum, summaries, sizeof(int32_t) * MT);
+    for (int v = 0, m = 0; v < B; m += views[v]->M, v++) {
+        SyncParams &P = Pv[v];
+        P = sync_params(views[v], heads[v]);
+        P.summary = sec<int32_t>(din, o_sum) + m;
+        P.tile_cnt = sec<int32_t>(din, o_cnt); P.tile_off = sec<int32_t>(din, o_off); P.fits = sec<int32_t>(din, o_fits);
+        P.o_index = sec<int32_t>(blk, L.index); P.o_creator = sec<int32_t>(blk, L.creator);
+        P.o_p0 = sec<int32_t>(blk, L.p0); P.o_p1 = sec<int32_t>(blk, L.p1); P.o_t = sec<double>(blk, L.t); P.o_sig = sec<uint8_t>(blk, L.sig);
+        P.tile0 = tile0[v]; P.ntiles = tile0[v + 1] - tile0[v];
+    }
+    cudaStream_t st = e->stream.get();
+    const size_t copy = in_bytes;
+    CK(cudaMemcpyAsync(din, hin, copy, cudaMemcpyHostToDevice, st));
+    const size_t smem = sizeof(int) * 2 * maxM;
+    int32_t *hdr = sec<int32_t>(blk, L.hdr);
+    if (batch) {
+        const SyncParams *dP = (const SyncParams *)din;
+        k_sync_count<<<dim3(maxtiles, B), SY_THREADS, smem, st>>>(dP);
+        k_sync_scan<<<1, 1024, 0, st>>>(sec<int32_t>(din, o_cnt), T, sec<int32_t>(din, o_t0), B, (int)rows,
+                                         sec<int32_t>(din, o_off), sec<int32_t>(din, o_fits), hdr);
+        k_sync_select<<<dim3(maxtiles, B), SY_THREADS, smem, st>>>(dP);
+    } else {
+        k_sync_count<<<maxtiles, SY_THREADS, smem, st>>>(Pv[0]);
+        k_sync_scan<<<1, 1024, 0, st>>>(sec<int32_t>(din, o_cnt), T, sec<int32_t>(din, o_t0), B, (int)rows,
+                                         sec<int32_t>(din, o_off), sec<int32_t>(din, o_fits), hdr);
+        k_sync_select<<<maxtiles, SY_THREADS, smem, st>>>(Pv[0]);
+    }
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    e->stats.kernel_launches += 3;
+    e->stats.h2d_bytes += (i64)copy;
+    const int total = hdr[0];
+    e->stats.d2h_bytes += (i64)sizeof(int32_t) * (2 * B + 2) + (total <= (i64)rows ? (i64)total * (4 * 5 + 8 + 64) : 0);
+    if ((size_t)total > rows || total > cap) {
+        memcpy(counts_out, hdr + 1, sizeof(int32_t) * B);
+        return fail(e, SW_E_CAPACITY, "%s: the reply holds %d events, cap is %d", what, total, cap);
+    }
+    for (int v = 0; v < B; v++)
+        if (reply_ids_ok(e, views[v], v, L, blk, hdr[1 + B + v], hdr[1 + v], O, what) < 0) return SW_E_ARG;
+    for (int v = 0; v < B; v++) reply_copy(views[v], L, blk, hdr[1 + B + v], hdr[1 + v], O);
+    memcpy(counts_out, hdr + 1, sizeof(int32_t) * B);
+    if (offsets_out) memcpy(offsets_out, hdr + 1 + B, sizeof(int32_t) * (B + 1));
+    return SW_OK;
+}
+
+// the checks of the batched calls: views, then every head and summary, before anything runs
+int sync_batch_args(sw_engine *const *engines, int B, const int *heads, const int32_t *summaries, const char *what) {
+    int rc = check_views(engines, B, what, false, false);
+    if (rc < 0) return rc;
+    sw_engine *e = engines[0];
+    for (int v = 0, m = 0; v < B; m += engines[v]->M, v++)
+        if (sync_args(e, engines[v], v, heads[v], summaries ? summaries + m : nullptr, what) < 0) return SW_E_ARG;
+    return 0;
+}
+}  // namespace
+
+int sw_sync_summary(sw_engine *e, int head, int32_t *heights_out) {
+    if (!e || !heights_out) return fail(e, SW_E_ARG, "bad argument");
+    if (e->nranks > 1) return fail(e, SW_E_UNSUPPORTED, "sw_sync_summary: one rank of a multi-GPU engine");
+    if (sync_args(e, e, 0, head, nullptr, "sw_sync_summary") < 0) return SW_E_ARG;
+    CK(cudaSetDevice(e->device));
+    sw_engine *views[1] = {e};
+    return sync_summary(e, views, 1, &head, heights_out, false);
+}
+
+int sw_batch_sync_summary(sw_engine *const *engines, int B, const int *heads, int32_t *out) {
+    sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
+    if (!e || !heads || !out) return fail(e, SW_E_ARG, "bad argument");
+    int rc = sync_batch_args(engines, B, heads, nullptr, "sw_batch_sync_summary");
+    if (rc < 0) return rc;
+    CK(cudaSetDevice(e->device));
+    return sync_summary(e, engines, B, heads, out, true);
+}
+
+int sw_sync_reply(sw_engine *e, int head, const int32_t *summary, int cap, int32_t *index_out, int32_t *count_out,
+                  uint8_t *ids, uint8_t *p0_ids, uint8_t *p1_ids, int32_t *creator, double *t, uint8_t *sig) {
+    const char *what = "sw_sync_reply";
+    if (!e || !summary || !count_out || cap < 0 || (cap > 0 && !index_out)) return fail(e, SW_E_ARG, "bad argument");
+    if (e->nranks > 1) return fail(e, SW_E_UNSUPPORTED, "%s: one rank of a multi-GPU engine", what);
+    if (sync_args(e, e, 0, head, summary, what) < 0) return SW_E_ARG;
+    CK(cudaSetDevice(e->device));
+    sw_engine *views[1] = {e};
+    int32_t cnt = 0;
+    const int rc = sync_reply(e, views, 1, &head, summary, cap, &cnt, nullptr, ReplyOut{index_out, ids, p0_ids, p1_ids, creator, t, sig}, false, what);
+    if (rc == SW_OK || rc == SW_E_CAPACITY) *count_out = cnt;
+    return rc < 0 ? rc : cnt;
+}
+
+int sw_batch_sync_reply(sw_engine *const *engines, int B, const int *heads, const int32_t *summaries, int cap,
+                        int32_t *offsets_out, int32_t *counts_out, int32_t *index_out, uint8_t *ids, uint8_t *p0_ids,
+                        uint8_t *p1_ids, int32_t *creator, double *t, uint8_t *sig) {
+    const char *what = "sw_batch_sync_reply";
+    sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
+    if (!e || !heads || !summaries || !offsets_out || !counts_out || cap < 0 || (cap > 0 && !index_out))
+        return fail(e, SW_E_ARG, "bad argument");
+    int rc = sync_batch_args(engines, B, heads, summaries, what);
+    if (rc < 0) return rc;
+    CK(cudaSetDevice(e->device));
+    std::vector<int32_t> cnt(B);
+    rc = sync_reply(e, engines, B, heads, summaries, cap, cnt.data(), offsets_out, ReplyOut{index_out, ids, p0_ids, p1_ids, creator, t, sig}, true, what);
+    if (rc == SW_OK || rc == SW_E_CAPACITY) memcpy(counts_out, cnt.data(), sizeof(int32_t) * B);
+    return rc;
+}
+
 // ---- checkpoint / resume: the engine's whole state as one binary file (sections of SoA columns)
 namespace {
 struct CkptHeader {
@@ -2527,7 +2796,12 @@ int sw_load(const char *path, int device, int capacity_events, sw_engine **out) 
     bool ok = true;
     for (const Section &s : ckpt_sections(e, H, idrec))
         ok = ok && (s.dev ? get_dev(e, f, s.p, s.bytes, tmp) : get_host(f, s.p, s.bytes));
-    for (size_t o = 0; ok && o < idrec.size(); o += 36) { Id32 k; int32_t v; memcpy(k.data(), &idrec[o], 32); memcpy(&v, &idrec[o + 32], 4); e->ids.emplace(k, v); }
+    e->id_of.assign(n, Id32{});
+    for (size_t o = 0; ok && o < idrec.size(); o += 36) {
+        Id32 k; int32_t v; memcpy(k.data(), &idrec[o], 32); memcpy(&v, &idrec[o + 32], 4);
+        e->ids.emplace(k, v);
+        if (v >= 0 && v < n) e->id_of[v] = k;
+    }
     fclose(f);
     if (!ok) { sw_destroy(e); return fail(nullptr, SW_E_ARG, "sw_load: %s is truncated or does not match its header", path); }
     // the derived columns live on the device too

@@ -29,7 +29,10 @@ SYMBOLS = [
     "sw_batch_decide_fame", "sw_batch_find_order", "sw_batch_append",
     "sw_get_consensus_times", "sw_get_rounds_received", "sw_find_order_out", "sw_batch_find_order_out",
     "sw_set_member_keys", "sw_verify_events", "sw_ingest_verified", "sw_batch_ingest_verified",
+    "sw_get_ids", "sw_sync_summary", "sw_sync_reply", "sw_batch_sync_summary", "sw_batch_sync_reply",
 ]
+
+REPLY_CAP = 4096      # the rows a sync reply is given room for per view, before the one retry at the exact count
 
 
 class SwStats(C.Structure):
@@ -101,6 +104,11 @@ def load_library(path: str = LIB_PATH):
     L.sw_batch_find_order_out.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, i32]
     L.sw_batch_append.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp]
     L.sw_batch_ingest_verified.argtypes = [vp, i32] + [vp] * 14
+    L.sw_get_ids.argtypes = [vp, i32, i32, vp]
+    L.sw_sync_summary.argtypes = [vp, i32, vp]
+    L.sw_sync_reply.argtypes = [vp, i32, vp, i32] + [vp] * 8
+    L.sw_batch_sync_summary.argtypes = [vp, i32, vp, vp]
+    L.sw_batch_sync_reply.argtypes = [vp, i32, vp, vp, i32] + [vp] * 9
     L.sw_save.argtypes = [vp, C.c_char_p]
     L.sw_load.argtypes = [C.c_char_p, i32, i32, P(vp)]
     _lib = L
@@ -252,6 +260,44 @@ class Engine:
         out = np.empty(ids.shape[0], np.int32)
         self._chk(self._lib.sw_lookup(self._h, ids.shape[0], _ptr(ids), _ptr(out)))
         return out
+
+    def ids(self, first=0, n=None):
+        """sw_get_ids: the 32-byte id of events [first, first+n) as an (n, 32) uint8 array, zeros for an event that has
+        none (it came through append, not ingest)."""
+        n = self.n_events - first if n is None else n
+        out = np.zeros((n, 32), np.uint8)
+        if n:
+            self._chk(self._lib.sw_get_ids(self._h, first, n, _ptr(out)))
+        return out
+
+    def sync_summary(self, head):
+        """sw_sync_summary: what this view sends when it asks a peer to sync (swirld.py:125-126), as M heights: of the
+        latest event of each member that `head` sees, -1 where it sees none."""
+        out = np.empty(self.M, np.int32)
+        self._chk(self._lib.sw_sync_summary(self._h, int(head), _ptr(out)))
+        return out
+
+    def sync_reply(self, head, summary, rows=True):
+        """sw_sync_reply: the events ask_sync (swirld.py:154-161) sends from `head` to a requester whose summary this is,
+        in ascending index.  Returns their indices, and with rows (index, (ids, p0_ids, p1_ids, creator, t, sig)):
+        the columns Engine.ingest takes.  rows needs every event of the reply to have come through ingest."""
+        summary = np.ascontiguousarray(summary, np.int32)
+        assert summary.shape == (self.M,)
+        cap = min(int(head) + 1, REPLY_CAP)
+        for attempt in range(2):
+            idx = np.empty(max(cap, 1), np.int32)
+            cols = _reply_columns(cap) if rows else None
+            cnt = C.c_int32(0)
+            rc = self._lib.sw_sync_reply(self._h, int(head), _ptr(summary), cap, _ptr(idx), C.byref(cnt),
+                                         *[_ptr(a) if rows else None for a in (cols or [None] * 6)])
+            if rc == -5 and attempt == 0:                  # SW_E_CAPACITY: cnt holds the exact count
+                cap = cnt.value
+                continue
+            n = self._chk(rc)
+            break
+        if not rows:
+            return idx[:n]
+        return idx[:n], tuple(a[:n] for a in cols)
 
     def append_trace(self, tr, first=0, n=None):
         n = tr.N - first if n is None else n
@@ -500,6 +546,58 @@ def batch_ingest(engines, batches):
     except ExceptionGroup as g:
         g.n_verified = nv.value
         raise
+
+
+def _reply_columns(n):
+    """Room for n rows in sw_ingest's layout: ids, p0_ids, p1_ids, creator, t, sig."""
+    n = max(n, 1)
+    return [np.empty((n, 32), np.uint8), np.empty((n, 32), np.uint8), np.empty((n, 32), np.uint8),
+            np.empty(n, np.int32), np.empty(n, np.float64), np.empty((n, 64), np.uint8)]
+
+
+def batch_sync_summary(engines, heads):
+    """sw_batch_sync_summary: Engine.sync_summary of several node-views (one device, any member counts) in one call.
+    Returns each view's summary."""
+    B = len(engines)
+    assert len(heads) == B
+    if B == 0:
+        return []
+    h = np.ascontiguousarray(heads, np.int32)
+    offs = np.cumsum([0] + [e.M for e in engines])
+    out = np.empty(max(1, int(offs[-1])), np.int32)
+    engines[0]._chk(engines[0]._lib.sw_batch_sync_summary(_handles(engines), B, _ptr(h), _ptr(out)))
+    return [out[a:b] for a, b in zip(offs[:-1], offs[1:])]
+
+
+def batch_sync_reply(engines, heads, summaries, rows=True):
+    """sw_batch_sync_reply: Engine.sync_reply of several node-views (one device, any member counts) in one call.
+    Returns each view's indices, and with rows (indices, columns): columns[v] = view v's (ids, p0_ids, p1_ids,
+    creator, t, sig), slices of one concatenation laid out as batch_ingest (sw_batch_ingest_verified) takes it."""
+    B = len(engines)
+    assert len(heads) == B and len(summaries) == B
+    if B == 0:
+        return ([], []) if rows else []
+    h = np.ascontiguousarray(heads, np.int32)
+    for e, s in zip(engines, summaries):
+        assert len(s) == e.M
+    S = np.ascontiguousarray(np.concatenate([np.asarray(s, np.int32) for s in summaries]), np.int32)
+    cap = int(min(sum(int(x) + 1 for x in heads), REPLY_CAP * B))
+    offs, cnt = np.zeros(B + 1, np.int32), np.zeros(B, np.int32)
+    for attempt in range(2):
+        idx = np.empty(max(cap, 1), np.int32)
+        cols = _reply_columns(cap) if rows else None
+        rc = engines[0]._lib.sw_batch_sync_reply(_handles(engines), B, _ptr(h), _ptr(S), cap, _ptr(offs), _ptr(cnt),
+                                                 _ptr(idx), *[_ptr(a) if rows else None for a in (cols or [None] * 6)])
+        if rc == -5 and attempt == 0:                      # SW_E_CAPACITY: cnt holds the exact counts
+            cap = int(cnt.sum())
+            continue
+        engines[0]._chk(rc)
+        break
+    ab = list(zip(offs[:-1].tolist(), offs[1:].tolist()))
+    index = [idx[a:b] for a, b in ab]
+    if not rows:
+        return index
+    return index, [tuple(c[a:b] for c in cols) for a, b in ab]
 
 
 def batch_find_order(engines, new_cs):
