@@ -36,21 +36,7 @@ class OrderMeta:
 
     def _times(self, r, X, wt, fam):
         F = np.array([w for w in wt[r] if w >= 0 and fam[w] == 1], np.int64)
-        if X.size == 0:
-            return np.empty((2, 0), np.float64)
-        C = self.creator[X]
-        A = np.repeat(F[:, None], X.size, axis=1)
-        sees = self.cs[A, C] >= X
-        cur = A.copy()
-        while True:                                  # swirld.py:298-302
-            go = sees & (self.cs[cur, C] >= X) & (self.p0[cur] >= 0)
-            if not go.any():
-                break
-            cur = np.where(go, self.p0[cur], cur)
-        s = np.sort(np.where(sees, self.t[cur], np.inf), axis=0)
-        n = sees.sum(axis=0)
-        cols = np.arange(X.size)
-        return s[n // 2, cols], s[(n + 1) // 2, cols]             # swirld.py:305 (n >= 2 for an ordered event)
+        return median_halves(self.cs, self.p0, self.creator, self.t, F, X)
 
     def find_order(self, new_c, n_divided):
         L, h = orc.lib(), self.o._h
@@ -78,6 +64,28 @@ class OrderMeta:
         if end:
             L.or_get_transactions(h, tx)
         return (tx[start:].copy(), np.array(self.ts[start:end], np.float64), np.array(self.rr[start:end], np.int32))
+
+
+def median_halves(cs, p0, creator, t, F, X):
+    """The two times whose mean is the consensus timestamp of each ordered event X of a round whose famous witnesses
+    are F: for every f in F that sees x, the time of the event where the walk down f's self-parents (swirld.py:298-302)
+    stops, and the median of those (swirld.py:305).  cs[i, c] reads can_see rows (an array, or anything indexed the
+    same way)."""
+    if X.size == 0:
+        return np.empty((2, 0), np.float64)
+    C = creator[X]
+    A = np.repeat(F[:, None], X.size, axis=1)
+    sees = cs[A, C] >= X
+    cur = A.copy()
+    while True:                                  # swirld.py:298-302
+        go = sees & (cs[cur, C] >= X) & (p0[cur] >= 0)
+        if not go.any():
+            break
+        cur = np.where(go, p0[cur], cur)
+    s = np.sort(np.where(sees, t[cur], np.inf), axis=0)
+    n = sees.sum(axis=0)
+    cols = np.arange(X.size)
+    return s[n // 2, cols], s[(n + 1) // 2, cols]             # swirld.py:305 (n >= 2 for an ordered event)
 
 
 def run_oracle_meta(tr, K, stake=None, coin_period=6, extra=False):
