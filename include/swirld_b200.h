@@ -254,6 +254,40 @@ int sw_batch_ingest_verified(sw_engine *const *engines, int B, const int *offset
                              int32_t *index_out, int32_t *count_out, int32_t *n_verified_out);
 int sw_lookup(sw_engine *e, int n, const uint8_t *ids, int32_t *index_out);   /* id -> arrival index, -1 unknown */
 
+/* ---- a node's own new events (Node.new_event, swirld.py:82-95, 139-144) on the GPU: Ed25519 signatures byte for byte
+ * as libsodium's crypto_sign_detached makes them, BLAKE2b-256 ids, and the events entered into the view.
+ * The view's signing key: sk is libsodium's 64-byte secret key (seed || pk).  Requires member keys
+ * (sw_set_member_keys), and sk[32..64) must be member `member`'s key; the device then checks that [a]B encodes to it.
+ * Otherwise SW_E_ARG, and the engine keeps the signing key it had (if any).  Only the expanded key (a, prefix) is kept,
+ * in device memory; the staging copies of sk are wiped before the call returns.  Setting a key again replaces it.
+ * sw_reset and sw_rewind keep it; sw_save never writes it (an engine from sw_load has none); sw_destroy overwrites it
+ * on the device before freeing.  Signing is constant time in the key and the nonce. */
+int sw_set_signing_key(sw_engine *e, int member, const uint8_t *sk);
+
+/* n events by the view's signing member.  msg[msg_off[i] .. msg_off[i+1]) is event i's signed message,
+ * dumps((d, p, t, pk)); pre[pre_off[i] .. pre_off[i+1]) is its preimage dumps(Event(d, p, t, pk, s)) with any 64 bytes
+ * at sig_at[i] in place of s.  Offsets are n+1 int64, monotone from 0.  sig_out gets the 64-byte signatures and ids_out
+ * the 32-byte ids, BLAKE2b-256 of the preimage with the signature in place.  With index_out NULL that is all (returns
+ * SW_OK).  Else the events are also ingested exactly as sw_ingest ingests the rows (ids_out, p0_ids, p1_ids, creator =
+ * the signing member, t, sig_out): parents by id, an unknown parent, a bad shape or a fork gives -1; returns the number
+ * appended.  PRECONDITION: msg, pre, p0_ids, p1_ids and t describe the same event; the engine does not parse pickle.
+ * SW_E_ARG before anything runs for no signing key, bad offsets or a sig_at outside [0, len - 64].  One pinned block
+ * in, one launch on the engine's stream, one copy back, one synchronisation (then the ingest's own append). */
+int sw_new_events(sw_engine *e, int n, const uint8_t *p0_ids, const uint8_t *p1_ids, const double *t,
+                  const uint8_t *msg, const int64_t *msg_off, const uint8_t *pre, const int64_t *pre_off,
+                  const int64_t *sig_at, uint8_t *sig_out, uint8_t *ids_out, int32_t *index_out);
+/* sw_new_events for B node-views in one call: rows offsets[v] .. offsets[v+1] (offsets[0] = 0) belong to view v and are
+ * signed by its key; msg_off / pre_off have offsets[B] + 1 entries over the whole concatenation and every other column
+ * is laid out like the rows.  The views share one device and may differ in M.  Every row is signed in the same launch on
+ * the first engine's stream; with index_out, the accepted rows append as sw_batch_ingest_verified's do and count_out[v]
+ * gets view v's count.  Each view's outputs and state equal those of its own single call, byte for byte.  Argument
+ * errors refuse the whole call before anything runs, as sw_batch_ingest_verified's do (a view without a signing key:
+ * SW_E_ARG).  A view's own failure (capacity: SW_E_CAPACITY) goes to count_out[v] and that view's sw_last_error. */
+int sw_batch_new_events(sw_engine *const *engines, int B, const int *offsets, const uint8_t *p0_ids,
+                        const uint8_t *p1_ids, const double *t, const uint8_t *msg, const int64_t *msg_off,
+                        const uint8_t *pre, const int64_t *pre_off, const int64_t *sig_at, uint8_t *sig_out,
+                        uint8_t *ids_out, int32_t *index_out, int32_t *count_out);
+
 /* Every event's 32-byte id from the engine's id map (sw_ingest), by arrival index, for [first, first+n) of the appended
  * events: 32 zero bytes for an event that has none (it came through sw_append).  SW_E_KEY for a range beyond them. */
 int sw_get_ids(sw_engine *e, int first, int n, uint8_t *out);

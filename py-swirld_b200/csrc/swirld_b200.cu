@@ -10,6 +10,7 @@
 #include "swirld_wide.cuh"
 #include "swirld_stream.cuh"
 #include "swirld_verify.cuh"
+#include "swirld_sign.cuh"
 #include "swirld_sync.cuh"
 
 #include <cstdlib>
@@ -265,6 +266,15 @@ struct sw_engine {
     Mem<swv::gc> d_vatab, d_vbtab;
     Pinned<uint8_t> h_vin, h_vflags;
     Mem<uint8_t> d_vin, d_vk, d_vflags;
+    // sw_set_signing_key / sw_new_events (swirld_sign.cuh): the comb table of j 256^k B, made once per engine; the
+    // expanded key a || prefix || A of member sign_member, in device memory only (d_skin and h_skin stage libsodium's
+    // secret key for one call and are wiped before it returns); a call's inputs go over through h_vin / d_vin, and its
+    // signatures and ids come back through h_sout.
+    bool have_sign = false, have_comb = false;
+    int sign_member = -1;
+    Mem<swv::gc> d_comb;
+    Mem<uint8_t> d_sk, d_skin, d_sout;
+    Pinned<uint8_t> h_skin, h_sout;
     sw_stats_t stats{};
     std::string err;
     size_t stage_bytes() const { return d_stage.cap() / STAGE_SLOTS; }
@@ -1667,7 +1677,7 @@ int append_views(sw_engine *const *engines, int B, const int *offsets, const int
 
 extern "C" {
 
-int sw_version(void) { return 207; }
+int sw_version(void) { return 208; }
 
 const char *sw_last_error(const sw_engine *e) { return e ? e->err.c_str() : g_create_error.c_str(); }
 
@@ -1683,6 +1693,10 @@ void sw_destroy(sw_engine *e) {
     wait_appends(e, -1);
     sync_streams(e);
     fold_spans(e);
+    if (e->d_sk.get()) {            // the signing key does not outlive the engine in freed device memory
+        cudaMemsetAsync(e->d_sk.get(), 0, e->d_sk.cap(), e->stream.get());
+        cudaStreamSynchronize(e->stream.get());
+    }
     delete e;
 }
 
@@ -2242,6 +2256,10 @@ int ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const
     ingest_commit(e, n, ids, P, index_out);
     return m;
 }
+
+int ingest_views(sw_engine *const *engines, int B, const int *offsets, const uint8_t *ids, const uint8_t *p0_ids,
+                 const uint8_t *p1_ids, const int32_t *creator, const double *t, const uint8_t *sig, const uint8_t *ok,
+                 int32_t *index_out, int32_t *count_out);
 }  // namespace
 
 int sw_ingest(sw_engine *e, int n, const uint8_t *ids, const uint8_t *p0_ids, const uint8_t *p1_ids,
@@ -2370,16 +2388,25 @@ int sw_batch_ingest_verified(sw_engine *const *engines, int B, const int *offset
     rc = verify_run(e, (int)rep.size(), rep.data(), vset.data(), engines, B, creator, sig, msg, msg_off, pre, pre_off, ids, flags.data());
     if (rc < 0) return rc;
     if (n_verified_out) *n_verified_out = (int32_t)rep.size();
+    std::vector<uint8_t> ok(N, 1);
+    for (int r = 0; r < N; r++) if (distinct[r] >= 0) ok[r] = flags[distinct[r]] == 3;
+    return ingest_views(engines, B, offsets, ids, p0_ids, p1_ids, creator, t, sig, ok.data(), index_out, count_out);
+}
+
+namespace {
+// The ingest of B node-views after their verdicts (sw_batch_ingest_verified, sw_batch_new_events): view v ingests rows
+// offsets[v] .. offsets[v+1] as its sw_ingest_verified would with verdicts ok[row] (null: all accepted).
+int ingest_views(sw_engine *const *engines, int B, const int *offsets, const uint8_t *ids, const uint8_t *p0_ids,
+                 const uint8_t *p1_ids, const int32_t *creator, const double *t, const uint8_t *sig, const uint8_t *ok,
+                 int32_t *index_out, int32_t *count_out) {
+    sw_engine *e = engines[0];
     // 3. every view's plan with its verdicts; a view that fails keeps its state and its error, and appends nothing
     std::vector<IngestPlan> plans(B);
     std::vector<int> aoff(B + 1, 0);
-    std::vector<uint8_t> ok;
     for (int v = 0; v < B; v++) {
         const int o = offsets[v], n = offsets[v + 1] - o;
-        ok.assign(n, 1);
-        for (int i = 0; i < n; i++) if (distinct[o + i] >= 0) ok[i] = flags[distinct[o + i]] == 3;
         count_out[v] = ingest_plan(engines[v], n, ids + (size_t)32 * o, p0_ids + (size_t)32 * o, p1_ids + (size_t)32 * o,
-                                   creator + o, t + o, sig + (size_t)64 * o, ok.data(), index_out + o, plans[v]);
+                                   creator + o, t + o, sig + (size_t)64 * o, ok ? ok + o : nullptr, index_out + o, plans[v]);
         if (count_out[v] < 0) plans[v] = IngestPlan();
         aoff[v + 1] = aoff[v] + plans[v].size();
     }
@@ -2409,6 +2436,169 @@ int sw_batch_ingest_verified(sw_engine *const *engines, int B, const int *offset
         count_out[v] = plans[v].size();
     }
     return first_err;
+}
+
+// Zeros over n bytes of host memory that the compiler may not drop
+void wipe(void *p, size_t n) {
+    volatile uint8_t *q = static_cast<volatile uint8_t *>(p);
+    for (size_t i = 0; i < n; i++) q[i] = 0;
+}
+
+// Calls of at most this many events sign with 8 lanes per event (k_sign_events<8>), larger ones with one (DESIGN §5)
+constexpr int SIGN_SPLIT_N = 4096;
+
+// sw_new_events' refusals, before anything runs: offsets (n + 1 of them, from 0, monotone) and sig_at in [0, len - 64]
+int sign_args(sw_engine *e, const char *what, int n, const uint8_t *msg, const int64_t *msg_off, const uint8_t *pre,
+              const int64_t *pre_off, const int64_t *sig_at) {
+    for (const int64_t *off : {msg_off, pre_off}) {
+        if (off[0] != 0) return fail(e, SW_E_ARG, "%s: offsets must start at 0", what);
+        for (int i = 0; i < n; i++)
+            if (off[i + 1] < off[i]) return fail(e, SW_E_ARG, "%s: offsets are not monotone at %d", what, i);
+    }
+    for (int i = 0; i < n; i++)
+        if (sig_at[i] < 0 || sig_at[i] > pre_off[i + 1] - pre_off[i] - 64)
+            return fail(e, SW_E_ARG, "%s: sig_at %lld of event %d is outside its preimage", what, (long long)sig_at[i], i);
+    if ((!msg && msg_off[n] > 0) || (!pre && pre_off[n] > 0)) return fail(e, SW_E_ARG, "%s: bad argument", what);
+    return 0;
+}
+
+// Sign events 0..n and hash their preimages: the inputs go over in one pinned block, k_sign_events runs on the compute
+// stream of e, the signatures and ids come back in one copy, one synchronisation.  Event j is signed by the key of
+// views[set[j]] (set null: of e); the table is e's.
+int sign_run(sw_engine *e, int n, const int *set, sw_engine *const *views, int nviews, const uint8_t *msg,
+             const int64_t *msg_off, const uint8_t *pre, const int64_t *pre_off, const int64_t *sig_at, uint8_t *sig_out,
+             uint8_t *ids_out) {
+    if (n == 0) return SW_OK;
+    const size_t nkeys = set ? (size_t)nviews : 1, mbytes = (size_t)msg_off[n], pbytes = (size_t)pre_off[n];
+    // the block: set | keys | msg_off | pre_off | sig_at | msg | pre, each section 256-byte aligned
+    const size_t o_keys = align256(set ? sizeof(int32_t) * n : 0), o_moff = o_keys + align256(sizeof(void *) * nkeys);
+    const size_t o_poff = o_moff + align256(sizeof(int64_t) * (n + 1)), o_at = o_poff + align256(sizeof(int64_t) * (n + 1));
+    const size_t o_msg = o_at + align256(sizeof(int64_t) * n), o_pre = o_msg + align256(mbytes), bytes = o_pre + pbytes;
+    const size_t want = std::max(bytes, 2 * e->d_vin.cap());
+    if (grow(e, bytes, e->d_vin.cap(), sized(e->d_vin, want), sized(e->h_vin, want)) < 0) return SW_E_CUDA;
+    const size_t wn = std::max((size_t)96 * n, 2 * e->d_sout.cap());
+    if (grow(e, (size_t)96 * n, e->d_sout.cap(), sized(e->d_sout, wn), sized(e->h_sout, wn)) < 0) return SW_E_CUDA;
+    uint8_t *h = e->h_vin.get(), *d = e->d_vin.get();
+    if (set) memcpy(h, set, sizeof(int32_t) * n);
+    const uint8_t **keys = reinterpret_cast<const uint8_t **>(h + o_keys);
+    for (size_t v = 0; v < nkeys; v++) keys[v] = (set ? views[v] : e)->d_sk.get();
+    memcpy(h + o_moff, msg_off, sizeof(int64_t) * (n + 1));
+    memcpy(h + o_poff, pre_off, sizeof(int64_t) * (n + 1));
+    memcpy(h + o_at, sig_at, sizeof(int64_t) * n);
+    if (mbytes) memcpy(h + o_msg, msg, mbytes);
+    if (pbytes) memcpy(h + o_pre, pre, pbytes);
+    cudaStream_t st = e->stream.get();
+    CK(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st));
+    const int32_t *dset = set ? reinterpret_cast<const int32_t *>(d) : nullptr;
+    const uint8_t *const *dkeys = reinterpret_cast<const uint8_t *const *>(d + o_keys);
+    const int64_t *dmo = reinterpret_cast<const int64_t *>(d + o_moff), *dpo = reinterpret_cast<const int64_t *>(d + o_poff);
+    const int64_t *dat = reinterpret_cast<const int64_t *>(d + o_at);
+    uint8_t *dsig = e->d_sout.get(), *dids = dsig + (size_t)64 * n;
+    if (n <= SIGN_SPLIT_N)
+        k_sign_events<8><<<(n + 15) / 16, 128, 0, st>>>(n, dset, dkeys, e->d_comb.get(), d + o_msg, dmo, d + o_pre, dpo, dat, dsig, dids);
+    else
+        k_sign_events<1><<<(int)std::min<long>((n + 127) / 128, 16L * e->n_sm), 128, 0, st>>>(n, dset, dkeys, e->d_comb.get(), d + o_msg,
+                                                                                               dmo, d + o_pre, dpo, dat, dsig, dids);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(e->h_sout.get(), dsig, (size_t)96 * n, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    memcpy(sig_out, e->h_sout.get(), (size_t)64 * n);
+    memcpy(ids_out, e->h_sout.get() + (size_t)64 * n, (size_t)32 * n);
+    e->stats.kernel_launches += 1;
+    e->stats.h2d_bytes += (i64)bytes;
+    e->stats.d2h_bytes += (i64)96 * n;
+    return SW_OK;
+}
+}  // namespace
+
+int sw_set_signing_key(sw_engine *e, int member, const uint8_t *sk) {
+    const char *what = "sw_set_signing_key";
+    if (!e || !sk) return fail(e, SW_E_ARG, "bad argument");
+    if (!e->have_keys) return fail(e, SW_E_ARG, "%s: no member keys (sw_set_member_keys)", what);
+    if (member < 0 || member >= e->M) return fail(e, SW_E_ARG, "%s: member %d out of range", what, member);
+    if (memcmp(sk + 32, e->h_vkeys.data() + (size_t)32 * member, 32))
+        return fail(e, SW_E_ARG, "%s: sk[32..64) is not member %d's key", what, member);
+    CK(cudaSetDevice(e->device));
+    cudaStream_t st = e->stream.get();
+    if (grow(e, 1, e->d_sk.get() ? 1 : 0, sized(e->d_sk, sws::SK_BYTES)) < 0 ||
+        grow(e, 1, e->d_skin.get() ? 1 : 0, sized(e->d_skin, 65), sized(e->h_skin, 65)) < 0)
+        return SW_E_CUDA;
+    if (!e->have_comb) {            // j 256^k B, from the base point's encoding, once per engine
+        if (grow(e, 1, 0, sized(e->d_comb, sws::ROWS * sws::COLS)) < 0) return SW_E_CUDA;
+        k_sign_table<<<1, 32, 0, st>>>(e->d_comb.get());
+        CK(cudaGetLastError());
+        e->stats.kernel_launches += 1;
+        e->have_comb = true;
+    }
+    uint8_t *h = e->h_skin.get();
+    memcpy(h, sk, 64);
+    cudaError_t s = cudaMemcpyAsync(e->d_skin.get(), h, 64, cudaMemcpyHostToDevice, st);
+    if (s == cudaSuccess) {
+        k_sign_key<<<1, 32, 0, st>>>(e->d_skin.get(), e->d_comb.get(), e->d_sk.get(), e->d_skin.get() + 64);
+        s = cudaGetLastError();
+    }
+    if (s == cudaSuccess) s = cudaMemcpyAsync(h + 64, e->d_skin.get() + 64, 1, cudaMemcpyDeviceToHost, st);
+    const cudaError_t w = cudaMemsetAsync(e->d_skin.get(), 0, 64, st);
+    if (s == cudaSuccess) s = w;
+    if (s == cudaSuccess) s = cudaStreamSynchronize(st);
+    wipe(h, 64);
+    if (s != cudaSuccess) return fail(e, SW_E_CUDA, "%s: %s", what, cudaGetErrorString(s));
+    e->stats.kernel_launches += 1;
+    e->stats.h2d_bytes += 64;
+    e->stats.d2h_bytes += 1;
+    if (!h[64]) return fail(e, SW_E_ARG, "%s: [a]B of the seed does not encode to member %d's key", what, member);
+    e->have_sign = true;
+    e->sign_member = member;
+    return SW_OK;
+}
+
+int sw_new_events(sw_engine *e, int n, const uint8_t *p0_ids, const uint8_t *p1_ids, const double *t,
+                  const uint8_t *msg, const int64_t *msg_off, const uint8_t *pre, const int64_t *pre_off,
+                  const int64_t *sig_at, uint8_t *sig_out, uint8_t *ids_out, int32_t *index_out) {
+    const char *what = "sw_new_events";
+    if (!e || n < 0 || (n > 0 && (!msg_off || !pre_off || !sig_at || !sig_out || !ids_out)) ||
+        (n > 0 && index_out && (!p0_ids || !p1_ids || !t)))
+        return fail(e, SW_E_ARG, "bad argument");
+    if (!e->have_sign) return fail(e, SW_E_ARG, "%s: no signing key (sw_set_signing_key)", what);
+    if (n == 0) return SW_OK;
+    int rc = sign_args(e, what, n, msg, msg_off, pre, pre_off, sig_at);
+    if (rc < 0) return rc;
+    CK(cudaSetDevice(e->device));
+    rc = sign_run(e, n, nullptr, nullptr, 0, msg, msg_off, pre, pre_off, sig_at, sig_out, ids_out);
+    if (rc < 0 || !index_out) return rc;
+    const std::vector<int32_t> creator(n, e->sign_member);
+    return ingest(e, n, ids_out, p0_ids, p1_ids, creator.data(), t, sig_out, nullptr, index_out);
+}
+
+int sw_batch_new_events(sw_engine *const *engines, int B, const int *offsets, const uint8_t *p0_ids,
+                        const uint8_t *p1_ids, const double *t, const uint8_t *msg, const int64_t *msg_off,
+                        const uint8_t *pre, const int64_t *pre_off, const int64_t *sig_at, uint8_t *sig_out,
+                        uint8_t *ids_out, int32_t *index_out, int32_t *count_out) {
+    const char *what = "sw_batch_new_events";
+    sw_engine *e = (engines && B > 0) ? engines[0] : nullptr;
+    if (!e || !offsets || !msg_off || !pre_off || (index_out && !count_out)) return fail(e, SW_E_ARG, "bad argument");
+    int rc = check_views(engines, B, what, false, index_out != nullptr);
+    if (rc < 0) return rc;
+    for (int v = 0; v < B; v++)
+        if (!engines[v]->have_sign) return fail(e, SW_E_ARG, "%s: view %d has no signing key (sw_set_signing_key)", what, v);
+    if (offsets[0] != 0) return fail(e, SW_E_ARG, "%s: offsets[0] = %d", what, offsets[0]);
+    for (int v = 0; v < B; v++)
+        if (offsets[v + 1] < offsets[v])
+            return fail(e, SW_E_ARG, "%s: offsets[%d] = %d > offsets[%d] = %d", what, v, offsets[v], v + 1, offsets[v + 1]);
+    const int N = offsets[B];
+    if (N > 0 && (!sig_at || !sig_out || !ids_out || (index_out && (!p0_ids || !p1_ids || !t))))
+        return fail(e, SW_E_ARG, "bad argument");
+    rc = sign_args(e, what, N, msg, msg_off, pre, pre_off, sig_at);
+    if (rc < 0) return rc;
+    CK(cudaSetDevice(e->device));
+    std::vector<int> set(N);
+    std::vector<int32_t> creator(N);
+    for (int v = 0; v < B; v++)
+        for (int r = offsets[v]; r < offsets[v + 1]; r++) { set[r] = v; creator[r] = engines[v]->sign_member; }
+    rc = sign_run(e, N, set.data(), engines, B, msg, msg_off, pre, pre_off, sig_at, sig_out, ids_out);
+    if (rc < 0) return rc;
+    if (!index_out) return SW_OK;
+    return ingest_views(engines, B, offsets, ids_out, p0_ids, p1_ids, creator.data(), t, sig_out, nullptr, index_out, count_out);
 }
 
 int sw_lookup(sw_engine *e, int n, const uint8_t *ids, int32_t *index_out) {

@@ -30,6 +30,7 @@ SYMBOLS = [
     "sw_get_consensus_times", "sw_get_rounds_received", "sw_find_order_out", "sw_batch_find_order_out",
     "sw_set_member_keys", "sw_verify_events", "sw_ingest_verified", "sw_batch_ingest_verified",
     "sw_get_ids", "sw_sync_summary", "sw_sync_reply", "sw_batch_sync_summary", "sw_batch_sync_reply",
+    "sw_set_signing_key", "sw_new_events", "sw_batch_new_events",
 ]
 
 REPLY_CAP = 4096      # the rows a sync reply is given room for per view, before the one retry at the exact count
@@ -109,6 +110,9 @@ def load_library(path: str = LIB_PATH):
     L.sw_sync_reply.argtypes = [vp, i32, vp, i32] + [vp] * 8
     L.sw_batch_sync_summary.argtypes = [vp, i32, vp, vp]
     L.sw_batch_sync_reply.argtypes = [vp, i32, vp, vp, i32] + [vp] * 9
+    L.sw_set_signing_key.argtypes = [vp, i32, vp]
+    L.sw_new_events.argtypes = [vp, i32] + [vp] * 11
+    L.sw_batch_new_events.argtypes = [vp, i32] + [vp] * 13
     L.sw_save.argtypes = [vp, C.c_char_p]
     L.sw_load.argtypes = [C.c_char_p, i32, i32, P(vp)]
     _lib = L
@@ -254,6 +258,36 @@ class Engine:
         self._chk(self._lib.sw_verify_events(self._h, n, _ptr(creator), _ptr(sig), _ptr(msg), _ptr(moff), _ptr(pre),
                                              _ptr(poff), _ptr(ids), _ptr(out)))
         return out[:n]
+
+    def set_signing_key(self, member, sk):
+        """sw_set_signing_key: this view signs its new events as `member` with libsodium's 64-byte secret key (seed ||
+        pk); pk must be member's key in set_member_keys.  Only the expanded key is kept, in device memory."""
+        sk = bytes(sk)
+        assert len(sk) == 64, "libsodium's secret key is 64 bytes"
+        buf = C.create_string_buffer(sk, 64)
+        try:
+            self._chk(self._lib.sw_set_signing_key(self._h, int(member), C.cast(buf, C.c_void_p)))
+        finally:
+            C.memset(buf, 0, 64)
+
+    def new_events(self, templates, p0_ids=None, p1_ids=None, t=None, ingest=True):
+        """sw_new_events: sign and hash events of this view's signing member.  templates[i] = (msg, pre, sig_at) as
+        events.event_template makes them.  Returns (sig, ids) as (n, 64) and (n, 32) uint8 arrays; with ingest (p0_ids,
+        p1_ids and t given) also enters the events as Engine.ingest would: (sig, ids, index_out, appended)."""
+        n = len(templates)
+        msg, moff, pre, poff, at = _templates(templates)
+        sig, ids = np.zeros((max(n, 1), 64), np.uint8), np.zeros((max(n, 1), 32), np.uint8)
+        if not ingest:
+            self._chk(self._lib.sw_new_events(self._h, n, None, None, None, _ptr(msg), _ptr(moff), _ptr(pre), _ptr(poff),
+                                              _ptr(at), _ptr(sig), _ptr(ids), None))
+            return sig[:n], ids[:n]
+        p0 = np.ascontiguousarray(p0_ids, np.uint8).reshape(n, 32)
+        p1 = np.ascontiguousarray(p1_ids, np.uint8).reshape(n, 32)
+        t = np.ascontiguousarray(t, np.float64).reshape(n)
+        out = np.empty(max(n, 1), np.int32)
+        m = self._chk(self._lib.sw_new_events(self._h, n, _ptr(p0), _ptr(p1), _ptr(t), _ptr(msg), _ptr(moff), _ptr(pre),
+                                              _ptr(poff), _ptr(at), _ptr(sig), _ptr(ids), _ptr(out)))
+        return sig[:n], ids[:n], out[:n], m
 
     def lookup(self, ids):
         ids = np.ascontiguousarray(ids, np.uint8).reshape(-1, 32)
@@ -546,6 +580,47 @@ def batch_ingest(engines, batches):
     except ExceptionGroup as g:
         g.n_verified = nv.value
         raise
+
+
+def _templates(templates):
+    """(msg, msg_off, pre, pre_off, sig_at) of (msg, pre, sig_at) triples, as sw_new_events takes them."""
+    (msg, moff), (pre, poff) = _packed([m for m, _, _ in templates]), _packed([p for _, p, _ in templates])
+    at = np.ascontiguousarray([a for _, _, a in templates] or [0], np.int64)
+    return msg, moff, pre, poff, at
+
+
+def batch_new_events(engines, templates, p0_ids=None, p1_ids=None, t=None, ingest=True):
+    """sw_batch_new_events: Engine.new_events of several node-views (one device) in one call, every event signed in one
+    launch.  templates[v] lists view v's (msg, pre, sig_at); with ingest, p0_ids[v], p1_ids[v] and t[v] are its columns.
+    Returns [(sig, ids)] per view, or with ingest [(sig, ids, index_out, appended)].  Argument errors raise at once; a
+    view's own failure raises as an ExceptionGroup after every other view has ingested (see _per_view)."""
+    B = len(engines)
+    assert len(templates) == B
+    if B == 0:
+        return []
+    ns = [len(x) for x in templates]
+    offs = np.zeros(B + 1, np.int32)
+    offs[1:] = np.cumsum(ns)
+    N = int(offs[-1])
+    msg, moff, pre, poff, at = _templates([x for view in templates for x in view])
+    sig, ids = np.zeros((max(N, 1), 64), np.uint8), np.zeros((max(N, 1), 32), np.uint8)
+    ab = list(zip(offs[:-1].tolist(), offs[1:].tolist()))
+    L = engines[0]._lib
+    if not ingest:
+        engines[0]._chk(L.sw_batch_new_events(_handles(engines), B, _ptr(offs), None, None, None, _ptr(msg), _ptr(moff),
+                                              _ptr(pre), _ptr(poff), _ptr(at), _ptr(sig), _ptr(ids), None, None))
+        return [(sig[a:b], ids[a:b]) for a, b in ab]
+    cat = lambda cols, shape, dt: np.ascontiguousarray(
+        np.concatenate([np.asarray(c, dt).reshape((n,) + shape) for c, n in zip(cols, ns)]) if N else np.zeros((1,) + shape, dt))
+    p0, p1, tt = cat(p0_ids, (32,), np.uint8), cat(p1_ids, (32,), np.uint8), cat(t, (), np.float64)
+    out = np.empty(max(N, 1), np.int32)
+    cnt = np.zeros(B, np.int32)
+    rc = L.sw_batch_new_events(_handles(engines), B, _ptr(offs), _ptr(p0), _ptr(p1), _ptr(tt), _ptr(msg), _ptr(moff),
+                               _ptr(pre), _ptr(poff), _ptr(at), _ptr(sig), _ptr(ids), _ptr(out), _ptr(cnt))
+    if rc < 0 and not (cnt < 0).any():
+        engines[0]._chk(rc)                # refused as a whole: nothing ran, count_out was not written
+    res = [(sig[a:b], ids[a:b], out[a:b].copy(), int(m)) for (a, b), m in zip(ab, cnt)]
+    return _per_view("batch_new_events", engines, res, cnt)
 
 
 def _reply_columns(n):
