@@ -196,6 +196,11 @@ int sw_event_elapsed_ms(sw_engine *e, int slot_a, int slot_b, double *ms_out);
 
 /* Profiling aid: 16 cycle counters of the round kernels (tools/rounds_cycles.py). */
 int sw_debug_counters(sw_engine *e, int64_t *out16, int clear);
+/* Profiling aid: the cluster round kernel's per-CTA step log, kept only when the engine was created with the
+ * environment variable SW_RC_STEPS = the number of steps to keep (tools/rc_steps.py; the record layout is in
+ * swirld_rcluster.cuh).  Copies at most cap_words words (a 16-word header, then 16 words per step and CTA) and
+ * returns the steps logged since the last clear (more than were kept if the log overflowed), 0 without a log. */
+int sw_rc_step_log(sw_engine *e, uint32_t *out, int64_t cap_words, int clear);
 
 /* ---- ingest: the step of Node.sync between the wire and divide_rounds (swirld.py:129-136, utils.py:8-21) in C++.
  * A batch of n events named by their 32-byte ids (BLAKE2b, swirld.py:95), parents given by id (32 zero bytes = none: a

@@ -181,6 +181,7 @@ struct sw_engine {
     // cluster round kernel (swirld_rcluster.cuh): seq-space rows of the current chunk, 64 ints per event (the round
     // stream's pieces use both buffers in turn, the compute stream the first), hand-over state
     Mem<int32_t> d_rsg[2], d_rccont;
+    Mem<unsigned> d_rcslog;       // the cluster kernel's per-CTA step log (SW_RC_STEPS; empty otherwise)
     bool rc_ok = false;           // a 16-CTA cluster with its shared memory can be resident on this device
     int rc_min_n = 2048;          // shorter chunks go to the grid-wide kernel directly
     RoundStream rs;
@@ -719,7 +720,7 @@ RbParams round_params(const sw_engine *e, const RoundTarget &T, int first, int n
 // The chunk goes to the cluster round kernel first: its parameters, with the seq-space rows of the target; the
 // cooperative kernel's R then continues from where the cluster stopped
 RcParams cluster_first(const sw_engine *e, const RoundTarget &T, RbParams &R) {
-    const RcParams Q{R, T.rsg, e->d_rccont.get()};
+    const RcParams Q{R, T.rsg, e->d_rccont.get(), e->d_rcslog.get()};
     R.cont = e->d_rccont.get();
     return Q;
 }
@@ -778,7 +779,8 @@ void rc_launch_config(cudaLaunchConfig_t &cfg, cudaLaunchAttribute *at, int clus
 template <int NC, bool UNIT>
 cudaError_t rc_setup(int *clusters) {
     cudaError_t er = cudaSuccess;
-    for (const void *fn : {(const void *)k_rounds_cluster<UNIT, RcParams>, (const void *)k_rounds_cluster<UNIT, const RcParams *>}) {
+    for (const void *fn : {(const void *)k_rounds_cluster<UNIT, RcParams>, (const void *)k_rounds_cluster<UNIT, const RcParams *>,
+                           (const void *)k_rounds_cluster_log<UNIT>}) {
         if (er == cudaSuccess) er = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RC_SMEM_BYTES);
         if (er == cudaSuccess) er = cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     }
@@ -798,7 +800,10 @@ int round_kernels(sw_engine *e, RSrc R, QSrc Q, int nv, int G, bool rc, cudaStre
         cudaLaunchConfig_t cfg;
         cudaLaunchAttribute at[1];
         rc_launch_config(cfg, at, nv, st);
-        CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster<UNIT, QSrc>, Q));
+        if constexpr (std::is_same<QSrc, RcParams>::value) {
+            if (Q.slog) CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster_log<UNIT>, Q));    // (SW_RC_STEPS)
+            else CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster<UNIT, QSrc>, Q));
+        } else CK(cudaLaunchKernelEx(&cfg, k_rounds_cluster<UNIT, QSrc>, Q));
     }
     void *args[] = {(void *)&R};
     CK(cudaLaunchCooperativeKernel((void *)k_rounds_batch<NC, UNIT, RSrc>, dim3(G, nv), dim3(RB_THREADS), args, 0, st));
@@ -1290,6 +1295,13 @@ int create(int M, int capacity_events, const int64_t *stake, int coin_period, in
             bool want = true;
             if (const char *v = getenv("SW_ROUNDS_CLUSTER")) want = atoi(v) != 0;
             if (const char *v = getenv("SW_RC_MIN_N")) e->rc_min_n = std::max(1, atoi(v));
+            if (const char *v = getenv("SW_RC_STEPS")) {         // profiling: log this many cluster steps per CTA
+                const unsigned cap = (unsigned)std::max(0, atoi(v));
+                const size_t words = RC_LOGH + (size_t)cap * RC_CS * RC_NLOG;
+                CK(e->d_rcslog.alloc(words)); CK(cudaMemsetAsync(e->d_rcslog.get(), 0, sizeof(unsigned) * words, e->stream.get()));
+                CK(cudaMemcpyAsync(e->d_rcslog.get() + 1, &cap, sizeof(unsigned), cudaMemcpyHostToDevice, e->stream.get()));
+                CK(cudaStreamSynchronize(e->stream.get()));
+            }
             if (want) {
                 int ncl = 0;
                 const cudaError_t er = SW_NCU(e, rc_setup, &ncl);
@@ -1522,6 +1534,7 @@ int chunk_views(sw_engine *e, sw_engine *const *engines, int B, const int *first
             if (rows_ready(x, first[v], n[v]) < 0) return SW_E_CUDA;
             // a view's window stays a round deep (16 pending events per chain) however few warps it has: they loop
             if (round_batch_prep(x, first[v], n[v], G, 16, use_rc, Rv[v], Qv[v]) < 0) { e->err = x->err; return SW_E_CUDA; }
+            Qv[v].slog = nullptr;                               // (the step log is for one cluster at a time)
             if (follow(x, x->stream.get(), e->stream.get()) < 0) { e->err = x->err; return SW_E_CUDA; }
         }
         CK(cudaMemcpyAsync(e->d_views.get() + v0, Rv.data() + v0, sizeof(RbParams) * nv, cudaMemcpyHostToDevice, e->stream.get()));
@@ -2131,6 +2144,20 @@ int sw_debug_counters(sw_engine *e, int64_t *out16, int clear) {
     CK(cudaMemcpy(out16, e->d_dbg.get(), sizeof(long long) * 16, cudaMemcpyDeviceToHost));
     if (clear) CK(cudaMemset(e->d_dbg.get(), 0, sizeof(long long) * 40));
     return SW_OK;
+}
+
+int sw_rc_step_log(sw_engine *e, uint32_t *out, int64_t cap_words, int clear) {
+    if (!e || cap_words < 0 || (cap_words > 0 && !out)) return SW_E_ARG;
+    if (!e->d_rcslog.get()) return 0;
+    CK(cudaSetDevice(e->device));
+    CK(cudaStreamSynchronize(e->stream.get()));
+    if (e->rs.on) CK(cudaStreamSynchronize(e->rs.stream.get()));
+    unsigned head[2];
+    CK(cudaMemcpy(head, e->d_rcslog.get(), sizeof(head), cudaMemcpyDeviceToHost));
+    const size_t words = std::min<size_t>((size_t)cap_words, RC_LOGH + (size_t)std::min(head[0], head[1]) * RC_CS * RC_NLOG);
+    if (words) CK(cudaMemcpy(out, e->d_rcslog.get(), sizeof(unsigned) * words, cudaMemcpyDeviceToHost));
+    if (clear) CK(cudaMemset(e->d_rcslog.get(), 0, sizeof(unsigned)));
+    return (int)head[0];
 }
 
 int sw_flush_l2(sw_engine *e, int64_t bytes) {

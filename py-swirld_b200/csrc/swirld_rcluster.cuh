@@ -11,7 +11,8 @@
 //     ("row(k)[c_] >= Wf_r[c_]") holds in seq space as it does in index space -- a member's events are ordered the
 //     same way in both -- and a mask S_r(k) is addressed by (member, position) without any lookup.
 //   * CTA q owns chains 4q..4q+3: a window of RC_WN consecutive rows per chain (and their event indices) in its
-//     shared memory, filled one step ahead by cp.async.  The state of chain c (position, round, window bounds) lives
+//     shared memory, filled one step ahead by bulk copies (one or two per chain and step, counted on an mbarrier;
+//     the rows' event indices by cp.async).  The state of chain c (position, round, window bounds) lives
 //     in the registers of thread c of EVERY CTA: all 16 CTAs do the same bookkeeping from the same results, so no
 //     decision ever has to be communicated.
 //   * a step (round r = lowest open round):
@@ -54,6 +55,31 @@ struct RcParams {
     RbParams R;
     const int32_t *rsg;      // [n][64] seq-space rows of the chunk's events in cev order (k_rb_prep)
     int32_t *cont;           // [0,64) positions, [64,128) rounds, [128] 1 = k_rounds_batch has work left
+    unsigned *slog;          // per-CTA step log (profiling, k_rounds_cluster_log), NULL unless the engine was created with SW_RC_STEPS
+};
+
+// The step log: a header of RC_LOGH words ([0] steps logged by the launches so far, [1] capacity in steps), then one
+// record of RC_NLOG words per (step, CTA), in cycles of that CTA's thread 0.  Clocks of different SMs are not
+// comparable, but every CTA starts a step when the same result words arrive and tests when the same masks arrive, so
+// RL_SENDER (results in -> own masks pushed) and RL_TESTER (masks in -> own results sent) can be compared across the
+// CTAs of one step: the largest of each is the CTA the others wait for.  tools/rc_steps.py reads it.
+#define RC_LOGH 16
+#define RC_NLOG 16
+enum {
+    RL_WAIT,    // wait for the last step's results
+    RL_CTL,     // bookkeeping (warp 0) and the wait for the rows issued a step ago
+    RL_BAR1,    // block barrier after the bookkeeping
+    RL_MASK,    // masks of my members into my table
+    RL_BAR2,    // block barrier before the push
+    RL_PUSH,    // my members' masks to the 15 other tables
+    RL_TEST1,   // test phase 1 (my rows only)
+    RL_MWAIT,   // wait for the other CTAs' masks
+    RL_TEST2,   // test phase 2 (the masks)
+    RL_BAR3,    // block barrier after the tests
+    RL_SEND,    // results of my chains to every CTA
+    RL_DEFER,   // final rounds of the last step, the copies of the next rows
+    RL_SENDER,  // results in -> masks pushed
+    RL_TESTER,  // masks in -> results sent
 };
 
 #define RC_SMEM_ROWS ((size_t)RC_CPC * RC_WN * 64 * 4)
@@ -71,8 +97,11 @@ __device__ __forceinline__ unsigned rc_map(const void *p, unsigned rank) {
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
     return r;
 }
-__device__ __forceinline__ void rc_cp16(void *dst, const void *src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+// one bulk copy (the TMA unit) of `bytes` (a multiple of 16, both addresses 16-byte aligned) from global memory into my
+// shared memory, counted on the mbarrier `mbar` of my CTA
+__device__ __forceinline__ void rc_bulk(void *dst, const void *src, unsigned bytes, unsigned mbar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 :: "r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src), "r"(bytes), "r"(mbar) : "memory");
 }
 
 __device__ __forceinline__ void rc_cp4(void *dst, const void *src) {
@@ -122,7 +151,7 @@ __device__ __forceinline__ void rc_sta_u32(unsigned addr, unsigned v, unsigned m
     asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" :: "r"(addr), "r"(v), "r"(mbar) : "memory");
 }
 
-template <bool UNIT>
+template <bool UNIT, bool LOG>
 __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
     const RbParams &P = Q.R;
     extern __shared__ __align__(16) unsigned char rc_smem[];
@@ -142,6 +171,7 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
     int *vres = iv + 1152 + RC_CPC * RC_WN;                                                      // [RC_CPC][RC_LW] test results
     int2 (*cst)[64] = reinterpret_cast<int2 (*)[64]>(iv + 1792);                                 // [chain][member] {threshold, span}
     const unsigned mbar0 = (unsigned)__cvta_generic_to_shared(iv + 2304);                        // mbarriers: masks (2 tables), results
+    unsigned *tsm = reinterpret_cast<unsigned *>(iv + 2320);     // step log, thread 0: [0, 15) clocks, [16] first record, [17] capacity
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int M = P.M;
@@ -183,6 +213,7 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
 
     if (tid == 0) {
         rc_mbar_init(mbar0, 1); rc_mbar_init(mbar0 + 8, 1); rc_mbar_init(mbar0 + 16, 1);
+        rc_mbar_init(mbar0 + 24, RC_CPC);                       // the window rows of my chains: one arrival per chain and step
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     int handed = 0;
@@ -241,17 +272,27 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
 
     long long c_t[6] = {0, 0, 0, 0, 0, 0}, c_steps = 0, c_tests = 0, c_unk = 0;
     int stall = 0, rmin = 0;
-    bool have_res = false;
+    bool have_res = false, rows_out = false;                    // rows_out: the bulk copies of this step are issued
+    // the step log (LOG only: a kernel of its own, so the marks cost the timed kernel nothing): where this launch's
+    // records begin (every CTA reads it before the first exchange; CTA 0 advances it after its loop), and thread 0's
+    // clock at each mark of a step
+    const bool lg = LOG && tid == 0;
+    if (lg) { tsm[16] = __ldcg(Q.slog); tsm[17] = __ldcg(Q.slog + 1); }
+    auto mark = [&](int k) { if constexpr (LOG) { if (tid == 0) tsm[k] = (unsigned)clock64(); } };
     unsigned it = 0;                                            // steps so far (mbarrier phases)
     for (; !handed; ++it) {
         const long long t0 = clock64();
+        mark(0);
         u64 (*maskbuf)[RC_MRS] = maskbuf0 + (it & 1) * 64;
         // ---- the results of the last step (every CTA holds all of them): positions, rounds, the mirror of Wf; then
         //      this step's ranges and windows.  One warp, no block-wide barrier inside.
         bool late = false;
         if (have_res) late = !rc_mbar_wait(mbar0 + 16, (it - 1) & 1);
+        mark(1);
         if (tid == 0) rc_mbar_expect(mbar0 + 16, 64 * 4);      // this step's results: one word per chain
-        asm volatile("cp.async.wait_all;" ::: "memory");        // (the rows issued a step ago)
+        if (rows_out) late |= !rc_mbar_wait(mbar0 + 24, (it - 1) & 1);   // the rows issued a step ago ...
+        rows_out = false;
+        asm volatile("cp.async.wait_all;" ::: "memory");        // ... and their event indices
         if (warp == 0) {
             bool hit[2] = {false, false}, prog = false;
             int hitseq[2] = {-1, -1};
@@ -318,6 +359,7 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
             }
             if (lane == 0) { ws[0] = rnext; ws[1] = status; }
         }
+        mark(2);
         const bool timed_out = __syncthreads_or(late);          // (never, unless a peer CTA died)
         const int rprev = rmin, status = ws[1];
         rmin = ws[0];
@@ -331,6 +373,7 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
             break;
         }
         const long long t1 = clock64();
+        mark(3);
         // ---- a: the masks of my members' ranges into my own table (4 warps per member), then each member's masks to
         //         every other CTA as one wide store per (member, CTA).  Bit b of a mask's low word is column 2b, of its
         //         high word column 2b+1: the tests only COUNT columns.
@@ -353,11 +396,13 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
                     }
                 }
             }
+            mark(4);
             if (tid < RC_CPC * 64) {                            // {threshold (+1 on the chain's own column: its self-parent), span}
                 const int cl2 = tid >> 6, m = tid & 63;
                 cst[cl2][m] = make_int2(wp[m] + (m == bx * RC_CPC + cl2 ? 1 : 0), cnts[m]);
             }
             __syncthreads();
+            mark(5);
             for (int pair = warp; pair < RC_CPC * RC_CS; pair += RC_THREADS / 32) {
                 const int cl2 = pair & (RC_CPC - 1), r = pair / RC_CPC, c2 = bx * RC_CPC + cl2;
                 if (r == bx || 2 * lane >= cnts[c2]) continue;
@@ -366,20 +411,34 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
             }
         }
         const long long t2 = clock64();
+        mark(6);
         // off the path the other CTAs wait on: the final rounds of the last step, the next rows of my chains' windows
+        mark(13);
         if (have_res && tid < RC_CPC * RC_LW) {
             const int cl = tid / RC_LW, j = tid % RC_LW, c = bx * RC_CPC + cl;
             if (j < s_nfin[c]) P.round[cevw[cl][(s_base[c] + j) & (RC_WN - 1)]] = rprev;
         }
-#pragma unroll
-        for (int cl = 0; cl < RC_CPC; cl++) {
-            const int c = bx * RC_CPC + cl, lo2 = s_old[c], nrow = wldp[c] - lo2;
-            if (nrow <= 0) continue;
-            const int32_t *src = Q.rsg + (size_t)(coff_s[c] + lo2 - cmin_s[c]) * 64;
-            for (int i = tid; i < nrow * 16; i += RC_THREADS) rc_cp16(&rsw[cl][(lo2 + (i >> 4)) & (RC_WN - 1)][(i & 15) * 4], src + i * 4);
-            if (tid < nrow) rc_cp4(&cevw[cl][(lo2 + tid) & (RC_WN - 1)], P.cev + off[c] + lo2 - cmin_s[c] + tid);
+        // the rows of chain cl by lane 0 of warp 5 cl (one warp per SM sub-partition), as one or two bulk copies (the
+        // window is a ring) that count their bytes on the rows' mbarrier; its event indices by the same warp.  Rows that
+        // a later row of the same step overwrites in the ring are never read: only the last RC_WN are copied.
+        if (warp % 5 == 0 && warp < 5 * RC_CPC) {
+            const int cl = warp / 5, c = bx * RC_CPC + cl, n = wldp[c] - s_old[c];
+            const int nrow = max(0, min(n, RC_WN)), lo2 = s_old[c] + max(0, n - RC_WN);
+            const size_t g = (size_t)(coff_s[c] + lo2 - cmin_s[c]);
+            if (lane == 0) {
+                rc_mbar_expect(mbar0 + 24, (unsigned)nrow * 256u);
+                if (nrow > 0) {
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // (after the generic reads of the slots)
+                    const int s0 = lo2 & (RC_WN - 1), n0 = min(nrow, RC_WN - s0);
+                    rc_bulk(rsw[cl][s0], Q.rsg + g * 64, (unsigned)n0 * 256u, mbar0 + 24);
+                    if (nrow > n0) rc_bulk(rsw[cl][0], Q.rsg + (g + n0) * 64, (unsigned)(nrow - n0) * 256u, mbar0 + 24);
+                }
+            }
+            for (int i = lane; i < nrow; i += 32) rc_cp4(&cevw[cl][(lo2 + i) & (RC_WN - 1)], P.cev + off[c] + (lo2 - cmin_s[c]) + i);
         }
+        rows_out = true;
         asm volatile("cp.async.commit_group;" ::: "memory");
+        mark(14);
         long long t3;
         // ---- b: first pending event with P_r (1) or beyond the masks (2), per chain
         if (UNIT) {
@@ -414,8 +473,10 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
             unk = ((ub >> (lane & ~3)) & 0xfu) != 0;
             const bool need = act && lv > thr_i && !unk;       // (lv <= thr: hits[c_] <= the live members)
             int v = (act && lv > thr_i && unk) ? 2 : 0;
+            mark(7);
             late = !rc_mbar_wait(mbar0 + 8 * (it & 1), (it >> 1) & 1);
             t3 = clock64();
+            mark(8);
             if (__any_sync(0xffffffffu, need)) {
                 c_tests++;
                 u64 x[16];
@@ -447,11 +508,13 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
             if (v == 2) c_unk++;
             if (pp == 0) vres[cl * RC_LW + t] = v;
             const int w2 = warp < RC_CPC ? swin[bx * RC_CPC + warp] : -1;   // (read before the barrier: warp 0 rewrites swin right after it)
+            mark(9);
             if (__syncthreads_or(late)) {
                 if (tid == 0 && lead) atomicMin(&P.scal[SC_ERR], -4);
                 handed = 1;
                 break;
             }
+            mark(10);
             if (warp < RC_CPC) {
                 const int c2 = bx * RC_CPC + warp;
                 const int x = vres[warp * RC_LW + lane];
@@ -465,13 +528,16 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
                 }
             }
         } else {
+            mark(7);
             late = !rc_mbar_wait(mbar0 + 8 * (it & 1), (it >> 1) & 1);
+            mark(8); mark(9);
             if (__syncthreads_or(late)) {
                 if (tid == 0 && lead) atomicMin(&P.scal[SC_ERR], -4);
                 handed = 1;
                 break;
             }
             t3 = clock64();
+            mark(10);
             // integer stakes: a 5-ary search with the chain's 4 warps, one test of swirld_rounds.cuh's kind per warp and pass
             if (tid < RC_CPC) { sa[tid] = -1; sb[tid] = max(swin[bx * RC_CPC + tid], 0); svb[tid] = 0; }
             __syncthreads();
@@ -552,11 +618,22 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
             }
         }
         const long long t4 = clock64();
+        mark(11);
         const long long t5 = clock64();
         have_res = true;
         c_t[0] += t1 - t0; c_t[1] += t2 - t1; c_t[2] += t3 - t2; c_t[3] += t4 - t3; c_t[4] += t5 - t4;
         c_steps++;
+        if constexpr (LOG) if (lg && tsm[16] + it < tsm[17]) {
+            unsigned *o = Q.slog + RC_LOGH + ((size_t)(tsm[16] + it) * RC_CS + bx) * RC_NLOG;
+            const unsigned dfr = tsm[14] - tsm[13];
+            o[RL_WAIT] = tsm[1] - tsm[0]; o[RL_CTL] = tsm[2] - tsm[1]; o[RL_BAR1] = tsm[3] - tsm[2];
+            o[RL_MASK] = tsm[4] - tsm[3]; o[RL_BAR2] = tsm[5] - tsm[4]; o[RL_PUSH] = tsm[6] - tsm[5];
+            o[RL_TEST1] = tsm[7] - tsm[6] - dfr; o[RL_MWAIT] = tsm[8] - tsm[7]; o[RL_TEST2] = tsm[9] - tsm[8];
+            o[RL_BAR3] = tsm[10] - tsm[9]; o[RL_SEND] = tsm[11] - tsm[10]; o[RL_DEFER] = dfr;
+            o[RL_SENDER] = tsm[6] - tsm[1]; o[RL_TESTER] = tsm[11] - tsm[8];
+        }
     }
+    if (rows_out) (void)rc_mbar_wait(mbar0 + 24, it & 1);    // (the loop was left inside the tests)
     asm volatile("cp.async.wait_all;" ::: "memory");
     __syncthreads();
     if (lead) {
@@ -580,11 +657,16 @@ __device__ __forceinline__ void rounds_cluster_body(const RcParams &Q) {
         atomicAdd(&o[7], 1ull);                                 // launches, and how many handed work back
         atomicAdd(&o[15], (unsigned long long)handed);
     }
+    if constexpr (LOG) if (lg && lead) Q.slog[0] = tsm[16] + (unsigned)c_steps;     // (the next launch's records follow this one's)
     rc_cluster_sync();                                          // nobody leaves while its shared memory may still be written
 }
 
 // several independent node-views (swirld_rounds.cuh, k_rounds_batch): one cluster per view (blockIdx.y), as many side
 // by side as the device holds -- the clusters never talk to each other, so this is an ordinary (non-cooperative) launch
 template <bool UNIT, class Src>
-__global__ void __launch_bounds__(RC_THREADS, 1) k_rounds_cluster(Src s) { rounds_cluster_body<UNIT>(params(s)); }
+__global__ void __launch_bounds__(RC_THREADS, 1) k_rounds_cluster(Src s) { rounds_cluster_body<UNIT, false>(params(s)); }
+// the same with the per-CTA step log (RcParams::slog), for one view: launched instead of k_rounds_cluster<UNIT, RcParams>
+// when the engine keeps the log
+template <bool UNIT>
+__global__ void __launch_bounds__(RC_THREADS, 1) k_rounds_cluster_log(RcParams q) { rounds_cluster_body<UNIT, true>(q); }
 SW_SRC_INSTANCES_OF(k_rounds_cluster, RcParams, false) SW_SRC_INSTANCES_OF(k_rounds_cluster, RcParams, true)

@@ -24,7 +24,7 @@ SYMBOLS = [
     "sw_decide_fame", "sw_find_order", "sw_n_events", "sw_n_divided", "sw_max_round",
     "sw_n_transactions", "sw_get_round", "sw_get_witness_flags", "sw_get_famous", "sw_get_can_see",
     "sw_get_witness_table", "sw_get_consensus", "sw_get_transactions", "sw_get_idx", "sw_get_height",
-    "sw_sync", "sw_stats", "sw_flush_l2", "sw_version", "sw_debug_counters", "sw_peer_handle", "sw_peer_connect",
+    "sw_sync", "sw_stats", "sw_flush_l2", "sw_version", "sw_debug_counters", "sw_rc_step_log", "sw_peer_handle", "sw_peer_connect",
     "sw_save", "sw_load", "sw_members", "sw_ingest", "sw_lookup", "sw_batch_divide_rounds",
     "sw_batch_decide_fame", "sw_batch_find_order", "sw_batch_append",
     "sw_get_consensus_times", "sw_get_rounds_received", "sw_find_order_out", "sw_batch_find_order_out",
@@ -90,6 +90,7 @@ def load_library(path: str = LIB_PATH):
     L.sw_flush_l2.argtypes = [vp, i64]
     L.sw_version.argtypes = []
     L.sw_debug_counters.argtypes = [vp, vp, i32]
+    L.sw_rc_step_log.argtypes = [vp, vp, i64, i32]
     L.sw_peer_handle.argtypes = [vp, vp]
     L.sw_peer_connect.argtypes = [vp, i32, i32, vp]
     L.sw_members.argtypes = [vp]
@@ -444,6 +445,15 @@ class Engine:
         out = np.zeros(16, np.int64)
         self._chk(self._lib.sw_debug_counters(self._h, _ptr(out), 1 if clear else 0))
         return out
+
+    def rc_step_log(self, clear=True):
+        """The cluster round kernel's step log (engine created with SW_RC_STEPS set): [steps, 16 CTAs, 16] uint32 in
+        cycles, fields in swirld_rcluster.cuh's RL_* order."""
+        n = self._chk(self._lib.sw_rc_step_log(self._h, None, 0, 0))
+        out = np.zeros(16 + n * 16 * 16, np.uint32)
+        self._chk(self._lib.sw_rc_step_log(self._h, _ptr(out), out.size, 1 if clear else 0))
+        kept = min(n, int(out[1]))
+        return out[16:16 + kept * 256].reshape(kept, 16, 16)
 
     # -- several GPUs of one box, M > 64 (include/swirld_b200.h: sw_peer_handle / sw_peer_connect)
     def peer_handle(self) -> bytes:
